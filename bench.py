@@ -2,6 +2,7 @@
 """Headline benchmark: images/sec end-to-end (letterbox -> NMS), yolov5s, batch 32, 640x640, fp16.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config c2|c3|c4|c5] [--scaling weak|strong]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
 
 `--config` selects one of BASELINE.json's configs (default c2 = configs[1], the headline):
@@ -18,6 +19,11 @@ Prints ONE JSON line (rank 0).  `value` = whole-job images/s with the uint8 inpu
 metric through the public API (`model.predict`) from pinned HOST tensors with the H2D copies and the D2H of the
 results inside the timed region.  `roofline` is the tensor-core roofline of the convolution launches (live CUDA
 events around the plan); `cpu_baseline` is the CPU oracle port of the reference path on this box's host cores.
+
+`--dump-outputs DIR` writes what the timed path returned in its last timed step (rank 0): the padded detections
+boxes [n, D, 4], scores [n, D], labels [n, D] (slots past an image's count zeroed) and the per-image counts [n], as
+float32 .npy files.  Inputs and weights
+are seeded, so two builds run with the same arguments can be compared output for output.
 
 `--impl reference` times the reference algorithm's CPU port (oracle/restate.py: the reference's own PyTorch CPU
 operators in fp32) with every host thread, on a bounded sample of the same workload per step.
@@ -129,8 +135,8 @@ def zoo_state_dict(model, gain: float, seed: int = 1, head_scale: float = 10.0):
 
 class NvmlClockSampler:
     """SM clock / throttle reasons from NVML, polled by a thread while the timed region runs.  In-process (no
-    nvidia-smi start-up inside the timed region: spawning it there showed up as multi-millisecond hiccups in
-    individual steps, mean 2.27 ms vs median 1.96 ms)."""
+    nvidia-smi start-up inside the timed region: spawning it there shows up as multi-millisecond hiccups in
+    individual steps)."""
 
     def __init__(self, index: int):
         import pynvml
@@ -234,20 +240,12 @@ class ClockSampler:
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx, "reasons": sorted(reasons), "samples": len(sm)}
 
 
-def conv_traffic():
-    """DRAM bytes of all convolution launches of one step, from the committed ncu capture (profiles/), or None."""
-    p = os.path.join(ROOT, "profiles", "r01_conv_traffic.json")
-    try:
-        with open(p) as f:
-            return float(json.load(f)["dram_bytes_per_step"])
-    except Exception:
-        return None
-
-
 def measured_peaks(sm_mhz=None, sm_max_mhz=None):
-    """(tensor TFLOP/s, HBM GB/s, source).  MEASURED_PEAKS.json holds a burst figure (a kernel timed alone, clocks at
-    maximum) and a sustained one (seconds-long loop under the 1 kW cap, ~1.4 GHz): the burst figure is the honest
-    denominator when this run's SM clock sat at (>= 95 % of) its maximum, the sustained one otherwise."""
+    """(tensor TFLOP/s, HBM GB/s, source).  MEASURED_PEAKS.json, when present, holds a burst figure (a kernel timed
+    alone, clocks at maximum) and a sustained one (seconds-long loop under the card's power cap): the burst figure is
+    the honest denominator when this run's SM clock sat at (>= 95 % of) its maximum, the sustained one otherwise.
+    Without it the denominators are NVIDIA's H100 SXM data-sheet figures (dense FP16 989 TFLOP/s, HBM3 3.35 TB/s, at
+    up to 700 W), which a power-limited card does not reach."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     burst = sm_mhz is not None and sm_max_mhz and sm_mhz >= 0.95 * sm_max_mhz
     if os.path.exists(p):
@@ -255,7 +253,7 @@ def measured_peaks(sm_mhz=None, sm_max_mhz=None):
             d = json.load(f)
         key = "bf16_tflops" if burst else "bf16_tflops_sustained"
         return float(d[key]), float(d["hbm_gbs"]), f"measured (MEASURED_PEAKS.json {key}, hbm_gbs)"
-    return (1590.0 if burst else 1400.0), 6650.0, "fallback (B200_PROFILING.md)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense FP16, HBM3)"
 
 
 def cpu_port_images_per_s(sd, steps: int, warmup: int, ims=None, size=(640, 640), thr=SCORE_THRESH):
@@ -342,6 +340,8 @@ def main():
     ap.add_argument("--score-thresh", type=float, default=None, help="override the post-process score threshold")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true", help="device-resident leg only (profiling runs)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's detections (boxes, scores, labels, counts) to DIR as float32 .npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -377,7 +377,7 @@ def main():
     if cfg["dtype"] == "bf16":
         model = model.to(torch.bfloat16)
 
-    # inputs: NBUF distinct batches, more than the 126 MB L2 in total, so no step finds its input in L2
+    # inputs: NBUF distinct batches, more than the 50 MB L2 in total, so no step finds its input in L2
     mixed = bool(cfg.get("mixed"))
     per_batch_bytes = n_local * 3 * size * size
     NBUF = 24 if mixed else max(2, min(4, -(-160_000_000 // per_batch_bytes)))
@@ -457,6 +457,18 @@ def main():
     ms_per_step = total_ms / args.steps
     value = world * n_local * args.steps / (total_ms / 1e3)
     boxes, scores, labels, counts, status = out
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        # slots past an image's count are never written by the NMS kernel: zero them so that the files depend only on
+        # the detections
+        valid = torch.arange(boxes.shape[1], device=boxes.device)[None, :] < counts.view(-1, 1)
+        for name, t in (("boxes", boxes), ("scores", scores), ("labels", labels)):
+            t = t.detach().float()
+            t = torch.where(valid.view(*valid.shape, *([1] * (t.dim() - 2))), t, torch.zeros((), device=t.device))
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), t.cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "counts.npy"), counts.detach().float().cpu().numpy())
     st = status.cpu().tolist()
     cand_per_img = st[0] / n_local
     det_per_img = float(counts.float().mean().item())
@@ -603,12 +615,12 @@ def main():
                        "score_thresh": thr, "nms_thresh": 0.45, "detections_per_img": D,
                        "candidates_per_image": cand_per_img, "detections_per_image": det_per_img,
                        "distinct_canvases": n_canvases,
-                       "l2": f"{NBUF} rotating input batches of {h2d_bytes / 1e6:.1f} MB (> 126 MB L2 in total); the activations of a step evict everything",
+                       "l2": f"{NBUF} rotating input batches of {h2d_bytes / 1e6:.1f} MB (> 50 MB L2 in total); the activations of a step evict everything",
                        "parallelism": f"dp{world}" + (" + one nccl all_gather of the packed detections per step (side stream)" if world > 1 else "")},
             "gpu_launches": (n_ops + 1 + 3) * args.steps,
             "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                         "traffic": conv_traffic() if args.config == "c2" else None, "peak_source": peak_src,
-                         "kernel": "conv_umma_kernel + conv3x3_patch_kernel (all conv launches of one step)",
+                         "peak_source": peak_src,
+                         "kernel": "conv_wgmma_kernel + conv3x3_patch_kernel (all conv launches of one step)",
                          "plan_ms": plan_ms, "launches_per_step": n_ops, "arena_bytes": plan_i.arena_bytes},
             "roofline_stages": {"hbm_peak_gbs": hbm, "timing": "CUDA events around each stage, median over steps (separate loop)",
                                 "letterbox": stage("letterbox", lb_bytes), "plan": stage("plan", 0),

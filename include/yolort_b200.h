@@ -1,5 +1,5 @@
 /*
- * yolort_b200 -- C ABI of the B200-native YOLOv5 inference path.
+ * yolort_b200 -- C ABI of the H100-native (sm_90a) YOLOv5 inference path.
  *
  * The reference (zhiqwang/yolort) has no FFI on this path: its boundary is the Python nn.Module
  * surface (yolort/models/yolov5.py:135 YOLOv5.forward, yolort/models/yolo.py:141 YOLO.forward).
@@ -157,10 +157,7 @@ typedef struct {
                                    super-pixel stem matrix [Cout_pad][3][128] (engine.stem_band); bit 2: take the
                                    halo-patch kernel's stride-2 parity-plane variant whatever the channel counts (tests);
                                    bit 3: do not split N over CTAs with resident weights (A/B timing, tests);
-                                   bit 4: four TMEM accumulator stages instead of two where they fit (measured equal or slower on
-                                   B200: 1.315 vs 1.312 ms per yolov5s plan; opt-in for A/B timing);
-                                   bit 5: four epilogue groups (608 threads) where that kernel variant applies (measured slower
-                                   than two on B200; opt-in for A/B timing and tests) */
+                                   other bits: must be zero */
   const yb_head_decode* decode; /* optional (host pointer, copied at plan creation): fused decode epilogue */
   const yb_conv_chain* chain;   /* optional (host pointer, copied at plan creation): chained pointwise tail  */
 } yb_op_desc;

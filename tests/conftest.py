@@ -12,18 +12,18 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box: pytest -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs an sm_90 (H100) CUDA device (pytest -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
-    """`gpu` tests need an sm_100 device: without one they are skipped (not failed), so a plain `pytest tests` works
+    """`gpu` tests need an sm_90 device: without one they are skipped (not failed), so a plain `pytest tests` works
     on a machine without a CUDA driver.  The product path itself still fails loudly without a GPU (test_host_logic)."""
     import torch
 
-    ok = torch.cuda.is_available() and torch.cuda.get_device_capability(0)[0] == 10
+    ok = torch.cuda.is_available() and torch.cuda.get_device_capability(0) == (9, 0)
     if ok:
         return
-    skip = pytest.mark.skip(reason="needs an sm_100 (B200) CUDA device")
+    skip = pytest.mark.skip(reason="needs an sm_90 (H100) CUDA device")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

@@ -1,4 +1,4 @@
-"""Parity at the REAL shapes of BASELINE.json's configs (B200), at north_star's tolerance.
+"""Parity at the REAL shapes of BASELINE.json's configs (H100), at north_star's tolerance.
 
 * stage-wise: every launch of the plan at the benchmark's own shape against a plain fp32 PyTorch op on the launch's
   own fp16/bf16 input (tests/stagewise.py): |err| <= 2^-9 (fp16) / 2^-6 (bf16) x (1 + |ref|), zero violations;
@@ -82,7 +82,6 @@ def test_c2_yolov5s_bs32_640_fp16_detections_vs_oracle():
     ims = bench.make_images(32, 1234)
     out = m([im.to(DEV) for im in ims])
     ref = R.detect(sd, ims[:8], score_thresh=bench.SCORE_THRESH)
-    # measured on B200 (round 2): matched 0.9967 (worst image 0.99), every matched box within 2.0e-4 x 640, |dscore| <= 2.0e-3
     util.assert_e2e_parity("c2 yolov5s bs32 640 fp16", out[:8], ref, 640.0, min_matched=0.99, min_within=0.999,
                            max_box_rel=1e-3, max_score_err=5e-3)
 

@@ -1,4 +1,4 @@
-"""tcgen05 implicit-GEMM convolution vs a plain fp32 PyTorch conv on the same fp16/bf16-rounded operands (B200)."""
+"""wgmma implicit-GEMM convolution vs a plain fp32 PyTorch conv on the same fp16/bf16-rounded operands (H100)."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -11,7 +11,7 @@ DEV = torch.device("cuda:0")
 
 
 def run_conv(N, H, W, Cin, Cout, k, s, p, dtype=torch.float16, act=True, residual=False, in_pad=0, out_pad=0, seed=0,
-             bias_scale=0.5, force_im2col=False, force_planes=False, wide=False):
+             bias_scale=0.5, force_im2col=False, force_planes=False):
     torch.backends.cudnn.allow_tf32 = False      # the fp32 reference must not run on TF32 tensor cores
     torch.backends.cuda.matmul.allow_tf32 = False
     g = torch.Generator().manual_seed(seed)
@@ -38,9 +38,7 @@ def run_conv(N, H, W, Cin, Cout, k, s, p, dtype=torch.float16, act=True, residua
     d.weight, d.Cin_pad, d.Cout_pad, d.bias = wp.data_ptr(), ci_pad, co_pad, bp.data_ptr()
     if residual:
         d.residual, d.res_cstride = res.data_ptr(), Cout
-    d.reserved = (1 if force_im2col else 0) | (4 if force_planes else 0) | (32 if wide else 0)
-    if wide:
-        assert _C.conv_config(d)["epilogue_groups"] == 4
+    d.reserved = (1 if force_im2col else 0) | (4 if force_planes else 0)
     plan = _C.Plan([d], DEV)
     plan.run()
     torch.cuda.synchronize()
@@ -115,24 +113,13 @@ def test_large_m_many_tiles():
 
 
 def test_silu_strongly_negative_preactivations():
-    """Pre-activations below -8: h + h tanh(h) evaluated with the fp16 tanh approximation cancels there (error up to
-    |v| 2^-12 on a result of a few 1e-3); the kernels switch such batches to v / (1 + e^-v) in fp32
-    (conv_epilogue.cuh: epilogue_batch_exact).  Large biases put ~10 % of the outputs in that range."""
+    """Pre-activations below -8, where SiLU is a few 1e-3 and an approximation through tanh in fp16 would cancel: the
+    epilogue evaluates v / (1 + e^-v) in fp32 and must stay within the stage-wise bound there.  Large biases put ~10 %
+    of the outputs in that range."""
     run_conv(2, 20, 20, 64, 64, 1, 1, 0, bias_scale=6.0, seed=21)
     run_conv(2, 24, 24, 64, 64, 3, 1, 1, bias_scale=6.0, seed=22, residual=True)
     run_conv(2, 20, 20, 64, 128, 1, 1, 0, bias_scale=6.0, seed=23, dtype=torch.bfloat16)
     run_conv(2, 24, 40, 32, 64, 3, 2, 1, bias_scale=6.0, seed=24)
-
-
-def test_conv1x1_wide_epilogue_variant():
-    """The opt-in four-group kernel variant (reserved bit 5: 608 threads, one accumulator stage per epilogue group) for
-    layers with at least four 128-row tiles per CTA, 64-column store boxes and an N tile <= 128: shapes past 592 tiles,
-    with / without a shortcut, fp16 / bf16, output into a channel window, ragged last tile."""
-    run_conv(8, 100, 100, 64, 64, 1, 1, 0, seed=31, wide=True)                          # 625 tiles, packed-half2 tail
-    run_conv(8, 100, 100, 128, 128, 1, 1, 0, seed=32, out_pad=64, wide=True)            # two boxes per tile
-    run_conv(9, 96, 97, 64, 64, 1, 1, 0, seed=33, residual=True, wide=True)             # fp32 tail, ragged M (83 808 pixels)
-    run_conv(8, 100, 100, 64, 128, 1, 1, 0, seed=34, dtype=torch.bfloat16, wide=True)
-    run_conv(8, 100, 100, 64, 64, 1, 1, 0, seed=35, bias_scale=6.0, wide=True)          # exact-SiLU slow path in the wide variant
 
 
 def test_rejects_unsupported():
@@ -142,7 +129,7 @@ def test_rejects_unsupported():
         _C.Plan([d], DEV)
 
 
-# ---- halo-patch 3x3 kernel (conv3x3_patch_sm100.cu) -------------------------------------------------------
+# ---- halo-patch 3x3 kernel (conv3x3_patch_sm90.cu)  -------------------------------------------------------
 @pytest.mark.parametrize("cin,cout", [(64, 64), (16, 32), (32, 32), (128, 128), (256, 256), (48, 48), (80, 80), (96, 192)])
 def test_patch_conv_channel_widths(cin, cout):
     """Halo-patch kernel over the channel widths of the zoo, incl. widths that do not fill a 64-channel chunk

@@ -1,4 +1,4 @@
-"""Plan infrastructure on the device (B200): shared weights across shapes, arena liveness reuse, LRU, invalidation when
+"""Plan infrastructure on the device (H100): shared weights across shapes, arena liveness reuse, LRU, invalidation when
 weights change, non-current devices, callable sub-modules / forward hooks, training-mode head outputs."""
 import time
 

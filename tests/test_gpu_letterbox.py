@@ -1,4 +1,4 @@
-"""Letterbox kernel vs the reference fixtures / oracle (B200)."""
+"""Letterbox kernel vs the reference fixtures / oracle (H100)."""
 import numpy as np
 import pytest
 import torch

@@ -1,5 +1,5 @@
 """LogitsDecoder / dense decode (SURVEY.md section 8f row 3) vs the oracle's restatement of
-box_head.py:328-360 (B200)."""
+box_head.py:328-360 (H100)."""
 import numpy as np
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""Whole-graph parity: backbone+PAN+head on the native plan vs reference fixtures / oracle, and end to end (B200)."""
+"""Whole-graph parity: backbone+PAN+head on the native plan vs reference fixtures / oracle, and end to end (H100)."""
 import numpy as np
 import pytest
 import torch

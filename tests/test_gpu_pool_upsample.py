@@ -1,4 +1,4 @@
-"""SPP max-pool cascade and nearest 2x upsample kernels vs PyTorch reference ops (B200)."""
+"""SPP max-pool cascade and nearest 2x upsample kernels vs PyTorch reference ops (H100)."""
 import pytest
 import torch
 import torch.nn.functional as F

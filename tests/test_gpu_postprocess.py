@@ -1,4 +1,4 @@
-"""decode + threshold + batched NMS kernels vs reference fixtures and the C/numpy oracle (B200)."""
+"""decode + threshold + batched NMS kernels vs reference fixtures and the C/numpy oracle (H100)."""
 import numpy as np
 import pytest
 import torch

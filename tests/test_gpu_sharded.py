@@ -1,5 +1,5 @@
 """predict_sharded on real devices (NCCL, one process per GPU) == the single-GPU forward on the same mixed-size batch.
-Needs two B200s: run with `gpurun --gpus 2 -- python -m pytest tests/test_gpu_sharded.py -m gpu`."""
+Needs two H100s: python -m pytest tests/test_gpu_sharded.py -m gpu; skipped on a single-GPU machine."""
 import os
 import socket
 

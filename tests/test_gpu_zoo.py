@@ -1,5 +1,5 @@
 """The other model sizes of BASELINE.json's configs (m / l / x: channel widths 48..1280, deeper C3 stacks, bf16,
-mixed input sizes, 1280-pixel canvas) against the CPU oracle (B200)."""
+mixed input sizes, 1280-pixel canvas) against the CPU oracle (H100)."""
 import numpy as np
 import pytest
 import torch

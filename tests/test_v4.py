@@ -99,7 +99,7 @@ def test_lowering_v4_topology(ver, n_ops):
     assert acts == want
 
 
-# ---- B200 ---------------------------------------------------------------------------------------------
+# ---- GPU ----------------------------------------------------------------------------------------------
 def _model(tag, ver):
     m = yolov5s(upstream_version=ver, size=(128, 128), score_thresh=0.15).eval()
     m.load_state_dict(_sd(tag))

@@ -11,7 +11,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# YB_LIB_PATH: A/B timing of alternative builds of the same ABI (scripts/ab_step.sh); never set in product use
+# YB_LIB_PATH: A/B timing of alternative builds of the same ABI (scripts/ab_step.py); never set in product use
 LIB_PATH = os.environ.get("YB_LIB_PATH") or os.path.join(_HERE, "libyolort_b200.so")
 
 YB_U8, YB_F16, YB_BF16, YB_F32 = 0, 1, 2, 3
@@ -148,7 +148,7 @@ def lib() -> ctypes.CDLL:
         return _lib
     if not os.path.exists(LIB_PATH):
         raise NativeLibraryError(
-            f"{LIB_PATH} is missing. Build it with `python __graft_entry__.py` (nvcc, sm_100a). "
+            f"{LIB_PATH} is missing. Build it with `python __graft_entry__.py` (nvcc, sm_90a). "
             "yolort_b200 has no PyTorch/CPU fallback path."
         )
     L = ctypes.CDLL(LIB_PATH)
@@ -243,7 +243,7 @@ def device_guard(device: torch.device):
 def require_cuda(t: torch.Tensor, what: str) -> None:
     if not t.is_cuda:
         raise NativeLibraryError(
-            f"{what}: tensor lives on {t.device}; the yolort_b200 path runs on sm_100a only (no CPU fallback)")
+            f"{what}: tensor lives on {t.device}; the yolort_b200 path runs on sm_90a only (no CPU fallback)")
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -345,7 +345,7 @@ def conv_config(op: "OpDesc") -> dict:
     keys = ("patch_kernel", "block_n", "n_tiles", "weights_resident", "tiles_per_pass", "slots", "ring", "store_cols",
             "store_bufs", "smem_bytes", "grid", "chained")
     cfg = dict(zip(keys, [int(v) for v in info]))
-    if not cfg["patch_kernel"]:     # slot 8 of the 1x1 / im2col kernel: epilogue groups (two staging buffers each)
+    if not cfg["patch_kernel"]:     # slot 8 of the 1x1 / im2col kernel: consumer warpgroups (sharing two staging buffers)
         cfg["epilogue_groups"] = cfg.pop("store_bufs")
     return cfg
 

@@ -4,7 +4,7 @@
 #include <vector>
 
 #include "common.cuh"
-#include "conv_sm100.h"
+#include "conv_sm90.h"
 
 namespace yb {
 namespace {

@@ -1,9 +1,9 @@
 // Chained pointwise tail (yb_conv_chain): parameters shared by the two convolution kernels and the host-side set-up.
 //
 // After the first convolution's epilogue has written its output boxes into the swizzled staging buffers (the layout a
-// TMA store reads AND the K-major layout a UMMA operand descriptor expresses), the MMA warp multiplies those boxes with
-// the resident tail weights into a tail accumulator of the same epilogue group; a second epilogue pass stores the
-// tail's output.  Reference chains: yolort/v5/models/common.py:94-116 (Bottleneck cv1 after the previous conv),
+// TMA store reads AND the K-major layout a wgmma operand descriptor expresses), the two consumer warpgroups multiply
+// those boxes with the resident tail weights into their (now drained) accumulator registers; a second epilogue pass
+// stores the tail's output.  Reference chains: yolort/v5/models/common.py:94-116 (Bottleneck cv1 after the previous conv),
 // :149-173 (C3: cv1||cv2 -> m.0.cv1, m.last.cv2 -> cv3 over the concat).
 #pragma once
 #include "conv_epilogue.cuh"
@@ -12,7 +12,7 @@ namespace yb {
 
 struct ChainParams {
   int on;
-  int n2;                 // accumulator columns of the tail GEMM (Cout_pad of the tail, multiple of 16, <= 256)
+  int n2;                 // accumulator columns of the tail GEMM (Cout_pad of the tail rounded up to a power of two)
   int own_chunks;         // own output boxes that feed the tail (1 or 2); box b sits in staging buffer b of the group
   int own_row_bytes;      // row pitch of an own box (= store_cols * 2 of the first convolution)
   int extra_on;           // one more operand chunk, TMA-loaded per tile into staging buffer `own_chunks`
@@ -23,7 +23,6 @@ struct ChainParams {
   uint32_t w2_sub_bytes;  // bytes reserved per weight chunk [n2][kc] (1024-aligned)
   int w2_chunks;          // own_chunks + extra_on
   int w2_row_bytes;       // kc * 2
-  uint32_t idesc2;
   const float* bias2;
   int bias2_len;
   EpilogueParams ep2;     // Cout / act of the tail (no residual)
@@ -63,8 +62,8 @@ inline const char* chain_setup(const yb_op_desc& d, int block_n, int n_tiles, in
   if (c.Cout_pad % 16 || c.Cout_pad < c.Cout || c.Cout_pad > 256 || c.Cout % 8) return "tail Cout/Cout_pad";
   if (c.out_cstride % 8 || c.out_cstride < c.Cout) return "tail out_cstride";
   if ((reinterpret_cast<uintptr_t>(c.out) & 15) || (reinterpret_cast<uintptr_t>(c.weight) & 15)) return "tail tensors must be 16-byte aligned";
-  const int n2 = c.Cout_pad;
-  if (2 * block_n + 2 * n2 > 512) return "accumulators of the convolution and its tail exceed TMEM";
+  int n2 = 16;   // a wgmma N; the weight rows past Cout_pad are zero-filled by the TMA unit
+  while (n2 < c.Cout_pad) n2 <<= 1;
   cp->on = 1;
   cp->n2 = n2;
   cp->own_chunks = own_chunks;
@@ -77,8 +76,6 @@ inline const char* chain_setup(const yb_op_desc& d, int block_n, int n_tiles, in
   cp->w2_sub_bytes = (static_cast<uint32_t>(n2 * kc * 2) + 1023u) & ~1023u;
   cp->w2_chunks = own_chunks + extra_on;
   cp->w2_row_bytes = kc * 2;
-  const uint32_t fmt = d.dtype == YB_BF16 ? 1u : 0u;
-  cp->idesc2 = (1u << 4) | (fmt << 7) | (fmt << 10) | (static_cast<uint32_t>(n2 >> 3) << 17) | (8u << 24);
   cp->bias2 = c.bias;
   cp->bias2_len = c.Cout_pad;
   cp->ep2.Cout = c.Cout;
@@ -90,6 +87,6 @@ inline const char* chain_setup(const yb_op_desc& d, int block_n, int n_tiles, in
 }
 
 // TMA-store box width of the tail's output (the kernels are instantiated for 64 and 32).
-inline int chain_store2_cols(int n2) { return (n2 % 64 == 0) ? 64 : ((n2 % 32 == 0) ? 32 : 16); }
+__host__ __device__ inline int chain_store2_cols(int n2) { return (n2 % 64 == 0) ? 64 : ((n2 % 32 == 0) ? 32 : 16); }
 
 }  // namespace yb

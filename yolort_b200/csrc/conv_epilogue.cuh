@@ -1,4 +1,11 @@
-// Epilogue helpers shared by the convolution kernels (bias + SiLU + residual + pack, swizzled staging).
+// Epilogue helpers shared by the convolution kernels (bias + activation + residual + pack, swizzled staging).
+//
+// The accumulator of a 128-row tile lives in the registers of the two consumer warpgroups, 64 rows each, in the wgmma
+// fragment layout: thread t of warpgroup g (warp w = t / 32, lane l) holds, for every 8-column block j,
+//   acc[4j + 0..1] = row g*64 + 16w + l/4,     columns 8j + 2(l%4) + 0..1
+//   acc[4j + 2..3] = row g*64 + 16w + l/4 + 8, same columns.
+// Each thread turns its column pairs into packed fp16/bf16 pairs and writes them into the swizzled staging box that a
+// TMA store (and, for a chained tail, a wgmma operand descriptor) reads.
 #pragma once
 #include "common.cuh"
 
@@ -22,11 +29,8 @@ __device__ __forceinline__ float rcp_approx(float x) {
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// SiLU(v) = v / (1 + 2^(-v*log2 e)); both transcendental steps on the MUFU pipe.
+// SiLU(v) = v / (1 + 2^(-v*log2 e)) in fp32; both transcendental steps on the MUFU pipe.
 __device__ __forceinline__ float silu(float v) { return v * rcp_approx(1.0f + ex2_approx(v * -1.4426950408889634f)); }
-
-// r3.1 graphs (yolort/v5/models/common.py:64 nn.Hardswish, :142 nn.LeakyReLU(0.1)), ATen's formulas
-// hardswish(x) = x * min(max(x + 3, 0), 6) / 6 ; leaky_relu(x) = x > 0 ? x : x * 0.1 -- see epilogue_box<.., kRareAct>.
 
 template <bool kBf16>
 __device__ __forceinline__ uint32_t pack2(float a, float b) {
@@ -48,255 +52,67 @@ __device__ __forceinline__ float2 unpack2(uint32_t u) {
 }
 
 // Physical 16-byte chunk index of logical chunk `j` in row `r` of a tile whose rows are `row_bytes`
-// long, under the TMA/UMMA swizzle of the same width (address bits [4,7) ^= bits [7,10), truncated).
+// long, under the TMA/wgmma swizzle of the same width (address bits [4,7) ^= bits [7,10), truncated).
 __device__ __forceinline__ int swizzle_chunk(int r, int j, int row_bytes) {
   if (row_bytes == 128) return j ^ (r & 7);
   if (row_bytes == 64) return j ^ ((r >> 1) & 3);
   return j ^ ((r >> 2) & 1);
 }
 
+// The two accumulator rows of this thread: position in the tile, output pixel, and whether it exists.
+struct FragRows {
+  int loc[2];
+  long long row[2];
+  bool ok[2];
+};
 
-// Slow path of epilogue_box for a batch that holds a strongly negative pre-activation (v < kSiluExactBelow).  Both fast
-// tails evaluate SiLU as h + h * tanh(h) with tanh.approx.f16x2, h = v / 2: for v < -8 tanh(h) is one or two fp16 steps
-// (2^-11) above -1 and h (1 + tanh h) -- a result of a few 1e-3 -- is off by up to |h| 2^-11 > 2^-9, the stage-wise
-// bound.  Such inputs are rare (none in the zoo's own layers, but random test tensors find them), so the whole warp
-// re-reads the batch from TMEM (the accumulator is still owned by this epilogue group) and evaluates
-// v / (1 + 2^(-v log2 e)) in fp32.  Out of line: the hot kernels carry one call, not a second inlined tail.
-constexpr float kSiluExactBelow = -6.0f;
-
+// bias -> activation (SiLU / linear, or the r3.1 Hardswish / LeakyReLU(0.1)) -> + shortcut, in fp32
 template <bool kBf16>
-__device__ __noinline__ void epilogue_batch_exact(int act, int Cout, const void* residual, int res_cstride, uint32_t taddr_b,
-                                                  const float* s_bias_b, long long row, bool row_ok, int col0_b, uint8_t* my_row,
-                                                  int row_in_tile, int chunk0, int n_chunks, int row_bytes) {
-  // (the parameter block is passed by value: a reference into the kernel's __grid_constant__ parameters would make
-  // the compiler copy the whole block to local memory)
-  const bool has_res = residual != nullptr && row_ok;
-  const uint16_t* rbase = reinterpret_cast<const uint16_t*>(residual) + row * res_cstride + col0_b;
-  for (int c = 0; c < n_chunks; ++c) {
-    uint32_t acc[16];
-    tmem_ld_32x32b_x16(taddr_b + c * 16, acc);
-    tmem_ld_wait();
-    float v[16];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      v[j] = __uint_as_float(acc[j]) + s_bias_b[c * 16 + j];
-      if (act == YB_ACT_SILU) v[j] = silu(v[j]);
-    }
-    if (has_res) {
-#pragma unroll
-      for (int j = 0; j < 16; j += 2) {
-        if (col0_b + c * 16 + j < Cout) {
-          const float2 f = unpack2<kBf16>(*reinterpret_cast<const uint32_t*>(rbase + c * 16 + j));
-          v[j] += f.x;
-          v[j + 1] += f.y;
-        }
-      }
-    }
-    uint4 o0, o1;
-    o0.x = pack2<kBf16>(v[0], v[1]);
-    o0.y = pack2<kBf16>(v[2], v[3]);
-    o0.z = pack2<kBf16>(v[4], v[5]);
-    o0.w = pack2<kBf16>(v[6], v[7]);
-    o1.x = pack2<kBf16>(v[8], v[9]);
-    o1.y = pack2<kBf16>(v[10], v[11]);
-    o1.z = pack2<kBf16>(v[12], v[13]);
-    o1.w = pack2<kBf16>(v[14], v[15]);
-    const int j0 = chunk0 + 2 * c;
-    *reinterpret_cast<uint4*>(my_row + swizzle_chunk(row_in_tile, j0, row_bytes) * 16) = o0;
-    *reinterpret_cast<uint4*>(my_row + swizzle_chunk(row_in_tile, j0 + 1, row_bytes) * 16) = o1;
+__device__ __forceinline__ uint32_t epilogue_pair(const EpilogueParams& p, float v0, float v1, long long row, bool row_ok,
+                                                  int gcol) {
+  if (p.act == YB_ACT_SILU) {
+    v0 = silu(v0);
+    v1 = silu(v1);
+  } else if (p.act == YB_ACT_HARDSWISH) {
+    v0 = v0 * fminf(fmaxf(v0 + 3.0f, 0.f), 6.0f) * (1.0f / 6.0f);
+    v1 = v1 * fminf(fmaxf(v1 + 3.0f, 0.f), 6.0f) * (1.0f / 6.0f);
+  } else if (p.act == YB_ACT_LEAKY01) {
+    v0 = v0 > 0.f ? v0 : v0 * 0.1f;
+    v1 = v1 > 0.f ? v1 : v1 * 0.1f;
   }
+  if (p.residual != nullptr && row_ok && gcol < p.Cout) {   // Cout % 8 == 0: a pair never straddles it
+    const uint16_t* r = reinterpret_cast<const uint16_t*>(p.residual) + row * p.res_cstride + gcol;
+    const float2 f = unpack2<kBf16>(__ldg(reinterpret_cast<const unsigned int*>(r)));
+    v0 += f.x;
+    v1 += f.y;
+  }
+  return pack2<kBf16>(v0, v1);
 }
 
-// One TMA-store box (kCols = 16/32/64 accumulator columns of this thread's output pixel), handled in batches
-// of up to 32 columns: the TMEM loads and residual loads of a batch are issued up front (one exposed latency
-// per 32 columns instead of one per 16), then bias + SiLU (+ residual) + pack and the swizzled smem writes.
-// kRareAct instantiates the r3.1 activations (Hardswish / LeakyReLU) in a separate copy: with them as extra
-// branches of the common copy the r6.0 plan measured 5% slower (ptxas schedules the SiLU batch differently).
-// kRes: the layer adds a residual (Bottleneck shortcut).  Those take the fp32 tail: SiLU(v) and the shortcut can cancel
-// (|sum| << |SiLU(v)|), and a SiLU value already rounded to fp16 then carries an error that is large against the
-// 2^-9 (1 + |ref|) bound of the SUM (tests/test_gpu_conv.py, random shortcuts: 2 violations in 338 k with the packed tail).
-// kBatchMax: columns whose TMEM / shortcut loads are in flight together (32; 16 for the four-group kernel variant, whose
-// threads live in 104 registers).
-template <bool kBf16, int kCols, bool kRareAct = false, bool kRes = true, int kBatchMax = 32>
-__device__ __forceinline__ void epilogue_box(const EpilogueParams& p, uint32_t taddr, const float* __restrict__ s_bias,
-                                             long long row, bool row_ok, int col0, uint8_t* my_row, int row_in_tile) {
-  constexpr int kBatch = kCols < kBatchMax ? kCols : kBatchMax;
-  constexpr int kChunks = kBatch / 16;
-  constexpr int kRowBytes = kCols * 2;
-  const bool has_res = kRes && p.residual != nullptr && row_ok;
-  const uint16_t* rbase = reinterpret_cast<const uint16_t*>(p.residual) + row * p.res_cstride + col0;
+// One TMA-store box: tile columns [c0, c0 + cols) of this thread's fragment -> swizzled staging rows of `cols * 2`
+// bytes.  kN: the accumulator columns `acc` holds (the loop over 8-column blocks is unrolled so that every register
+// index is a constant).  n0: output channel of tile column 0; s_bias is indexed by tile column.
+template <bool kBf16, int kN>
+__device__ __forceinline__ void epilogue_box(const EpilogueParams& p, const float* acc, int c0, int cols,
+                                             const float* __restrict__ s_bias, const FragRows& fr, int n0, uint8_t* buf,
+                                             int lane) {
+  const int row_bytes = cols * 2;
+  const int q2 = 2 * (lane & 3);
 #pragma unroll
-  for (int b0 = 0; b0 < kCols; b0 += kBatch) {
-    uint32_t acc[kChunks][16];
+  for (int j = 0; j < kN / 8; ++j) {
+    if (8 * j >= c0 && 8 * j < c0 + cols) {
+      const int col = 8 * j + q2;
+      const float b0 = s_bias[col], b1 = s_bias[col + 1];
 #pragma unroll
-    for (int c = 0; c < kChunks; ++c) tmem_ld_32x32b_x16(taddr + b0 + c * 16, acc[c]);
-    uint4 res[kChunks][2];
-    if (has_res) {
-#pragma unroll
-      for (int c = 0; c < kChunks; ++c) {
-        const int col = col0 + b0 + c * 16;
-        const uint4* r = reinterpret_cast<const uint4*>(rbase + b0 + c * 16);
-        res[c][0] = (col < p.Cout) ? __ldg(r) : make_uint4(0, 0, 0, 0);
-        res[c][1] = (col + 8 < p.Cout) ? __ldg(r + 1) : make_uint4(0, 0, 0, 0);
+      for (int rr = 0; rr < 2; ++rr) {
+        const uint32_t o = epilogue_pair<kBf16>(p, acc[4 * j + 2 * rr] + b0, acc[4 * j + 2 * rr + 1] + b1,
+                                                fr.row[rr], fr.ok[rr], n0 + col);
+        const int r = fr.loc[rr];
+        *reinterpret_cast<uint32_t*>(buf + r * row_bytes + swizzle_chunk(r, (col - c0) >> 3, row_bytes) * 16 +
+                                     ((col - c0) & 7) * 2) = o;
       }
-    }
-    tmem_ld_wait();
-#ifndef YB_EPILOGUE_F32
-    // fp16 outputs with SiLU (or none): the whole tail in packed half2 arithmetic -- bias in fp32, ONE rounding to
-    // half2, h = v/2 (exact), tanh.approx.f16x2, HFMA2 h*t+h.  About 4
-    // instructions per element pair instead of 18.  Error budget per output: rounding of v (0.5 ulp), tanh.approx
-    // (<= 0.25 ulp of the result), the fused multiply-add (0.5 ulp) -- below the 2 ulp that
-    // the stage-wise bound 2^-9 (1 + |ref|) leaves at the start of a binade (layers WITHOUT a shortcut only: kRes above).
-    // Measured on B200: zero violations over
-    // every launch of yolov5s batch 32 640^2 / yolov5l mixed batch / yolov5x 1280^2 (worst |err| 4.4e-3 vs 3.9e-3 for
-    // the fp32 tail below), end-to-end parity unchanged, plan 1.335 -> 1.316 ms.  -DYB_EPILOGUE_F32 builds the fp32 tail
-    // for fp16 too (A/B: scripts/ab_step.sh); bf16 and the r3.1 activations always take it.
-    if constexpr (!kBf16 && !kRareAct && !kRes) {
-      uint32_t o[kBatch / 2];
-#pragma unroll
-      for (int j = 0; j < kBatch; j += 4) {
-        const float4 b4 = *reinterpret_cast<const float4*>(s_bias + b0 + j);
-        const uint32_t p0 = pack2<false>(__uint_as_float(acc[j >> 4][(j & 15) + 0]) + b4.x, __uint_as_float(acc[j >> 4][(j & 15) + 1]) + b4.y);
-        const uint32_t p1 = pack2<false>(__uint_as_float(acc[j >> 4][(j & 15) + 2]) + b4.z, __uint_as_float(acc[j >> 4][(j & 15) + 3]) + b4.w);
-        o[j / 2] = p0;
-        o[j / 2 + 1] = p1;
-      }
-      bool packed_ok = true;
-      if (p.act == YB_ACT_SILU) {
-        __half2 mn = __float2half2_rn(0.f);   // running minimum of the pre-activations (epilogue_batch_exact)
-#pragma unroll
-        for (int j = 0; j < kBatch / 2; ++j) {
-          __half2 hv = *reinterpret_cast<__half2*>(&o[j]);
-          mn = __hmin2(mn, hv);
-          const __half2 h = __hmul2(hv, __float2half2_rn(0.5f));
-          uint32_t hp = *reinterpret_cast<const uint32_t*>(&h), tp;
-          asm("tanh.approx.f16x2 %0, %1;" : "=r"(tp) : "r"(hp));
-          const __half2 r = __hfma2(h, *reinterpret_cast<__half2*>(&tp), h);
-          o[j] = *reinterpret_cast<const uint32_t*>(&r);
-        }
-        // rows outside the output (ragged tiles, the junk rows of the wrap tiling) hold arbitrary data: they must not
-        // steer the warp's choice, or two launches on the same input could round their valid rows differently
-        packed_ok = !row_ok || __hge(__hmin(__low2half(mn), __high2half(mn)), __float2half_rn(kSiluExactBelow));
-      }
-#ifdef YB_NO_SILU_GUARD      // A/B build without the guard (scripts/ab_step.sh)
-      packed_ok = true;
-#endif
-      if (!__all_sync(0xffffffffu, packed_ok)) {   // warp-uniform: the slow path re-reads TMEM (a warp-collective load)
-        epilogue_batch_exact<kBf16>(p.act, p.Cout, p.residual, p.res_cstride, taddr + b0, s_bias + b0, row, row_ok, col0 + b0, my_row, row_in_tile, b0 >> 3, kChunks, kRowBytes);
-        continue;
-      }
-      {
-#pragma unroll
-      for (int c = 0; c < kChunks; ++c) {
-        const int j0 = (b0 >> 3) + 2 * c;
-        *reinterpret_cast<uint4*>(my_row + swizzle_chunk(row_in_tile, j0, kRowBytes) * 16) = make_uint4(o[c * 8], o[c * 8 + 1], o[c * 8 + 2], o[c * 8 + 3]);
-        *reinterpret_cast<uint4*>(my_row + swizzle_chunk(row_in_tile, j0 + 1, kRowBytes) * 16) = make_uint4(o[c * 8 + 4], o[c * 8 + 5], o[c * 8 + 6], o[c * 8 + 7]);
-      }
-      }
-      continue;
-    }
-#endif
-    // Staged so that the kBatch independent SiLU chains overlap (ptxas otherwise emits them one element at a
-    // time: LDS -> EX2 -> RCP back to back, exposing ~80 cycles of latency per element).
-    float v[kBatch];
-#pragma unroll
-    for (int j = 0; j < kBatch; j += 4) {
-      const float4 b4 = *reinterpret_cast<const float4*>(s_bias + b0 + j);
-      v[j + 0] = __uint_as_float(acc[j >> 4][(j & 15) + 0]) + b4.x;
-      v[j + 1] = __uint_as_float(acc[j >> 4][(j & 15) + 1]) + b4.y;
-      v[j + 2] = __uint_as_float(acc[j >> 4][(j & 15) + 2]) + b4.z;
-      v[j + 3] = __uint_as_float(acc[j >> 4][(j & 15) + 3]) + b4.w;
-    }
-    if constexpr (kRareAct) {
-      if (p.act == YB_ACT_HARDSWISH) {
-#pragma unroll
-        for (int j = 0; j < kBatch; ++j) v[j] = v[j] * fminf(fmaxf(v[j] + 3.0f, 0.f), 6.0f) * (1.0f / 6.0f);
-      } else {
-#pragma unroll
-        for (int j = 0; j < kBatch; ++j) v[j] = v[j] > 0.f ? v[j] : v[j] * 0.1f;
-      }
-    } else if (p.act == YB_ACT_SILU) {
-      float mn = 0.f;
-#pragma unroll
-      for (int j = 0; j < kBatch; ++j) mn = fminf(mn, v[j]);
-#ifdef YB_NO_SILU_GUARD
-      mn = 0.f;
-#endif
-      if (__any_sync(0xffffffffu, row_ok && mn < kSiluExactBelow)) {   // see epilogue_batch_exact (valid rows only decide)
-        epilogue_batch_exact<kBf16>(p.act, p.Cout, p.residual, p.res_cstride, taddr + b0, s_bias + b0, row, row_ok, col0 + b0, my_row, row_in_tile, b0 >> 3, kChunks, kRowBytes);
-        continue;
-      }
-      // SiLU(v) = h + h*tanh(h), h = v/2.  tanh.approx.f16x2 evaluates two elements per MUFU op (0.5 op per
-      // element instead of the 2 of exp+rcp, which made 1x1 layers MUFU-bound: 16 ops/clk/SM).  Its ~2^-11
-      // absolute error is below the fp16 rounding of the stored activation for |v| < ~4 (measured network
-      // rel-RMS error 6.4e-4 vs 4.6e-4 with an exact SiLU).
-#pragma unroll
-      for (int j = 0; j < kBatch; j += 2) {
-        const float h0 = 0.5f * v[j], h1 = 0.5f * v[j + 1];
-        const uint32_t hp = pack2<false>(h0, h1);
-        uint32_t tp;
-        asm("tanh.approx.f16x2 %0, %1;" : "=r"(tp) : "r"(hp));
-        const float2 t = unpack2<false>(tp);
-        v[j] = fmaf(h0, t.x, h0);
-        v[j + 1] = fmaf(h1, t.y, h1);
-      }
-    }
-    if (has_res) {
-#pragma unroll
-      for (int c = 0; c < kChunks; ++c) {
-        const uint32_t ru[8] = {res[c][0].x, res[c][0].y, res[c][0].z, res[c][0].w,
-                                res[c][1].x, res[c][1].y, res[c][1].z, res[c][1].w};
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float2 f = unpack2<kBf16>(ru[j]);
-          v[c * 16 + 2 * j] += f.x;
-          v[c * 16 + 2 * j + 1] += f.y;
-        }
-      }
-    }
-#pragma unroll
-    for (int c = 0; c < kChunks; ++c) {
-      uint4 o0, o1;
-      const float* w = v + c * 16;
-      o0.x = pack2<kBf16>(w[0], w[1]);
-      o0.y = pack2<kBf16>(w[2], w[3]);
-      o0.z = pack2<kBf16>(w[4], w[5]);
-      o0.w = pack2<kBf16>(w[6], w[7]);
-      o1.x = pack2<kBf16>(w[8], w[9]);
-      o1.y = pack2<kBf16>(w[10], w[11]);
-      o1.z = pack2<kBf16>(w[12], w[13]);
-      o1.w = pack2<kBf16>(w[14], w[15]);
-      const int j0 = (b0 >> 3) + 2 * c;
-      *reinterpret_cast<uint4*>(my_row + swizzle_chunk(row_in_tile, j0, kRowBytes) * 16) = o0;
-      *reinterpret_cast<uint4*>(my_row + swizzle_chunk(row_in_tile, j0 + 1, kRowBytes) * 16) = o1;
     }
   }
-}
-
-template <bool kBf16, bool kRareAct, bool kRes = true>
-__device__ __forceinline__ void epilogue_box_dispatch(const EpilogueParams& p, int store_cols, uint32_t taddr,
-                                                      const float* s_bias, long long row, bool row_ok, int col0,
-                                                      uint8_t* my_row, int row_in_tile) {
-  if (store_cols == 64)
-    epilogue_box<kBf16, 64, kRareAct, kRes>(p, taddr, s_bias, row, row_ok, col0, my_row, row_in_tile);
-  else if (store_cols == 32)
-    epilogue_box<kBf16, 32, kRareAct, kRes>(p, taddr, s_bias, row, row_ok, col0, my_row, row_in_tile);
-  else
-    epilogue_box<kBf16, 16, kRareAct, kRes>(p, taddr, s_bias, row, row_ok, col0, my_row, row_in_tile);
-}
-
-// Kernel-level specialisation (dtype, TMA-store box width, activation family, fused decode).  Every variant the hot
-// path uses is its own kernel with exactly ONE epilogue copy inlined: with all copies inlined in one kernel and
-// selected at run time, adding the r3.1 activations cost the r6.0 plan 5-13% (measured A/B on the same box,
-// 1.85 -> 1.95 / 2.10 ms); kStoreCols == 0 keeps the run-time selection for the rarely used variants.
-template <bool kBf16, int kStoreCols, bool kRareAct, bool kRes = true, int kBatchMax = 32>
-__device__ __forceinline__ void epilogue_box_select(const EpilogueParams& p, int store_cols, uint32_t taddr,
-                                                    const float* s_bias, long long row, bool row_ok, int col0,
-                                                    uint8_t* my_row, int row_in_tile) {
-  if constexpr (kStoreCols != 0)
-    epilogue_box<kBf16, kStoreCols, kRareAct, kRes, kBatchMax>(p, taddr, s_bias, row, row_ok, col0, my_row, row_in_tile);
-  else
-    epilogue_box_dispatch<kBf16, kRareAct, kRes>(p, store_cols, taddr, s_bias, row, row_ok, col0, my_row, row_in_tile);
 }
 
 }  // namespace yb

@@ -1,5 +1,5 @@
 // Score-key encoding and reference-order arithmetic shared by the stand-alone decode kernel (decode_nms.cu) and the
-// fused decode epilogue of the head convolutions (conv_sm100.cu).
+// fused decode epilogue of the head convolutions (conv_sm90.cu).
 #pragma once
 #include "common.cuh"
 

@@ -172,8 +172,7 @@ __global__ void decode_candidates_kernel(const __grid_constant__ DecodeParams p,
 // objectness of its pixel's anchors and scans the classes of those that pass, 32 pixels wide, out of shared memory, a
 // raw-logit pre-test sparing the exact sigmoid for almost every class.  Candidates are
 // collected in a block-local list and appended to the image's key arena with ONE global atomic per block: with an
-// atomic per candidate group the kernel sat at 120-127 us whatever else changed -- ~2 000 same-address L2 atomics per
-// image, ~27 cycles each, only ~7 images in flight (measured on B200, yolov5s batch 32; the per-anchor kernel above: 92 us).
+// atomic per candidate group the kernel is bound by ~2 000 same-address L2 atomics per image.
 // Arithmetic, candidate keys and the dense box array are those of the kernel above.
 constexpr int kRowPixels = 32;       // pixels per warp
 constexpr int kRowWarps = 4;         // warps per block
@@ -468,8 +467,7 @@ __device__ void bitonic_sort_smem(uint64_t* keys, int n) {
 // Bitonic sort of R * blockDim.x keys (blockDim.x = kNmsThreads) with the keys in REGISTERS: thread t owns elements
 // t*R .. t*R+R-1.  Of the log2(n)(log2(n)+1)/2 compare-exchange stages only those whose partner distance reaches into
 // another warp (j >= 32 R) go through shared memory with a barrier; distances inside a warp use shuffles and distances
-// below R stay inside the thread.  2048 keys: 10 barrier stages instead of 66 (measured: 50 k -> see profiles/ cycles for the
-// per-image sort of the bench's ~1100 candidates).  Same network as bitonic_sort_smem, so the same (total) order.
+// below R stay inside the thread.  2048 keys: 10 barrier stages instead of 66.  Same network as bitonic_sort_smem, so the same (total) order.
 template <int R>
 __device__ void bitonic_sort_regs(uint64_t* s) {
   const int tid = threadIdx.x;

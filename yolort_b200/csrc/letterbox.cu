@@ -5,7 +5,7 @@
 //                                      recompute_scale_factor=True), i.e. ATen upsample_bilinear2d
 //   batch_images            :297-330 -> new_full(fill) + centred copy
 // and fuses the uint8 -> [0,1] conversion of the default loader (yolov5.py:218-228) plus the layout
-// change the first convolution wants (space-to-depth NHWC, see conv_sm100.cu / engine.py).
+// change the first convolution wants (space-to-depth NHWC, see conv_sm90.cu / engine.py).
 //
 // HBM-bound: per image it reads 3*h*w source bytes and writes the canvas once.  The hot variant
 // (letterbox_s2d_tile_kernel: uint8 sources -> the plan's space-to-depth canvas) stages the source rectangle of a
@@ -135,7 +135,7 @@ __device__ __forceinline__ __nv_bfloat16 cvt_out<__nv_bfloat16>(float v) {
 
 // byte -> float without a conversion instruction: 0x4B000000 | b is the float 2^23 + b, exactly; subtracting 2^23 leaves b.
 // (The conversion pipe, I2F / F2F, runs at a fraction of the ALU rate: the uint8 -> fp16 canvas was bound by it, ~48 us
-// for 39 M values whatever the memory access pattern -- measured on B200 with two different kernels.)
+// for 39 M values whatever the memory access pattern.)
 __device__ __forceinline__ float byte_to_float(uint32_t word, int k) {   // byte k (0..3) of `word`
   return __fsub_rn(__uint_as_float(__byte_perm(word, 0x4B000000u, 0x7540u | static_cast<uint32_t>(k))), 8388608.0f);
 }
@@ -377,7 +377,7 @@ letterbox_s2d_tile_kernel(const __grid_constant__ BatchGeom bg, int img0, int Hb
 // any serving front end that resizes on the host): nothing to interpolate, nothing to pad.  What bounds this copy is
 // the number of 128-byte lines a STORE instruction touches (one L1 wavefront per line), not arithmetic: with a thread
 // per space-to-depth pixel a warp's 16-byte stores sit 32 bytes apart (8 lines per instruction, the tile kernel's copy
-// path: 47 us), with a thread per 8 canvas pixels 128 bytes apart (32 lines: 60 - 66 us, measured).  Here LANE l WRITES
+// path), with a thread per 8 canvas pixels 128 bytes apart (32 lines).  Here LANE l WRITES
 // BYTES [16 l, 16 l + 16) of a 512-byte run: lane (x, dy) = (l / 2, l % 2) converts canvas row 2Y + dy, columns 2X,
 // 2X + 1 (three 2-byte loads; even / odd lanes read two source rows, 32 contiguous bytes each) into its half of
 // space-to-depth pixel X -- four lines per store instruction, four such runs per warp.

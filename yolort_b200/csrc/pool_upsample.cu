@@ -8,7 +8,7 @@
 //  * nearest-neighbour 2x upsample (nn.Upsample(scale_factor=2), path_aggregation_network.py:123,134),
 //    writing into a channel window of the next concat buffer.
 #include "common.cuh"
-#include "conv_sm100.h"
+#include "conv_sm90.h"
 
 namespace yb {
 namespace {
@@ -154,8 +154,8 @@ int validate_pool_or_upsample(const yb_op_desc& d) {
 
 int spp_pool_launch(const yb_op_desc& d, cudaStream_t stream) {
   // channel octets per CTA: as many (8, 4, 2, 1) as divide the octet count and fit 3 buffers in shared memory
-  // (measured on B200, 256 channels at 20 x 20, batch 32: G = 1 / 2 / 4 all 22.5 us, G = 8 24.6 us -- the kernel is bound by
-  // its seven barrier-separated passes per CTA, not by the lines a load touches; two octets keep loads at whole sectors)
+  // (the kernel is bound by its seven barrier-separated passes per CTA, not by the lines a load touches; two octets keep
+  // loads at whole sectors)
   int G = 2;
   while (G > 1 && (((d.Cin >> 3) % G) != 0 || static_cast<size_t>(d.H) * d.W * 16 * 3 * G > 200 * 1024)) G >>= 1;
   const size_t plane_smem = static_cast<size_t>(d.H) * d.W * 16 * 3 * G;

@@ -134,8 +134,7 @@ def stem_superpixel(w: torch.Tensor, b: torch.Tensor, pack: int = 4) -> Tuple[to
     Exact: output pixel x = pack*X + po reads input pixels x + b - 1 = pack*(X + S - 1) + pi, i.e. column tap
     b = pack*(S-1) + pi - po + 1 when that lies in {0,1,2}; all other entries of the expanded kernel are zero.
     The memory layouts do not change (NHWC rows are contiguous), only the GEMM's shape does: the 16-channel
-    space-to-depth stem input would otherwise be fetched by the TMA unit in 32-byte rows (measured 372 us for
-    the loads alone); as 128-byte super-pixels the stem runs like an ordinary 64->128 3x3 layer."""
+    space-to-depth stem input would otherwise be fetched by the TMA unit in 32-byte rows; as 128-byte super-pixels the stem runs like an ordinary 64->128 3x3 layer."""
     co, ci, kh, kw = w.shape
     assert (kh, kw) == (3, 3)
     out = torch.zeros((pack * co, pack * ci, 3, 3), dtype=w.dtype, device=w.device)
@@ -156,7 +155,7 @@ def stem_band(w: torch.Tensor, b: torch.Tensor) -> Tuple[torch.Tensor, torch.Ten
     holds, per filter row ky, the 96 weights over (r, c) with r = po + kx the position inside that span; everything
     else of the 4Co x (3*3*64) super-pixel matrix is structurally zero and is not stored.  Layout
     [4*Co, 3, 128]: 96 real K-columns per filter row padded to two 64-column blocks (the kernel multiplies 6 K=16
-    steps per row and never touches the padding).  Measured on B200 (yolov5s batch 32): 164 -> 88 us."""
+    steps per row and never touches the padding)."""
     co, ci, kh, kw = w.shape
     assert (ci, kh, kw) == (16, 3, 3)
     out = torch.zeros((4 * co, 3, 128), dtype=w.dtype, device=w.device)
@@ -327,8 +326,8 @@ def lower_yolo(model: nn.Module, dtype: torch.dtype, device: torch.device, stem_
     t0 = L.buf("body.0", 2, w.shape[0])
     # The stem runs over "super-pixels" of 4 horizontally adjacent s2d pixels (128-byte TMA rows instead of 32).  Its
     # expanded weight matrix is block-banded, and when the band (6 slabs of 4*Cout x 64) fits in shared memory next to
-    # two patches (4*Cout <= 128: yolov5n / s) the banded kernel variant multiplies only the band (measured on B200,
-    # yolov5s batch 32: 164 -> 88 us); wider stems (m / l / x) use the dense super-pixel form.
+    # two patches (4*Cout <= 128: yolov5n / s) the banded kernel variant multiplies only the band; wider stems
+    # (m / l / x) use the dense super-pixel form.
     spk = 4
     co4 = spk * w.shape[0]
     if stem_variant == "band" or (stem_variant == "auto" and co4 % 64 == 0 and co4 <= 128
@@ -554,8 +553,6 @@ class PlanInstance:
         code = _C.dtype_code(L.dtype)
         self._chains: List[_C.ConvChain] = []    # yb_conv_chain blocks the descriptors point at (kept alive)
         no_nsplit = os.environ.get("YB_NO_NSPLIT", "0") == "1"    # A/B timing: keep streamed weights + tile pairs
-        acc2 = os.environ.get("YB_ACC4", "0") == "1"              # A/B timing: four accumulator stages instead of two
-        no_wide = os.environ.get("YB_WIDE", "0") == "1"           # A/B timing: four epilogue groups where they apply
 
         def make_desc(op: _Op, ptr) -> "_C.OpDesc":
             d = _C.OpDesc()
@@ -576,7 +573,7 @@ class PlanInstance:
                 d.Cout_pad, _, d.Cin_pad = op.weight.shape
                 if op.band:
                     d.Cin_pad = 64     # [Cout_pad, 3, 2 x 64] banded stem matrix: one 64-channel chunk of super-pixels
-            d.reserved = (1 if op.force_im2col else 0) | (2 if op.band else 0) | (8 if no_nsplit else 0) | (16 if acc2 else 0) | (32 if no_wide else 0)
+            d.reserved = (1 if op.force_im2col else 0) | (2 if op.band else 0) | (8 if no_nsplit else 0)
             if op.residual is not None:
                 d.residual, d.res_cstride = ptr(op.residual), op.residual.buf.C
             return d
@@ -784,7 +781,7 @@ class Engine:
     def __init__(self, model: nn.Module, dtype: torch.dtype, device: torch.device, max_arena_bytes: Optional[int] = None):
         if device.type != "cuda":
             raise _C.NativeLibraryError(
-                f"yolort_b200 runs on sm_100a GPUs only; model parameters are on {device} (no CPU fallback)")
+                f"yolort_b200 runs on sm_90a GPUs only; model parameters are on {device} (no CPU fallback)")
         if dtype not in (torch.float16, torch.bfloat16):
             raise _C.NativeLibraryError(f"compute dtype must be float16 or bfloat16, got {dtype}")
         _C.lib()

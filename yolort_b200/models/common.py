@@ -4,7 +4,7 @@ These modules reproduce the parameter/buffer names of the reference blocks
 (yolort/v5/models/common.py:42-73 Conv, :94-116 Bottleneck, :119-146 BottleneckCSP, :149-173 C3, :176-187 SPP,
 :210-234 Focus) so that a
 reference `state_dict` loads unchanged.  They do not compute: the arithmetic of the whole
-backbone is executed by the sm_100a execution plan (yolort_b200/engine.py -> libyolort_b200.so).
+backbone is executed by the sm_90a execution plan (yolort_b200/engine.py -> libyolort_b200.so).
 Calling `forward` on a block is an error by design -- there is no PyTorch/CPU fallback.
 """
 from torch import nn
@@ -16,7 +16,7 @@ BN_MOMENTUM = 0.03
 class _PlanOnly(nn.Module):
     def forward(self, *args, **kwargs):  # pragma: no cover - guard
         raise RuntimeError(
-            f"{type(self).__name__} is executed by the sm_100a plan (yolort_b200.engine); "
+            f"{type(self).__name__} is executed by the sm_90a plan (yolort_b200.engine); "
             "it has no eager PyTorch forward."
         )
 

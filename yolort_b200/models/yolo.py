@@ -133,8 +133,8 @@ class YOLO(nn.Module):
         """Plan instance for a batch of N canvases of H x W.  `keep_intermediates=True` gives every activation its
         own bytes (inspection / stage-wise tests); the default arena reuses the bytes of dead activations.
         `chunked=True`: the variant `YOLOv5.predict` uses for host inputs (front ops runnable per image chunk)."""
-        # The fused decode epilogue (heads emit NMS candidates instead of logits) is functional but, as measured in
-        # round 1, slower than storing fp16 logits + the stand-alone decode kernel; opt-in until it is tuned.
+        # The fused decode epilogue (heads emit NMS candidates instead of logits) is functional; opt-in until it is
+        # shown to be faster than storing fp16 logits + the stand-alone decode kernel.
         fuse = os.environ.get("YB_FUSED_DECODE", "0") == "1"
         return self.engine().plan(N, H, W, self.post_config() if fuse else None, keep_intermediates, chunked and not fuse)
 

@@ -44,9 +44,7 @@ def pack_detections(boxes: Tensor, scores: Tensor, labels: Tensor, counts: Optio
 class DetectionGather:
     """The per-step exchange of a data-parallel serving loop, kept off the compute stream: packing the padded outputs of
     `forward_padded` into the [n, D+1, 6] payload (half a dozen small element-wise launches) and the ONE NCCL all-gather
-    both run on a side stream, so the next step's letterbox / convolutions start right after the NMS kernel.  (Measured
-    on 2 x B200, weak scaling at 32 images per GPU: 1.478 - 1.489 ms per step against 1.453 ms on one GPU, efficiency
-    0.98, with the pack on either stream; NCCL restricted to one channel made it worse, 1.541 ms.)
+    both run on a side stream, so the next step's letterbox / convolutions start right after the NMS kernel.
 
         g = DetectionGather(device)
         for batch in batches:
