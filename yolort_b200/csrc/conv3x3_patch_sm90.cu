@@ -169,6 +169,11 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
                      const PatchParams p) {
   constexpr bool kChain = kN2 != 0;
   constexpr int kTileAcc = kN <= 64 ? kN : kN / 2;   // accumulator registers per thread: two tiles when kN <= 64
+  // Register budget.  The N = 128 instance and the N = 64 instances with a chained tail spill within the 168 registers
+  // that __launch_bounds__ gives every thread, so their producers hand registers to the consumers (40 / 232).  The
+  // other instances fit in 168 without spilling and keep the even split: with 232 registers ptxas builds a schedule for
+  // them that runs 1-2.5 % slower on the H100 (pair-task and stride-2 launches).
+  constexpr bool kRealloc = kN == 128 || (kChain && kN == 64);
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t a_full[kMaxA], a_empty[kMaxA];
   __shared__ __align__(8) uint64_t b_full[kMaxB], b_empty[kMaxB];
@@ -210,10 +215,11 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
   // (or stores over them) and waits for the previous grid to complete first.
   if (warp != 2) asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  if (warp < 4)
-    regs_producer();
-  else
-    regs_consumer();
+  // Each role raises or lowers its register budget on a path of its own: the producer warps return before the consumer
+  // code, so ptxas never reaches the consumers from the 40-register budget.
+  if constexpr (kRealloc) {
+    if (warp < 4) regs_producer();
+  }
 
   if (warp == 0) {
     // ===================== patch (A) producer (warp-uniform loop, one elected lane issues) =====================
@@ -288,6 +294,7 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
     return;
   }
   if (warp < 4) return;
+  if constexpr (kRealloc) regs_consumer();
 
   // ===================== consumers: MMA + epilogue of 64 accumulator rows each =====================
   const int g = (warp >> 2) - 1;
