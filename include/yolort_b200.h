@@ -88,6 +88,7 @@ int yb_scale_coords_params(int Hb, int Wb, int src_h, int src_w, float* out3);
 #define YB_OP_CONV 0       /* act(conv(x) * bn_scale + bn_shift) [+ residual]; BN pre-folded      */
 #define YB_OP_SPP_POOL 1   /* y[c:2c]=mp5(x) y[2c:3c]=mp9(x) y[3c:4c]=mp13(x), stride 1, -inf pad */
 #define YB_OP_UPSAMPLE2X 2 /* nearest x2 (nn.Upsample(scale_factor=2))                            */
+#define YB_OP_ATTENTION 3  /* multi-head softmax(Q_h K_h^T / sqrt(d)) V_h over the H*W tokens of each image  */
 
 #define YB_ACT_NONE 0
 #define YB_ACT_SILU 1
@@ -137,6 +138,17 @@ typedef struct {
 
 /* All activation tensors are NHWC views: element (n,y,x,c) at base[((n*H+y)*W+x)*cstride + c].
  * `cstride` >= channels lets a producer write straight into a slice of a concat buffer. */
+/* YB_OP_ATTENTION (the nn.MultiheadAttention core of the reference's TransformerLayer, yolort/v5/models/common.py:
+ * 308-331; its in- and out-projections are YB_OP_CONV 1x1 ops) reads the fields as follows:
+ *   in:        the packed [q | k | v] NHWC view, Cin = 3E, in_cstride >= 3E
+ *   out:       an NHWC view, Cout = E, out_cstride >= E
+ *   N, H, W:   the sequence of image n is its L = H*W pixels in row-major order; Ho == H, Wo == W
+ *   ksize:     the number of heads; head h reads channels [h*d, (h+1)*d) of each third and writes the same window
+ *              of `out`, d = E / heads = 64 (the only head width implemented)
+ *   weight, bias, residual, decode and chain must be NULL; act and reserved must be 0; Cin_pad, Cout_pad, stride,
+ *   pad and res_cstride are not read.
+ * The op computes softmax(Q_h K_h^T / sqrt(d)) V_h for every image and head, with no mask, fp32 softmax and
+ * accumulation.  Channel counts and strides must be multiples of 8 and both tensors 16-byte aligned. */
 typedef struct {
   int32_t kind;
   int32_t dtype;                /* YB_F16 or YB_BF16 (accumulation is always fp32) */

@@ -23,12 +23,15 @@ using namespace yb;
 struct yb_plan {
   struct Step {
     yb_op_desc desc;
-    ConvOp* conv;  // non-null for YB_OP_CONV
+    ConvOp* conv;       // non-null for YB_OP_CONV
+    AttentionOp* attn;  // non-null for YB_OP_ATTENTION
   };
   std::vector<Step> steps;
   ~yb_plan() {
-    for (auto& s : steps)
+    for (auto& s : steps) {
       if (s.conv) conv_op_destroy(s.conv);
+      if (s.attn) attention_op_destroy(s.attn);
+    }
   }
 };
 
@@ -54,6 +57,7 @@ extern "C" int yb_plan_create(const yb_op_desc* ops, int n_ops, yb_plan** plan_o
     yb_plan::Step st;
     st.desc = ops[i];
     st.conv = nullptr;
+    st.attn = nullptr;
     int rc = YB_OK;
     if (ops[i].in == nullptr || ops[i].out == nullptr) {
       set_error("plan_create: op %d has a null tensor", i);
@@ -65,6 +69,8 @@ extern "C" int yb_plan_create(const yb_op_desc* ops, int n_ops, yb_plan** plan_o
       } else {
         rc = conv_op_create(ops[i], &st.conv);
       }
+    } else if (ops[i].kind == YB_OP_ATTENTION) {
+      rc = attention_op_create(ops[i], &st.attn);   // validates before any driver call
     } else if (ops[i].kind == YB_OP_SPP_POOL || ops[i].kind == YB_OP_UPSAMPLE2X) {
       rc = validate_pool_or_upsample(ops[i]);
     } else {
@@ -96,6 +102,9 @@ extern "C" int yb_plan_run_range(yb_plan* plan, int first, int count, void* stre
     switch (st.desc.kind) {
       case YB_OP_CONV:
         rc = conv_op_launch(st.conv, stream);
+        break;
+      case YB_OP_ATTENTION:
+        rc = attention_op_launch(st.attn, stream);
         break;
       case YB_OP_SPP_POOL:
         rc = spp_pool_launch(st.desc, stream);

@@ -106,6 +106,14 @@ __device__ __forceinline__ void tma_load_2d(const void* desc, uint64_t* bar, voi
       "l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_3d(const void* desc, uint64_t* bar, void* smem_dst, int c0, int c1,
+                                            int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
 // im2col-mode load of an NHWC tensor: coordinates {c, w, h, n} of the first base pixel and the
 // filter-tap offsets {off_w, off_h}; the engine walks `pixelsPerColumn` output positions.
 __device__ __forceinline__ void tma_load_im2col_4d(const void* desc, uint64_t* bar, void* smem_dst,
@@ -124,6 +132,12 @@ __device__ __forceinline__ void tma_store_2d(const void* desc, const void* smem_
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
                    reinterpret_cast<uint64_t>(desc)),
                "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void tma_store_3d(const void* desc, const void* smem_src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(desc)),
+               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
                : "memory");
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }

@@ -441,6 +441,12 @@ int mma_n(int n) {
 
 }  // namespace
 
+int encode_tiled_entry(EncodeTiledFn* out) {
+  const int rc = load_driver_entry_points();
+  if (rc == YB_OK) *out = g_encode_tiled;
+  return rc;
+}
+
 using ConvKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
                               const ConvKernelParams);
 

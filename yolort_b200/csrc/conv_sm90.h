@@ -25,6 +25,16 @@ int conv_configure_check(const yb_op_desc& d, int* info = nullptr);         // h
 int conv_op_launch(const ConvOp* op, cudaStream_t stream);
 void conv_op_destroy(ConvOp* op);
 
+// cuTensorMapEncodeTiled from the driver (looked up once)
+int encode_tiled_entry(EncodeTiledFn* out);
+
+// multi-head attention (attention_sm90.cu)
+struct AttentionOp;
+int attention_configure_check(const yb_op_desc& d);   // host-only validation (no driver calls)
+int attention_op_create(const yb_op_desc& d, AttentionOp** out);
+int attention_op_launch(const AttentionOp* op, cudaStream_t stream);
+void attention_op_destroy(AttentionOp* op);
+
 // HBM-bound helpers of the neck (pool_upsample.cu)
 int spp_pool_launch(const yb_op_desc& d, cudaStream_t stream);
 int upsample2x_launch(const yb_op_desc& d, cudaStream_t stream);

@@ -25,7 +25,7 @@ import torch
 from torch import nn
 
 from . import _C
-from .models.common import C3, BottleneckCSP, Conv, Focus, SPP
+from .models.common import C3, C3TR, BottleneckCSP, Conv, Focus, SPP, TransformerBlock
 
 
 def _round_up(v: int, m: int) -> int:
@@ -225,8 +225,10 @@ class _Lowering:
         self.conv(name, w, b, src, dst, k, s, p, act_code(m.act), residual)
 
     def block(self, name, m, src: _View, dst: _View):
-        """C3 (r4.0 / r6.0 graphs) or BottleneckCSP (r3.1)."""
-        if isinstance(m, C3):
+        """C3 (r4.0 / r6.0 graphs), C3TR (yolov5ts) or BottleneckCSP (r3.1)."""
+        if isinstance(m, C3TR):      # a C3 subclass: tested first
+            self.c3tr(name, m, src, dst)
+        elif isinstance(m, C3):
             self.c3(name, m, src, dst)
         elif isinstance(m, BottleneckCSP):
             self.csp(name, m, src, dst)
@@ -283,6 +285,71 @@ class _Lowering:
                 self.ops[-1].chain_store = False
             y = out
         self.conv_module(f"{name}.cv3", m.cv3, _View(cat, 0, 2 * c_), dst)
+
+    def c3tr(self, name, m: C3TR, src: _View, dst: _View):
+        """common.py:360-367: cv3(cat(m(cv1(x)), cv2(x))) with m a TransformerBlock; cv1 || cv2 and cv3 as in c3()."""
+        div = src.buf.div
+        c_ = m.cv1.conv.out_channels
+        cat = self.buf(f"{name}.cat", div, 2 * c_)
+        w1, b1 = fold_conv_bn(m.cv1)
+        w2, b2 = fold_conv_bn(m.cv2)
+        self.conv(f"{name}.cv1+cv2", torch.cat([w1, w2], 0), torch.cat([b1, b2], 0), src,
+                  _View(cat, 0, 2 * c_), 1, 1, 0, _C.YB_ACT_SILU)
+        self.transformer(f"{name}.m", m.m, _View(cat, 0, c_), _View(cat, 0, c_))
+        self.conv_module(f"{name}.cv3", m.cv3, _View(cat, 0, 2 * c_), dst)
+
+    def transformer(self, name, m: TransformerBlock, src: _View, dst: _View):
+        """TransformerBlock over the H*W tokens of each image (common.py:334-357, TransformerLayer :308-331) as 1x1
+        convolutions (act NONE) around one attention op per layer.  Every linear map in front of the attention folds
+        into its neighbour in fp64 and is rounded once:
+            pos   p' = (I + W_linear) p + b_linear
+            qkv   [W_in,q W_q ; W_in,k W_k ; W_in,v W_v] p' + in_proj_bias          (E -> 3E)
+            attn  softmax(Q_h K_h^T / sqrt(d)) V_h per head                          (YB_OP_ATTENTION)
+            out   x1 = W_out a + b_out + p'
+            fc    x2 = (W_fc2 W_fc1) x1 + x1
+        The 1/sqrt(d) scale stays in the attention op.  flops_per_pixel counts the reference's work (q, k, v and
+        in_proj are four E x E products; fc1 and fc2 two)."""
+        if m.conv is not None:
+            raise NotImplementedError(f"{name}: transformer block with an input Conv (c1 != c2)")
+        if len(m.tr) == 0:
+            raise NotImplementedError(f"{name}: transformer block without layers")
+        div = src.buf.div
+        E = m.c2
+        lin = m.linear
+        W = lin.weight.detach().double()
+        eye = torch.eye(E, dtype=torch.float64, device=W.device)
+
+        def w4(t):       # [Cout, E] linear map -> 1x1 convolution weight
+            return t.reshape(t.shape[0], E, 1, 1)
+
+        x = _View(self.buf(f"{name}.p", div, E), 0, E)
+        self.conv(f"{name}.linear(pos)", w4(eye + W), lin.bias.detach().double(), src, x, 1, 1, 0, _C.YB_ACT_NONE,
+                  ref_flops_per_pixel=2 * E * E)
+        n = len(m.tr)
+        for i, layer in enumerate(m.tr):
+            ma = layer.ma
+            heads = ma.num_heads
+            if E % heads or E // heads != 64 or not getattr(ma, "_qkv_same_embed_dim", True) or ma.in_proj_bias is None:
+                raise NotImplementedError(f"{name}.tr.{i}: the attention kernel implements 64-wide heads with a packed "
+                                          f"in-projection and bias (E={E}, heads={heads})")
+            p = f"{name}.tr.{i}"
+            w_in = ma.in_proj_weight.detach().double()
+            w_qkv = torch.cat([w_in[:E] @ layer.q.weight.detach().double(),
+                               w_in[E:2 * E] @ layer.k.weight.detach().double(),
+                               w_in[2 * E:] @ layer.v.weight.detach().double()], 0)
+            qkv = _View(self.buf(f"{p}.qkv", div, 3 * E), 0, 3 * E)
+            self.conv(f"{p}.q|k|v+in_proj", w4(w_qkv), ma.in_proj_bias.detach().double(), x, qkv, 1, 1, 0,
+                      _C.YB_ACT_NONE, ref_flops_per_pixel=12 * E * E)
+            att = _View(self.buf(f"{p}.attn", div, E), 0, E)
+            self.ops.append(_Op(_C.YB_OP_ATTENTION, qkv, att, ksize=heads, name=f"{p}.ma(attention)"))
+            x1 = _View(self.buf(f"{p}.x1", div, E), 0, E)
+            self.conv(f"{p}.ma.out_proj", w4(ma.out_proj.weight.detach().double()), ma.out_proj.bias.detach().double(),
+                      att, x1, 1, 1, 0, _C.YB_ACT_NONE, residual=x, ref_flops_per_pixel=2 * E * E)
+            out = dst if i == n - 1 else _View(self.buf(f"{p}.y", div, E), 0, E)
+            w_fc = layer.fc2.weight.detach().double() @ layer.fc1.weight.detach().double()
+            self.conv(f"{p}.fc2*fc1", w4(w_fc), torch.zeros(E, dtype=torch.float64, device=W.device), x1, out, 1, 1, 0,
+                      _C.YB_ACT_NONE, residual=x1, ref_flops_per_pixel=4 * E * E)
+            x = out
 
     def spp(self, name, m: SPP, src: _View, dst: _View):
         if tuple(m.k) != (5, 9, 13):
@@ -574,6 +641,8 @@ class PlanInstance:
                 if op.band:
                     d.Cin_pad = 64     # [Cout_pad, 3, 2 x 64] banded stem matrix: one 64-channel chunk of super-pixels
             d.reserved = (1 if op.force_im2col else 0) | (2 if op.band else 0) | (8 if no_nsplit else 0)
+            if op.kind == _C.YB_OP_ATTENTION:
+                d.reserved = 0        # heads travel in ksize; the attention op has no option bits
             if op.residual is not None:
                 d.residual, d.res_cstride = ptr(op.residual), op.residual.buf.C
             return d
@@ -637,6 +706,9 @@ class PlanInstance:
             d = make_desc(op, ptr)
             name = op.name
             flops = N * (H // op.dst.buf.div) * (W // op.dst.buf.div // op.pack) * op.flops_per_pixel if op.kind == _C.YB_OP_CONV else 0
+            if op.kind == _C.YB_OP_ATTENTION:   # Q K^T and P V: 4 L E per token
+                tokens = (H // op.dst.buf.div) * (W // op.dst.buf.div)
+                flops = N * tokens * 4 * tokens * op.dst.C
             if len(grp) == 2:
                 tail = L.ops[grp[1]]
                 c = make_chain(op, tail, ptr)

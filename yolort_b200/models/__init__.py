@@ -1,11 +1,13 @@
-"""Model constructors with the reference's names and kwargs (yolort/models/__init__.py:24-185), plus
+"""Model constructors with the reference's names and kwargs (yolort/models/__init__.py:24-185, `yolov5ts` at
+:169-185), plus
 `yolov5x`, which the reference defines as an architecture (yolo.py:592-619) but does not export."""
 from typing import Any
 
 from .yolo import YOLO
 from .yolov5 import YOLOv5
 
-__all__ = ["YOLO", "YOLOv5", "yolov5n", "yolov5s", "yolov5m", "yolov5l", "yolov5x", "yolov5n6", "yolov5s6", "yolov5m6"]
+__all__ = ["YOLO", "YOLOv5", "yolov5n", "yolov5s", "yolov5m", "yolov5l", "yolov5x", "yolov5n6", "yolov5s6", "yolov5m6",
+           "yolov5ts"]
 
 
 def _make(size: str, p6: bool = False):
@@ -37,3 +39,15 @@ yolov5x = _make("x")
 yolov5n6 = _make("n", p6=True)
 yolov5s6 = _make("s", p6=True)
 yolov5m6 = _make("m", p6=True)
+
+
+def yolov5ts(upstream_version: str = "r4.0", export_friendly: bool = False, **kwargs: Any) -> YOLOv5:
+    """yolov5s r4.0 with a transformer block in the neck (models/__init__.py:169-185).
+
+    Args:
+        upstream_version (str): "r4.0", the only release the reference builds it for.
+        export_friendly (bool): accepted for signature compatibility; there is no export path here.
+    """
+    if upstream_version != "r4.0":
+        raise NotImplementedError("Currently only supports r4.0 versions")
+    return YOLOv5(arch="yolov5_darknet_tan_s_r40", **kwargs)

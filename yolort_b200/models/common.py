@@ -2,7 +2,7 @@
 
 These modules reproduce the parameter/buffer names of the reference blocks
 (yolort/v5/models/common.py:42-73 Conv, :94-116 Bottleneck, :119-146 BottleneckCSP, :149-173 C3, :176-187 SPP,
-:210-234 Focus) so that a
+:210-234 Focus, :308-367 TransformerLayer / TransformerBlock / C3TR) so that a
 reference `state_dict` loads unchanged.  They do not compute: the arithmetic of the whole
 backbone is executed by the sm_90a execution plan (yolort_b200/engine.py -> libyolort_b200.so).
 Calling `forward` on a block is an error by design -- there is no PyTorch/CPU fallback.
@@ -99,3 +99,40 @@ class Focus(_PlanOnly):
     def __init__(self, c1: int, c2: int, k: int = 1, s: int = 1, p=None, version: str = "r4.0"):
         super().__init__()
         self.conv = Conv(c1 * 4, c2, k, s, p, version=version)
+
+
+class TransformerLayer(_PlanOnly):
+    """common.py:308-331: x = ma(q(x), k(x), v(x)) + x; x = fc2(fc1(x)) + x (no LayerNorm, no activation).  `ma` is
+    nn.MultiheadAttention held for its parameters only (in_proj_weight [3c, c], in_proj_bias, out_proj)."""
+
+    def __init__(self, c: int, num_heads: int):
+        super().__init__()
+        self.q = nn.Linear(c, c, bias=False)
+        self.k = nn.Linear(c, c, bias=False)
+        self.v = nn.Linear(c, c, bias=False)
+        self.ma = nn.MultiheadAttention(embed_dim=c, num_heads=num_heads)
+        self.fc1 = nn.Linear(c, c, bias=False)
+        self.fc2 = nn.Linear(c, c, bias=False)
+
+
+class TransformerBlock(_PlanOnly):
+    """common.py:334-357: optional Conv when c1 != c2, learnable position embedding p + linear(p), then the layers,
+    over the H*W tokens of each image (row-major pixel order)."""
+
+    def __init__(self, c1: int, c2: int, num_heads: int, num_layers: int):
+        super().__init__()
+        self.conv = None
+        if c1 != c2:
+            self.conv = Conv(c1, c2)
+        self.linear = nn.Linear(c2, c2)
+        self.tr = nn.Sequential(*[TransformerLayer(c2, num_heads) for _ in range(num_layers)])
+        self.c2 = c2
+
+
+class C3TR(C3):
+    """common.py:360-367: C3 whose bottlenecks are replaced by TransformerBlock(c_, c_, 4 heads, n layers)."""
+
+    def __init__(self, c1: int, c2: int, n: int = 1, shortcut: bool = True, e: float = 0.5):
+        super().__init__(c1, c2, n, shortcut, e)
+        c_ = int(c2 * e)
+        self.m = TransformerBlock(c_, c_, 4, n)

@@ -15,6 +15,7 @@ from .. import _C
 from .anchor_utils import AnchorGenerator
 from .backbone_utils import darknet_pan_backbone
 from .box_head import PostProcess, YOLOHead
+from .transformer import darknet_tan_backbone
 
 __all__ = [
     "YOLO",
@@ -34,6 +35,7 @@ __all__ = [
     "yolov5_darknet_pan_m6_r60",
     "yolov5_darknet_pan_l6_r60",
     "yolov5_darknet_pan_x6_r60",
+    "yolov5_darknet_tan_s_r40",
 ]
 
 DEFAULT_STRIDES = [8, 16, 32]
@@ -316,3 +318,16 @@ yolov5_darknet_pan_s6_r60 = _factory("s", 0.33, 0.5, use_p6=True)
 yolov5_darknet_pan_m6_r60 = _factory("m", 0.67, 0.75, use_p6=True)
 yolov5_darknet_pan_l6_r60 = _factory("l", 1.0, 1.0, use_p6=True)
 yolov5_darknet_pan_x6_r60 = _factory("x", 1.33, 1.25, use_p6=True)
+
+
+def yolov5_darknet_tan_s_r40(pretrained: bool = False, progress: bool = True, num_classes: int = 80,
+                             **kwargs: Any) -> YOLO:
+    """yolov5 small r4.0 with a transformer block (C3TR) as the first block of the neck (yolort/models/yolo.py:837-862,
+    yolort/models/transformer.py)."""
+    backbone = darknet_tan_backbone("darknet_s_r4_0", 0.33, 0.5, version="r4.0")
+    model = YOLO(backbone, num_classes, **kwargs)
+    if pretrained:
+        raise ValueError(
+            "No checkpoint is available offline for model yolov5_darknet_tan_s_r40_coco; load a converted state_dict "
+            "with model.load_state_dict(...)")
+    return model
