@@ -89,11 +89,14 @@ int yb_scale_coords_params(int Hb, int Wb, int src_h, int src_w, float* out3);
 #define YB_OP_SPP_POOL 1   /* y[c:2c]=mp5(x) y[2c:3c]=mp9(x) y[3c:4c]=mp13(x), stride 1, -inf pad */
 #define YB_OP_UPSAMPLE2X 2 /* nearest x2 (nn.Upsample(scale_factor=2))                            */
 #define YB_OP_ATTENTION 3  /* multi-head softmax(Q_h K_h^T / sqrt(d)) V_h over the H*W tokens of each image  */
+#define YB_OP_DWCONV 4     /* depthwise k x k convolution, one group per channel (MobileNetV3 InvertedResidual)  */
+#define YB_OP_SE 5         /* in-place squeeze-excitation x <- x * hardsigmoid(W2 relu(W1 mean_hw(x) + b1) + b2)  */
 
 #define YB_ACT_NONE 0
 #define YB_ACT_SILU 1
 #define YB_ACT_HARDSWISH 2 /* r3.1 Conv (yolort/v5/models/common.py:64)              */
 #define YB_ACT_LEAKY01 3   /* r3.1 BottleneckCSP: LeakyReLU(0.1) after the concat BN (:141-142) */
+#define YB_ACT_RELU 4      /* MobileNetV3 "RE" blocks (torchvision mobilenetv3.py)              */
 
 /* Optional fused post-processing of a detection-head convolution (yolort/models/box_head.py:68-82 followed by
  * :328-360,418): instead of storing the logits, the epilogue applies sigmoid / anchor decode / multi-label
@@ -149,6 +152,28 @@ typedef struct {
  *   pad and res_cstride are not read.
  * The op computes softmax(Q_h K_h^T / sqrt(d)) V_h for every image and head, with no mask, fp32 softmax and
  * accumulation.  Channel counts and strides must be multiples of 8 and both tensors 16-byte aligned. */
+/* YB_OP_DWCONV (the depthwise convolution of torchvision's InvertedResidual, yolort/models/yolo_lite.py:74-105; also
+ * the stride-2 subsample of the FPN's LastLevelMaxPool, as ksize 1 with unit weights) reads the fields as follows:
+ *   in, out:   NHWC views with Cin == Cout == C, C and both cstrides multiples of 8
+ *   ksize, stride, pad:  ksize in {1, 3, 5}, stride in {1, 2}, pad == ksize / 2, zero padding;
+ *              Ho == (H + 2 pad - ksize) / stride + 1, Wo likewise
+ *   act:       YB_ACT_NONE, YB_ACT_RELU or YB_ACT_HARDSWISH
+ *   weight:    [ksize * ksize][C] in the compute dtype (tap-major, channels contiguous; BN folded)
+ *   bias:      [C] fp32
+ *   residual, decode and chain must be NULL, reserved 0; Cin_pad, Cout_pad and res_cstride are not read.
+ * out[n,y,x,c] = act(sum_ij w[i*k+j][c] * in[n, y*s-p+i, x*s-p+j, c] + b[c]), fp32 accumulation, one rounding.
+ * in, out and weight must be 16-byte aligned, bias 4-byte aligned.
+ *
+ * YB_OP_SE (torchvision.ops.SqueezeExcitation inside InvertedResidual) works in place and reads the fields as follows:
+ *   in, out:   the same NHWC view (in == out, in_cstride == out_cstride), Cin == Cout == C, C <= 2048 a multiple of 8;
+ *              Ho == H, Wo == W
+ *   ksize:     the squeeze width S (fc1: C -> S, fc2: S -> C), 1 <= S <= 1024
+ *   weight:    fp32 [C][S] (W1 transposed: fc1.weight[s][c] at [c*S + s]) followed by fp32 [S][C] (W2 transposed:
+ *              fc2.weight[c][s] at [C*S + s*C + c])
+ *   bias:      fp32 [S] (fc1.bias) followed by fp32 [C] (fc2.bias)
+ *   act, stride and pad are not read; residual, decode and chain must be NULL, reserved 0.
+ * Per image: m = mean_hw(x) in fp32, g = hardsigmoid(W2 relu(W1 m + b1) + b2), x <- round(x * g).  The mean is summed
+ * in a fixed order without atomics (a repeated run gives the same bits).  weight and bias must be 16-byte aligned. */
 typedef struct {
   int32_t kind;
   int32_t dtype;                /* YB_F16 or YB_BF16 (accumulation is always fp32) */

@@ -71,6 +71,10 @@ extern "C" int yb_plan_create(const yb_op_desc* ops, int n_ops, yb_plan** plan_o
       }
     } else if (ops[i].kind == YB_OP_ATTENTION) {
       rc = attention_op_create(ops[i], &st.attn);   // validates before any driver call
+    } else if (ops[i].kind == YB_OP_DWCONV) {
+      rc = dwconv_configure_check(ops[i]);
+    } else if (ops[i].kind == YB_OP_SE) {
+      rc = se_configure_check(ops[i]);
     } else if (ops[i].kind == YB_OP_SPP_POOL || ops[i].kind == YB_OP_UPSAMPLE2X) {
       rc = validate_pool_or_upsample(ops[i]);
     } else {
@@ -105,6 +109,12 @@ extern "C" int yb_plan_run_range(yb_plan* plan, int first, int count, void* stre
         break;
       case YB_OP_ATTENTION:
         rc = attention_op_launch(st.attn, stream);
+        break;
+      case YB_OP_DWCONV:
+        rc = dwconv_launch(st.desc, stream);
+        break;
+      case YB_OP_SE:
+        rc = se_launch(st.desc, stream);
         break;
       case YB_OP_SPP_POOL:
         rc = spp_pool_launch(st.desc, stream);

@@ -66,7 +66,7 @@ struct FragRows {
   bool ok[2];
 };
 
-// bias -> activation (SiLU / linear, or the r3.1 Hardswish / LeakyReLU(0.1)) -> + shortcut, in fp32
+// bias -> activation (SiLU / linear, the r3.1 Hardswish / LeakyReLU(0.1), or MobileNetV3's ReLU) -> + shortcut, in fp32
 template <bool kBf16>
 __device__ __forceinline__ uint32_t epilogue_pair(const EpilogueParams& p, float v0, float v1, long long row, bool row_ok,
                                                   int gcol) {
@@ -76,9 +76,12 @@ __device__ __forceinline__ uint32_t epilogue_pair(const EpilogueParams& p, float
   } else if (p.act == YB_ACT_HARDSWISH) {
     v0 = v0 * fminf(fmaxf(v0 + 3.0f, 0.f), 6.0f) * (1.0f / 6.0f);
     v1 = v1 * fminf(fmaxf(v1 + 3.0f, 0.f), 6.0f) * (1.0f / 6.0f);
-  } else if (p.act == YB_ACT_LEAKY01) {
-    v0 = v0 > 0.f ? v0 : v0 * 0.1f;
-    v1 = v1 > 0.f ? v1 : v1 * 0.1f;
+  } else if (p.act >= YB_ACT_LEAKY01) {
+    // LeakyReLU(0.1) and ReLU as max(v, slope * v) with slope 0.1 or 0 (ReLU of a negative input gives -0, which
+    // equals 0).  One shared branch: a branch of its own, or a select per element, measurably slows every instance.
+    const float slope = p.act == YB_ACT_LEAKY01 ? 0.1f : 0.f;
+    v0 = fmaxf(v0, v0 * slope);
+    v1 = fmaxf(v1, v1 * slope);
   }
   if (p.residual != nullptr && row_ok && gcol < p.Cout) {   // Cout % 8 == 0: a pair never straddles it
     const uint16_t* r = reinterpret_cast<const uint16_t*>(p.residual) + row * p.res_cstride + gcol;

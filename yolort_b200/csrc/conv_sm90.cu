@@ -490,7 +490,7 @@ static int conv_configure(const yb_op_desc& d, ConvKernelParams& kp, dim3& grid,
   YB_REQUIRE(d.dtype == YB_F16 || d.dtype == YB_BF16, "conv: dtype must be f16 or bf16");
   YB_REQUIRE((d.reserved & ~15) == 0, "conv: reserved bits 4 and up must be zero, got 0x%x", d.reserved);
   YB_REQUIRE(d.ksize >= 1 && d.ksize <= 7 && d.stride >= 1 && d.stride <= 2, "conv: ksize/stride");
-  YB_REQUIRE(d.act >= YB_ACT_NONE && d.act <= YB_ACT_LEAKY01, "conv: unknown activation %d", d.act);
+  YB_REQUIRE(d.act >= YB_ACT_NONE && d.act <= YB_ACT_RELU, "conv: unknown activation %d", d.act);
   YB_REQUIRE(d.Cin % 8 == 0 && d.in_cstride % 8 == 0 && d.in_cstride >= d.Cin,
              "conv: Cin/in_cstride must be multiples of 8 (16-byte TMA granularity), got %d/%d", d.Cin,
              d.in_cstride);

@@ -35,6 +35,12 @@ int attention_op_create(const yb_op_desc& d, AttentionOp** out);
 int attention_op_launch(const AttentionOp* op, cudaStream_t stream);
 void attention_op_destroy(AttentionOp* op);
 
+// MobileNetV3 depthwise convolution and squeeze-excitation (mobilenet_sm90.cu)
+int dwconv_configure_check(const yb_op_desc& d);      // host-only validation (no driver calls)
+int dwconv_launch(const yb_op_desc& d, cudaStream_t stream);
+int se_configure_check(const yb_op_desc& d);          // host-only validation (no driver calls)
+int se_launch(const yb_op_desc& d, cudaStream_t stream);
+
 // HBM-bound helpers of the neck (pool_upsample.cu)
 int spp_pool_launch(const yb_op_desc& d, cudaStream_t stream);
 int upsample2x_launch(const yb_op_desc& d, cudaStream_t stream);

@@ -95,6 +95,8 @@ def act_code(act: nn.Module) -> int:
         return _C.YB_ACT_SILU
     if isinstance(act, nn.Hardswish):
         return _C.YB_ACT_HARDSWISH
+    if isinstance(act, nn.ReLU):
+        return _C.YB_ACT_RELU
     if isinstance(act, nn.Identity):
         return _C.YB_ACT_NONE
     raise NotImplementedError(f"no epilogue for activation {type(act).__name__}")
@@ -124,6 +126,21 @@ def stem_to_s2d(w: torch.Tensor) -> torch.Tensor:
                 for dx in range(2):
                     q = (dy * 2 + dx) * 4
                     out[:, q:q + 3, a, b] = w[:, :, 2 * a + dy, 2 * b + dx]
+    return out
+
+
+def stem_s2_to_s2d(w: torch.Tensor) -> torch.Tensor:
+    """[Co,3,3,3] stride-2 pad-1 kernel -> [Co,16,3,3] stride-1 pad-1 kernel over the space-to-depth input whose channel
+    is (dy*2+dx)*4 + c (c == 3 is a zero channel).  Output pixel y reads input rows 2y-1+ky = 2(y-1+a)+dy, so the taps map
+    as ky=0 -> (a=0, dy=1), ky=1 -> (a=1, dy=0), ky=2 -> (a=1, dy=1), the same in x; the a=2 / b=2 taps stay zero."""
+    co = w.shape[0]
+    assert tuple(w.shape[1:]) == (3, 3, 3)
+    out = torch.zeros((co, 16, 3, 3), dtype=w.dtype, device=w.device)
+    tap = ((0, 1), (1, 0), (1, 1))
+    for ky, (a, dy) in enumerate(tap):
+        for kx, (b, dx) in enumerate(tap):
+            q = (dy * 2 + dx) * 4
+            out[:, q:q + 3, a, b] = w[:, :, ky, kx]
     return out
 
 
@@ -364,6 +381,69 @@ class _Lowering:
     def upsample(self, name, src: _View, dst: _View):
         self.ops.append(_Op(_C.YB_OP_UPSAMPLE2X, src, dst, name=name))
 
+    def dwconv(self, name, w, b, src: _View, dst: _View, k, s, act):
+        """Depthwise k x k / s convolution (YB_OP_DWCONV): w [C,1,k,k] (BN folded, fp64) -> [k*k][C] in the compute
+        dtype, b -> fp32 [C]."""
+        C = src.C
+        assert tuple(w.shape) == (C, 1, k, k) and dst.C == C, (name, tuple(w.shape), src.C, dst.C)
+        wp = w.reshape(C, k * k).t().contiguous().to(self.dtype).to(self.device)
+        bp = b.to(torch.float32).to(self.device).contiguous()
+        self.ops.append(_Op(_C.YB_OP_DWCONV, src, dst, k, s, k // 2, act, wp, bp, None, name, 2 * k * k * C))
+
+    def squeeze_excitation(self, name, m: nn.Module, x: _View):
+        """torchvision.ops.SqueezeExcitation (ops/misc.py): x * hardsigmoid(fc2(relu(fc1(mean_hw(x))))) in place
+        (YB_OP_SE).  fc1 / fc2 stay fp32 and unrounded, transposed so that the kernel reads them coalesced."""
+        if not (isinstance(m.activation, nn.ReLU) and isinstance(m.scale_activation, nn.Hardsigmoid)):
+            raise NotImplementedError(f"{name}: SE kernel implements relu / hardsigmoid")
+        S, C = m.fc1.out_channels, m.fc1.in_channels
+        assert C == x.C and m.fc2.out_channels == C and m.fc2.in_channels == S
+        w1t = m.fc1.weight.detach().reshape(S, C).t().float()
+        w2t = m.fc2.weight.detach().reshape(C, S).t().float()
+        w = torch.cat([w1t.reshape(-1), w2t.reshape(-1)]).to(self.device).contiguous()
+        b = torch.cat([m.fc1.bias.detach().float(), m.fc2.bias.detach().float()]).to(self.device).contiguous()
+        self.ops.append(_Op(_C.YB_OP_SE, x, x, ksize=S, weight=w, bias=b, name=name))
+
+    def conv_norm_act(self, name, m: nn.Sequential, src: _View, dst: _View, residual=None):
+        """torchvision Conv2dNormActivation: conv [-> FrozenBatchNorm2d] [-> activation], one group, BN folded in fp64
+        (scale = w * rsqrt(rv + eps), shift = b - rm * scale)."""
+        conv, bn, act = _split_conv_norm_act(name, m)
+        if conv.groups != 1:
+            raise NotImplementedError(f"{name}: grouped convolution outside the depthwise case")
+        w, b = _fold_conv_norm(conv, bn)
+        k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
+        self.conv(name, w, b, src, dst, k, s, p, act, residual)
+
+    def inverted_residual(self, name, m: nn.Module, src: _View) -> _View:
+        """torchvision InvertedResidual: [1x1 expand] -> depthwise k x k / s -> [SE] -> 1x1 project (no act)
+        [+ input when use_res_connect].  Every fact comes from the modules."""
+        from torchvision.ops import SqueezeExcitation
+
+        x = src
+        mods = list(m.block)
+        for j, sub in enumerate(mods):
+            sn = f"{name}.block.{j}"
+            if isinstance(sub, SqueezeExcitation):
+                self.squeeze_excitation(sn, sub, x)
+                continue
+            conv, bn, act = _split_conv_norm_act(sn, sub)
+            if conv.groups > 1:
+                if conv.groups != conv.in_channels or conv.out_channels != conv.in_channels:
+                    raise NotImplementedError(f"{sn}: grouped convolution that is not depthwise")
+                k, s = conv.kernel_size[0], conv.stride[0]
+                if conv.kernel_size != (k, k) or conv.stride != (s, s) or conv.padding != (k // 2, k // 2) \
+                        or conv.dilation != (1, 1):
+                    raise NotImplementedError(f"{sn}: depthwise kernel implements square k x k / s, pad k // 2")
+                w, b = _fold_conv_norm(conv, bn)
+                dst = _View(self.buf(sn, x.buf.div * s, x.C), 0, x.C)
+                self.dwconv(sn, w, b, x, dst, k, s, act)
+            else:
+                last = j == len(mods) - 1
+                co = conv.out_channels
+                dst = _View(self.buf(name if last else sn, x.buf.div, co), 0, co)
+                self.conv_norm_act(sn, sub, x, dst, residual=src if (last and m.use_res_connect) else None)
+            x = dst
+        return x
+
 
 def lower_yolo(model: nn.Module, dtype: torch.dtype, device: torch.device, stem_variant: str = "auto"):
     """Walk YOLO.backbone / YOLO.head and emit (lowering, input_buf, head_bufs, features).
@@ -483,6 +563,127 @@ def lower_yolo(model: nn.Module, dtype: torch.dtype, device: torch.device, stem_
     return L, x0, head_bufs, {f"p{l + 3}": r for l, r in enumerate(results)}
 
 
+def _split_conv_norm_act(name, m: nn.Sequential):
+    """(conv, norm or None, activation code) of a torchvision Conv2dNormActivation."""
+    mods = list(m)
+    conv = mods[0]
+    if not isinstance(conv, nn.Conv2d):
+        raise NotImplementedError(f"{name}: expected a Conv2dNormActivation, got {type(m).__name__}")
+    bn = None
+    act = _C.YB_ACT_NONE
+    for sub in mods[1:]:
+        if hasattr(sub, "running_var"):
+            bn = sub
+        else:
+            act = act_code(sub)
+    return conv, bn, act
+
+
+def _fold_conv_norm(conv: nn.Conv2d, bn) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Conv (optional bias) followed by an optional (Frozen)BatchNorm2d, folded in fp64."""
+    w = conv.weight.detach().double()
+    b = conv.bias.detach().double() if conv.bias is not None else torch.zeros(w.shape[0], dtype=torch.float64,
+                                                                                device=w.device)
+    if bn is None:
+        return w, b
+    scale, shift = bn_scale_shift(bn)
+    return w * scale.view(-1, 1, 1, 1), b * scale + shift
+
+
+def lower_lite(model: nn.Module, dtype: torch.dtype, device: torch.device):
+    """Walk a YOLO whose backbone is BackboneWithFPN (MobileNetV3 features + FPN, yolort/models/yolo_lite.py) and emit
+    (lowering, input_buf, head_bufs, features), like lower_yolo.
+
+      * stem: the 3x3/s2/p1 convolution is an exact 3x3/s1/p1 convolution over the space-to-depth canvas
+        (stem_s2_to_s2d), run over super-pixels of 4 (stem_superpixel);
+      * InvertedResidual: expand -> YB_OP_DWCONV -> YB_OP_SE (in place) -> project, the projection's residual being
+        the block input when use_res_connect;
+      * FPN (torchvision ops/feature_pyramid_network.py), coarsest level first: inner[i](x_i) takes `last` as its
+        residual when both sit at the same stride, and YB_OP_UPSAMPLE2X(last) when `last` is twice as coarse; the
+        LastLevelMaxPool level (max_pool2d(k=1, s=2)) is a ksize-1 stride-2 YB_OP_DWCONV with unit weights;
+      * the 1x1 head convolutions over "0", "1", "2" and "pool"."""
+    from torchvision.ops.feature_pyramid_network import LastLevelMaxPool
+
+    L = _Lowering(dtype, device)
+    bb = model.backbone
+    body, fpn = bb.body, bb.fpn
+    return_layers = dict(body.return_layers)
+    layers = list(body.named_children())
+    if len(model.head.head) != len(return_layers) + 1 or not isinstance(fpn.extra_blocks, LastLevelMaxPool):
+        raise NotImplementedError("lowering covers BackboneWithFPN with LastLevelMaxPool and one head per level")
+
+    x0 = L.buf("input.s2d", 2, 16)
+    name0, stem = layers[0]
+    conv, bn, act = _split_conv_norm_act(f"body.{name0}", stem)
+    if conv.kernel_size != (3, 3) or conv.stride != (2, 2) or conv.padding != (1, 1) or conv.in_channels != 3 \
+            or conv.groups != 1:
+        raise NotImplementedError("stem must be a 3x3/s2/p1 convolution over RGB")
+    w, b = _fold_conv_norm(conv, bn)
+    co = w.shape[0]
+    t0 = L.buf(f"body.{name0}", 2, co)
+    spk = 4
+    w_sp, b_sp = stem_superpixel(stem_s2_to_s2d(w), b, spk)
+    L.conv(f"body.{name0}(stem: 3x3/s2 as 3x3 over s2d super-pixels)", w_sp, b_sp, _View(x0, 0, 16), _View(t0, 0, co),
+           3, 1, 1, act, ref_flops_per_pixel=spk * 2 * co * 3 * 9, pack=spk)
+    cur = _View(t0, 0, co)
+    taps: Dict[str, _View] = {}
+    if name0 in return_layers:
+        taps[return_layers[name0]] = cur
+    for name, m in layers[1:]:
+        if hasattr(m, "use_res_connect"):
+            cur = L.inverted_residual(f"body.{name}", m, cur)
+        else:
+            c = _split_conv_norm_act(f"body.{name}", m)[0]
+            if c.kernel_size != (1, 1) or c.stride != (1, 1):
+                raise NotImplementedError(f"body.{name}: expected the closing 1x1 convolution")
+            dst = _View(L.buf(f"body.{name}", cur.buf.div, c.out_channels), 0, c.out_channels)
+            L.conv_norm_act(f"body.{name}", m, cur, dst)
+            cur = dst
+        if name in return_layers:
+            taps[return_layers[name]] = cur
+    xs = [taps[k] for k in sorted(taps, key=int)]
+
+    oc = bb.out_channels
+    inner, layer = fpn.inner_blocks, fpn.layer_blocks
+    nl = len(xs)
+    results: List[Optional[_View]] = [None] * nl
+    last = _View(L.buf(f"fpn.inner{nl - 1}", xs[-1].buf.div, oc), 0, oc)
+    L.conv_norm_act(f"fpn.inner_blocks.{nl - 1}", inner[nl - 1], xs[-1], last)
+    results[-1] = _View(L.buf(str(nl - 1), xs[-1].buf.div, oc), 0, oc)
+    L.conv_norm_act(f"fpn.layer_blocks.{nl - 1}", layer[nl - 1], last, results[-1])
+    for idx in range(nl - 2, -1, -1):
+        div = xs[idx].buf.div
+        if last.buf.div == div:          # F.interpolate to the same size: the identity
+            top_down = last
+        elif last.buf.div == 2 * div:
+            top_down = _View(L.buf(f"fpn.up{idx}", div, oc), 0, oc)
+            L.upsample(f"fpn.interpolate{idx}", last, top_down)
+        else:
+            raise NotImplementedError("FPN levels must be 1x or 2x apart")
+        new = _View(L.buf(f"fpn.inner{idx}", div, oc), 0, oc)
+        L.conv_norm_act(f"fpn.inner_blocks.{idx}", inner[idx], xs[idx], new, residual=top_down)
+        last = new
+        results[idx] = _View(L.buf(str(idx), div, oc), 0, oc)
+        L.conv_norm_act(f"fpn.layer_blocks.{idx}", layer[idx], last, results[idx])
+    pool = _View(L.buf("pool", 2 * results[-1].buf.div, oc), 0, oc)
+    ones = torch.ones((oc, 1, 1, 1), dtype=torch.float64)
+    L.dwconv("fpn.extra_blocks(max_pool2d k1 s2)", ones, torch.zeros(oc, dtype=torch.float64), results[-1], pool, 1, 2,
+             _C.YB_ACT_NONE)
+    feats = {str(i): r for i, r in enumerate(results)}
+    feats["pool"] = pool
+
+    head_bufs = []
+    for i, (key, hc) in enumerate(zip(list(feats), model.head.head)):
+        feat = feats[key]
+        co = hc.out_channels
+        co_buf = _round_up(co, 16)
+        hb = L.buf(f"head.{i}", feat.buf.div, co_buf)
+        L.conv(f"head.head.{i}", hc.weight.detach().double(), hc.bias.detach().double(), feat, _View(hb, 0, co_buf), 1,
+               1, 0, _C.YB_ACT_NONE)
+        head_bufs.append(hb)
+    return L, x0, head_bufs, feats
+
+
 # ---------------------------------------------------------------------------------------------------
 # plan instances
 # ---------------------------------------------------------------------------------------------------
@@ -491,7 +692,12 @@ class Lowered:
     once per Engine and shared by every PlanInstance (a plan adds only an activation arena and TMA descriptors)."""
 
     def __init__(self, model: nn.Module, dtype: torch.dtype, device: torch.device, stem_variant: str = "auto"):
-        self.L, self.x0, self.head_bufs, self.feats = lower_yolo(model, dtype, device, stem_variant)
+        from .models.yolo_lite import BackboneWithFPN
+
+        if isinstance(model.backbone, BackboneWithFPN):
+            self.L, self.x0, self.head_bufs, self.feats = lower_lite(model, dtype, device)
+        else:
+            self.L, self.x0, self.head_bufs, self.feats = lower_yolo(model, dtype, device, stem_variant)
         self.n_heads = len(self.head_bufs)
         self.weight_bytes = sum(op.weight.numel() * op.weight.element_size() + op.bias.numel() * 4
                                 for op in self.L.ops if op.weight is not None)
@@ -640,9 +846,11 @@ class PlanInstance:
                 d.Cout_pad, _, d.Cin_pad = op.weight.shape
                 if op.band:
                     d.Cin_pad = 64     # [Cout_pad, 3, 2 x 64] banded stem matrix: one 64-channel chunk of super-pixels
+            elif op.kind in (_C.YB_OP_DWCONV, _C.YB_OP_SE):
+                d.weight, d.bias = op.weight.data_ptr(), op.bias.data_ptr()
             d.reserved = (1 if op.force_im2col else 0) | (2 if op.band else 0) | (8 if no_nsplit else 0)
-            if op.kind == _C.YB_OP_ATTENTION:
-                d.reserved = 0        # heads travel in ksize; the attention op has no option bits
+            if op.kind in (_C.YB_OP_ATTENTION, _C.YB_OP_DWCONV, _C.YB_OP_SE):
+                d.reserved = 0        # these ops have no option bits
             if op.residual is not None:
                 d.residual, d.res_cstride = ptr(op.residual), op.residual.buf.C
             return d
@@ -705,7 +913,8 @@ class PlanInstance:
             op = L.ops[grp[0]]
             d = make_desc(op, ptr)
             name = op.name
-            flops = N * (H // op.dst.buf.div) * (W // op.dst.buf.div // op.pack) * op.flops_per_pixel if op.kind == _C.YB_OP_CONV else 0
+            flops = N * (H // op.dst.buf.div) * (W // op.dst.buf.div // op.pack) * op.flops_per_pixel \
+                if op.kind in (_C.YB_OP_CONV, _C.YB_OP_DWCONV) else 0
             if op.kind == _C.YB_OP_ATTENTION:   # Q K^T and P V: 4 L E per token
                 tokens = (H // op.dst.buf.div) * (W // op.dst.buf.div)
                 flops = N * tokens * 4 * tokens * op.dst.C

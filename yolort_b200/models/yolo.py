@@ -168,7 +168,10 @@ class YOLO(nn.Module):
     def run_head(self, features: List[Tensor]) -> List[Tensor]:
         """`head(features)`: the raw per-level logits [N, A, H, W, nc+5] (yolort/models/box_head.py:68-82); the same
         list in training and eval mode."""
-        s0 = int(self.anchor_generator.strides[0])
+        # the canvas is the first feature map times its divisor in the lowering (not strides[0]: the lite model's first
+        # map sits at stride 16 while its anchor generator says 8)
+        low = self.engine().lowered()
+        s0 = low.feats[min(low.feats)].buf.div
         N, _, h0, w0 = (int(v) for v in features[0].shape)
         plan = self.get_plan(N, h0 * s0, w0 * s0)
         keys = sorted(plan.features)
