@@ -91,6 +91,7 @@ int yb_scale_coords_params(int Hb, int Wb, int src_h, int src_w, float* out3);
 #define YB_OP_ATTENTION 3  /* multi-head softmax(Q_h K_h^T / sqrt(d)) V_h over the H*W tokens of each image  */
 #define YB_OP_DWCONV 4     /* depthwise k x k convolution, one group per channel (MobileNetV3 InvertedResidual)  */
 #define YB_OP_SE 5         /* in-place squeeze-excitation x <- x * hardsigmoid(W2 relu(W1 mean_hw(x) + b1) + b2)  */
+#define YB_OP_AVGPOOL 6    /* global average pool y[n,0,0,c] = mean_hw(x[n,:,:,c]) (nn.AdaptiveAvgPool2d(1))       */
 
 #define YB_ACT_NONE 0
 #define YB_ACT_SILU 1
@@ -173,7 +174,16 @@ typedef struct {
  *   bias:      fp32 [S] (fc1.bias) followed by fp32 [C] (fc2.bias)
  *   act, stride and pad are not read; residual, decode and chain must be NULL, reserved 0.
  * Per image: m = mean_hw(x) in fp32, g = hardsigmoid(W2 relu(W1 m + b1) + b2), x <- round(x * g).  The mean is summed
- * in a fixed order without atomics (a repeated run gives the same bits).  weight and bias must be 16-byte aligned. */
+ * in a fixed order without atomics (a repeated run gives the same bits).  weight and bias must be 16-byte aligned.
+ *
+ * YB_OP_AVGPOOL (the AdaptiveAvgPool2d(1) of the DarkNet classifiers, yolort/models/darknetv4.py, darknetv6.py) reads
+ * the fields as follows:
+ *   in, out:   NHWC views with Cin == Cout == C, C and both cstrides multiples of 8; N <= 65535
+ *   Ho, Wo:    1 (the output view holds one pixel per image: out[n*out_cstride + c])
+ *   weight, bias, residual, decode and chain must be NULL; act and reserved must be 0; ksize, stride, pad, Cin_pad,
+ *   Cout_pad and res_cstride are not read.
+ * out[n,0,0,c] = round(sum_{y,x} in[n,y,x,c] / (H*W)): the sum is fp32 in a fixed order without atomics (a repeated
+ * run gives the same bits), divided once and rounded once to the compute dtype.  in and out must be 16-byte aligned. */
 typedef struct {
   int32_t kind;
   int32_t dtype;                /* YB_F16 or YB_BF16 (accumulation is always fp32) */

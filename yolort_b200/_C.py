@@ -16,7 +16,7 @@ LIB_PATH = os.environ.get("YB_LIB_PATH") or os.path.join(_HERE, "libyolort_b200.
 
 YB_U8, YB_F16, YB_BF16, YB_F32 = 0, 1, 2, 3
 YB_LAYOUT_NCHW, YB_LAYOUT_S2D16 = 0, 1
-YB_OP_CONV, YB_OP_SPP_POOL, YB_OP_UPSAMPLE2X, YB_OP_ATTENTION, YB_OP_DWCONV, YB_OP_SE = 0, 1, 2, 3, 4, 5
+YB_OP_CONV, YB_OP_SPP_POOL, YB_OP_UPSAMPLE2X, YB_OP_ATTENTION, YB_OP_DWCONV, YB_OP_SE, YB_OP_AVGPOOL = 0, 1, 2, 3, 4, 5, 6
 YB_ACT_NONE, YB_ACT_SILU, YB_ACT_HARDSWISH, YB_ACT_LEAKY01, YB_ACT_RELU = 0, 1, 2, 3, 4
 YB_MAX_LEVELS, YB_MAX_ANCHORS = 4, 4
 NMS_TV_AUTO, NMS_EXACT_PER_CLASS, NMS_OFFSET_TRICK = 0, 1, 2

@@ -75,6 +75,8 @@ extern "C" int yb_plan_create(const yb_op_desc* ops, int n_ops, yb_plan** plan_o
       rc = dwconv_configure_check(ops[i]);
     } else if (ops[i].kind == YB_OP_SE) {
       rc = se_configure_check(ops[i]);
+    } else if (ops[i].kind == YB_OP_AVGPOOL) {
+      rc = avgpool_configure_check(ops[i]);
     } else if (ops[i].kind == YB_OP_SPP_POOL || ops[i].kind == YB_OP_UPSAMPLE2X) {
       rc = validate_pool_or_upsample(ops[i]);
     } else {
@@ -115,6 +117,9 @@ extern "C" int yb_plan_run_range(yb_plan* plan, int first, int count, void* stre
         break;
       case YB_OP_SE:
         rc = se_launch(st.desc, stream);
+        break;
+      case YB_OP_AVGPOOL:
+        rc = avgpool_launch(st.desc, stream);
         break;
       case YB_OP_SPP_POOL:
         rc = spp_pool_launch(st.desc, stream);

@@ -41,6 +41,10 @@ int dwconv_launch(const yb_op_desc& d, cudaStream_t stream);
 int se_configure_check(const yb_op_desc& d);          // host-only validation (no driver calls)
 int se_launch(const yb_op_desc& d, cudaStream_t stream);
 
+// global average pool of the classifiers (pool_global_sm90.cu)
+int avgpool_configure_check(const yb_op_desc& d);     // host-only validation (no driver calls)
+int avgpool_launch(const yb_op_desc& d, cudaStream_t stream);
+
 // HBM-bound helpers of the neck (pool_upsample.cu)
 int spp_pool_launch(const yb_op_desc& d, cudaStream_t stream);
 int upsample2x_launch(const yb_op_desc& d, cudaStream_t stream);

@@ -32,12 +32,19 @@ def _round_up(v: int, m: int) -> int:
     return (v + m - 1) // m * m
 
 
+GLOBAL = 0           # _Buf.div of a buffer with one pixel per image whatever the canvas (pooled vectors)
+
+
 @dataclass
 class _Buf:
     name: str
-    div: int          # spatial divisor w.r.t. the canvas
+    div: int          # spatial divisor w.r.t. the canvas, or GLOBAL
     C: int            # total channels (pixel stride)
     offset: int = 0   # byte offset in the arena
+
+    def hw(self, H: int, W: int) -> Tuple[int, int]:
+        """Spatial extent of this buffer on an H x W canvas."""
+        return (1, 1) if self.div == GLOBAL else (H // self.div, W // self.div)
 
 
 @dataclass
@@ -381,6 +388,73 @@ class _Lowering:
     def upsample(self, name, src: _View, dst: _View):
         self.ops.append(_Op(_C.YB_OP_UPSAMPLE2X, src, dst, name=name))
 
+    def stem(self, prefix: str, stem: nn.Module, stem_variant: str) -> Tuple[_Buf, _View]:
+        """The CSPDarknet stem over the plan's space-to-depth canvas: (canvas buffer, stem output view).  A Focus
+        (r3.1 / r4.0) is a channel permutation of the s2d input, the r6.0 6x6/s2/p2 convolution an exact 3x3/s1/p1
+        convolution over it."""
+        x0 = self.buf("input.s2d", 2, 16)
+        if isinstance(stem, Focus):       # r3.1 / r4.0: Focus = 2x2 space-to-depth + 3x3/s1/p1 conv (darknetv4.py:82)
+            stem = stem.conv
+            if stem.conv.kernel_size != (3, 3) or stem.conv.stride != (1, 1) or stem.conv.padding != (1, 1):
+                raise NotImplementedError("Focus stem must be the 3x3/s1/p1 convolution")
+            w, b = fold_conv_bn(stem)
+            w_s2d = focus_to_s2d(w)
+        else:                             # r6.0: 6x6/s2/p2 conv == 3x3/s1/p1 over the same space-to-depth input
+            if stem.conv.kernel_size != (6, 6) or stem.conv.stride != (2, 2) or stem.conv.padding != (2, 2):
+                raise NotImplementedError("stem must be the r6.0 6x6/s2/p2 convolution")
+            w, b = fold_conv_bn(stem)
+            w_s2d = stem_to_s2d(w)
+        co = w.shape[0]
+        t0 = self.buf(f"{prefix}.0", 2, co)
+        # The stem runs over "super-pixels" of 4 horizontally adjacent s2d pixels (128-byte TMA rows instead of 32).  Its
+        # expanded weight matrix is block-banded, and when the band (6 slabs of 4*Cout x 64) fits in shared memory next
+        # to two patches (4*Cout <= 128: yolov5n / s) the banded kernel variant multiplies only the band; wider stems
+        # (m / l / x) use the dense super-pixel form.
+        spk = 4
+        co4 = spk * co
+        if stem_variant == "band" or (stem_variant == "auto" and co4 % 64 == 0 and co4 <= 128
+                                      and act_code(stem.act) in (_C.YB_ACT_SILU, _C.YB_ACT_NONE)):
+            w_b, b_b = stem_band(w_s2d, b)
+            self.conv_band(f"{prefix}.0(stem: banded 3x3 over s2d super-pixels)", w_b, b_b, _View(x0, 0, 16),
+                           _View(t0, 0, co), act_code(stem.act), ref_flops_per_pixel=spk * 2 * co * 3 * 36)
+        else:
+            w_sp, b_sp = stem_superpixel(w_s2d, b, spk)
+            self.conv(f"{prefix}.0(stem: 3x3 over s2d super-pixels)", w_sp, b_sp, _View(x0, 0, 16), _View(t0, 0, co),
+                      3, 1, 1, act_code(stem.act), ref_flops_per_pixel=spk * 2 * co * 3 * 36, pack=spk,
+                      force_im2col=(stem_variant == "im2col"))
+        return x0, _View(t0, 0, co)
+
+    def stages(self, prefix: str, mods: List[nn.Module], cur: _View, tap_dst: Dict[int, _View]) -> _View:
+        """Modules 1.. of a CSPDarknet body after the stem: 3x3/s2 Convs, blocks (C3 / BottleneckCSP) and the closing
+        SPP of r3.1 / r4.0.  Module i writes into tap_dst[i] when given (a concat window of the neck).  Returns the
+        last output."""
+        div = cur.buf.div
+        for i, m in enumerate(mods, start=1):
+            name = f"{prefix}.{i}"
+            if isinstance(m, Conv):
+                div *= 2
+                co = m.conv.out_channels
+                t = self.buf(name, div, co)
+                self.conv_module(name, m, cur, _View(t, 0, co))
+                cur = _View(t, 0, co)
+            elif isinstance(m, SPP):      # r3.1 / r4.0 keep the SPP as the last body module (darknetv4.py:97)
+                co = m.cv2.conv.out_channels
+                dst = _View(self.buf(name, div, co), 0, co)
+                self.spp(name, m, cur, dst)
+                cur = dst
+            else:
+                if not isinstance(m, (C3, BottleneckCSP)):
+                    raise NotImplementedError(f"{name}: no lowering for {type(m).__name__}")
+                co = (m.cv3 if isinstance(m, C3) else m.cv4).conv.out_channels
+                dst = tap_dst.get(i) or _View(self.buf(name, div, co), 0, co)
+                assert dst.C == co
+                self.block(name, m, cur, dst)
+                cur = dst
+        return cur
+
+    def avgpool(self, name, src: _View, dst: _View):
+        self.ops.append(_Op(_C.YB_OP_AVGPOOL, src, dst, name=name))
+
     def dwconv(self, name, w, b, src: _View, dst: _View, k, s, act):
         """Depthwise k x k / s convolution (YB_OP_DWCONV): w [C,1,k,k] (BN folded, fp64) -> [k*k][C] in the compute
         dtype, b -> fp32 [C]."""
@@ -457,36 +531,7 @@ def lower_yolo(model: nn.Module, dtype: torch.dtype, device: torch.device, stem_
     if nl not in (3, 4) or len(model.head.head) != nl or has_p6 != (nl == 4):
         raise NotImplementedError("lowering covers the r6.0 topologies: 3 levels, or 4 levels with the P6 block")
 
-    x0 = L.buf("input.s2d", 2, 16)
-    stem = body["0"]
-    if isinstance(stem, Focus):       # r3.1 / r4.0: Focus = 2x2 space-to-depth + 3x3/s1/p1 conv (darknetv4.py:82)
-        stem = stem.conv
-        if stem.conv.kernel_size != (3, 3) or stem.conv.stride != (1, 1) or stem.conv.padding != (1, 1):
-            raise NotImplementedError("Focus stem must be the 3x3/s1/p1 convolution")
-        w, b = fold_conv_bn(stem)
-        w_s2d = focus_to_s2d(w)
-    else:                             # r6.0: 6x6/s2/p2 conv == 3x3/s1/p1 over the same space-to-depth input
-        if stem.conv.kernel_size != (6, 6) or stem.conv.stride != (2, 2) or stem.conv.padding != (2, 2):
-            raise NotImplementedError("stem must be the r6.0 6x6/s2/p2 convolution")
-        w, b = fold_conv_bn(stem)
-        w_s2d = stem_to_s2d(w)
-    t0 = L.buf("body.0", 2, w.shape[0])
-    # The stem runs over "super-pixels" of 4 horizontally adjacent s2d pixels (128-byte TMA rows instead of 32).  Its
-    # expanded weight matrix is block-banded, and when the band (6 slabs of 4*Cout x 64) fits in shared memory next to
-    # two patches (4*Cout <= 128: yolov5n / s) the banded kernel variant multiplies only the band; wider stems
-    # (m / l / x) use the dense super-pixel form.
-    spk = 4
-    co4 = spk * w.shape[0]
-    if stem_variant == "band" or (stem_variant == "auto" and co4 % 64 == 0 and co4 <= 128
-                                  and act_code(stem.act) in (_C.YB_ACT_SILU, _C.YB_ACT_NONE)):
-        w_b, b_b = stem_band(w_s2d, b)
-        L.conv_band("body.0(stem: banded 3x3 over s2d super-pixels)", w_b, b_b, _View(x0, 0, 16), _View(t0, 0, w.shape[0]),
-                    act_code(stem.act), ref_flops_per_pixel=spk * 2 * w.shape[0] * 3 * 36)
-    else:
-        w_sp, b_sp = stem_superpixel(w_s2d, b, spk)
-        L.conv("body.0(stem: 3x3 over s2d super-pixels)", w_sp, b_sp, _View(x0, 0, 16), _View(t0, 0, w.shape[0]), 3, 1, 1,
-               act_code(stem.act), ref_flops_per_pixel=spk * 2 * w.shape[0] * 3 * 36, pack=spk,
-               force_im2col=(stem_variant == "im2col"))
+    x0, stem_out = L.stem("body", body["0"], stem_variant)
 
     # Concat buffers of the neck (path_aggregation_network.py:215-237), level l at stride 8 << l:
     #   cat_dn[l] = [up(lateral from level l+1) | body tap of level l]   (descending pass, l < nl-1)
@@ -496,29 +541,8 @@ def lower_yolo(model: nn.Module, dtype: torch.dtype, device: torch.device, stem_
     cat_dn = {l: L.buf(f"pan.cat{nl - 1 - l}[up(lat{nl - 1 - l})|f{taps[l]}]", 8 << l, 2 * ch[l]) for l in range(nl - 1)}
     cat_up = {l: L.buf(f"pan.cat_p{l + 3}[down(p{l + 2})|lat{nl - l}]", 8 << l, 2 * ch[l - 1]) for l in range(1, nl)}
 
-    cur = _View(t0, 0, w.shape[0])
-    div = 2
     tap_dst = {taps[l]: _View(cat_dn[l], ch[l], ch[l]) for l in range(min(nl - 1, 3))}
-    for i in range(1, 9):
-        m = body[str(i)]
-        if isinstance(m, Conv):
-            div *= 2
-            co = m.conv.out_channels
-            t = L.buf(f"body.{i}", div, co)
-            L.conv_module(f"body.{i}", m, cur, _View(t, 0, co))
-            cur = _View(t, 0, co)
-        elif isinstance(m, SPP):      # r3.1 / r4.0 keep the SPP as the last body module (darknetv4.py:97)
-            co = m.cv2.conv.out_channels
-            dst = _View(L.buf(f"body.{i}", div, co), 0, co)
-            L.spp(f"body.{i}", m, cur, dst)
-            cur = dst
-        else:
-            co = (m.cv3 if isinstance(m, C3) else m.cv4).conv.out_channels
-            dst = tap_dst.get(i) or _View(L.buf(f"body.{i}", div, co), 0, co)
-            assert dst.C == co
-            L.block(f"body.{i}", m, cur, dst)
-            cur = dst
-    top = cur
+    top = L.stages("body", [body[str(i)] for i in range(1, 9)], stem_out, tap_dst)
     if has_p6:   # IntermediateLevelP6 (path_aggregation_network.py:34-41): stride-64 level from the last tap
         p6m = pan.intermediate_blocks.p6
         t = _View(L.buf("pan.p6.conv", 64, ch[3]), 0, ch[3])
@@ -684,6 +708,41 @@ def lower_lite(model: nn.Module, dtype: torch.dtype, device: torch.device):
     return L, x0, head_bufs, feats
 
 
+def lower_darknet(model: nn.Module, dtype: torch.dtype, device: torch.device, stem_variant: str = "auto"):
+    """Walk a DarkNetV4 / DarkNetV6 classifier (yolort/models/darknetv4.py:33-136, darknetv6.py:31-127) and emit
+    (lowering, input_buf, head_bufs, features), like lower_yolo.
+
+      * features: the stem and stages of the detection body (_Lowering.stem / stages), ending at stride 32;
+      * avgpool: YB_OP_AVGPOOL into a GLOBAL buffer (one pixel per image);
+      * classifier.0 + Hardswish: a 1x1 YB_OP_CONV over the [N,1,1,C] map (M = N rows) with the Hardswish epilogue;
+        Dropout is the identity in eval mode and emits nothing;
+      * classifier.3: a 1x1 YB_OP_CONV whose output channels are zero-padded to a multiple of 8 (callers slice
+        [:, :num_classes]).
+    `features` holds the final feature map and the pooled vector, so that the sub-modules can run on their own."""
+    L = _Lowering(dtype, device)
+    mods = list(model.features)
+    x0, cur = L.stem("features", mods[0], stem_variant)
+    cur = L.stages("features", mods[1:], cur, {})
+    if cur.buf.div != 32:
+        raise NotImplementedError(f"the features must end at stride 32, got {cur.buf.div}")
+    cls = list(model.classifier)
+    if not (len(cls) == 4 and isinstance(cls[0], nn.Linear) and isinstance(cls[2], nn.Dropout)
+            and isinstance(cls[3], nn.Linear)):
+        raise NotImplementedError("classifier must be Linear -> activation -> Dropout -> Linear")
+    fc1, fc2 = cls[0], cls[3]
+    C, hid, nc = cur.C, fc1.out_features, fc2.out_features
+    pooled = _View(L.buf("avgpool", GLOBAL, C), 0, C)
+    L.avgpool("avgpool", cur, pooled)
+    hidden = _View(L.buf("classifier.0", GLOBAL, hid), 0, hid)
+    L.conv("classifier.0", fc1.weight.detach().double().view(hid, C, 1, 1), fc1.bias.detach().double(), pooled, hidden,
+           1, 1, 0, act_code(cls[1]))
+    ncb = _round_up(nc, 8)
+    logits = L.buf("classifier.3", GLOBAL, ncb)
+    L.conv("classifier.3", fc2.weight.detach().double().view(nc, hid, 1, 1), fc2.bias.detach().double(), hidden,
+           _View(logits, 0, ncb), 1, 1, 0, _C.YB_ACT_NONE)
+    return L, x0, [logits], {"features": cur, "avgpool": pooled}
+
+
 # ---------------------------------------------------------------------------------------------------
 # plan instances
 # ---------------------------------------------------------------------------------------------------
@@ -692,9 +751,12 @@ class Lowered:
     once per Engine and shared by every PlanInstance (a plan adds only an activation arena and TMA descriptors)."""
 
     def __init__(self, model: nn.Module, dtype: torch.dtype, device: torch.device, stem_variant: str = "auto"):
+        from .models._classifier import DarkNetClassifier
         from .models.yolo_lite import BackboneWithFPN
 
-        if isinstance(model.backbone, BackboneWithFPN):
+        if isinstance(model, DarkNetClassifier):
+            self.L, self.x0, self.head_bufs, self.feats = lower_darknet(model, dtype, device, stem_variant)
+        elif isinstance(model.backbone, BackboneWithFPN):
             self.L, self.x0, self.head_bufs, self.feats = lower_lite(model, dtype, device)
         else:
             self.L, self.x0, self.head_bufs, self.feats = lower_yolo(model, dtype, device, stem_variant)
@@ -728,7 +790,7 @@ def assign_offsets(L: _Lowering, x0: _Buf, keep: List[_Buf], N: int, H: int, W: 
         launches = [(i,) for i in range(len(L.ops))]
     step_of = {i: t for t, grp in enumerate(launches) for i in grp}
     n_ops = len(launches)          # time is counted in launches
-    size = {id(b): _round_up(N * (H // b.div) * (W // b.div) * b.C * esz, 1024) for b in L.bufs}
+    size = {id(b): _round_up(N * b.hw(H, W)[0] * b.hw(H, W)[1] * b.C * esz, 1024) for b in L.bufs}
     first = {id(b): n_ops for b in L.bufs}
     last = {id(b): -1 for b in L.bufs}
     first[id(x0)] = -1
@@ -811,7 +873,7 @@ class PlanInstance:
     def __init__(self, low: Lowered, N: int, H: int, W: int, post: Optional[dict] = None, keep_intermediates: bool = False,
                  chunked: bool = False, fuse_chains: bool = True):
         L, x0, head_bufs, feats = low.L, low.x0, low.head_bufs, low.feats
-        grain = max(b.div for b in L.bufs)
+        grain = max(b.div for b in L.bufs)          # GLOBAL buffers fit any canvas
         if H % grain or W % grain:
             raise ValueError(f"canvas {H}x{W} must be a multiple of {grain}")
         self.N, self.H, self.W = N, H, W
@@ -829,8 +891,8 @@ class PlanInstance:
 
         def make_desc(op: _Op, ptr) -> "_C.OpDesc":
             d = _C.OpDesc()
-            hi, wi = H // op.src.buf.div, W // op.src.buf.div
-            ho, wo = H // op.dst.buf.div, W // op.dst.buf.div
+            hi, wi = op.src.buf.hw(H, W)
+            ho, wo = op.dst.buf.hw(H, W)
             d.kind, d.dtype = op.kind, code
             k = op.pack
             if wi % k or wo % k:
@@ -849,7 +911,7 @@ class PlanInstance:
             elif op.kind in (_C.YB_OP_DWCONV, _C.YB_OP_SE):
                 d.weight, d.bias = op.weight.data_ptr(), op.bias.data_ptr()
             d.reserved = (1 if op.force_im2col else 0) | (2 if op.band else 0) | (8 if no_nsplit else 0)
-            if op.kind in (_C.YB_OP_ATTENTION, _C.YB_OP_DWCONV, _C.YB_OP_SE):
+            if op.kind in (_C.YB_OP_ATTENTION, _C.YB_OP_DWCONV, _C.YB_OP_SE, _C.YB_OP_AVGPOOL):
                 d.reserved = 0        # these ops have no option bits
             if op.residual is not None:
                 d.residual, d.res_cstride = ptr(op.residual), op.residual.buf.C
@@ -900,7 +962,7 @@ class PlanInstance:
                                         front_ops=front_ops, launches=launches)
         self.arena = torch.zeros((max(total, 1024),), dtype=torch.uint8, device=L.device)
         self.arena_bytes = total
-        self.unshared_bytes = sum(_round_up(N * (H // b.div) * (W // b.div) * b.C * esz, 1024) for b in L.bufs)
+        self.unshared_bytes = sum(_round_up(N * b.hw(H, W)[0] * b.hw(H, W)[1] * b.C * esz, 1024) for b in L.bufs)
         base = self.arena.data_ptr()
 
         def ptr(v: _View) -> int:
@@ -913,8 +975,8 @@ class PlanInstance:
             op = L.ops[grp[0]]
             d = make_desc(op, ptr)
             name = op.name
-            flops = N * (H // op.dst.buf.div) * (W // op.dst.buf.div // op.pack) * op.flops_per_pixel \
-                if op.kind in (_C.YB_OP_CONV, _C.YB_OP_DWCONV) else 0
+            ho, wo = op.dst.buf.hw(H, W)
+            flops = N * ho * (wo // op.pack) * op.flops_per_pixel if op.kind in (_C.YB_OP_CONV, _C.YB_OP_DWCONV) else 0
             if op.kind == _C.YB_OP_ATTENTION:   # Q K^T and P V: 4 L E per token
                 tokens = (H // op.dst.buf.div) * (W // op.dst.buf.div)
                 flops = N * tokens * 4 * tokens * op.dst.C
@@ -924,7 +986,7 @@ class PlanInstance:
                 self._chains.append(c)
                 d.chain = ctypes.addressof(c)
                 name = f"{op.name} -> {tail.name}"
-                flops += N * (H // tail.dst.buf.div) * (W // tail.dst.buf.div) * tail.flops_per_pixel
+                flops += N * tail.dst.buf.hw(H, W)[0] * tail.dst.buf.hw(H, W)[1] * tail.flops_per_pixel
             descs.append(d)
             self.op_names.append(name)
             self.op_flops.append(flops)
@@ -952,7 +1014,7 @@ class PlanInstance:
             self.plan_fused = _C.Plan(fused, L.device)
 
         def nhwc(b: _Buf) -> torch.Tensor:
-            h, w = H // b.div, W // b.div
+            h, w = b.hw(H, W)
             n = N * h * w * b.C
             o = offsets[id(b)]
             return self.arena[o: o + n * esz].view(L.dtype).view(N, h, w, b.C)

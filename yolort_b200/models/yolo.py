@@ -145,7 +145,8 @@ class YOLO(nn.Module):
         forward then goes stage by stage through the sub-modules' __call__ so that the hooks fire."""
         return any(m._forward_hooks or m._forward_pre_hooks for m in (self.backbone, self.head, self.post_process))
 
-    def _write_samples(self, plan, samples: Tensor) -> None:
+    @staticmethod
+    def _write_samples(plan, samples: Tensor) -> None:
         """A pre-letterboxed NCHW batch -> the plan's space-to-depth input (identity geometry)."""
         N, _, H, W = (int(v) for v in samples.shape)
         geoms = (_C.LetterboxGeom * N)()
