@@ -32,6 +32,7 @@ extern "C" {
 #define YB_F16 1
 #define YB_BF16 2
 #define YB_F32 3
+#define YB_F8E4M3 4 /* float8 e4m3 ("fn": max 448, no infinities); values are stored divided by a power-of-two scale */
 
 const char* yb_last_error(void);
 int yb_abi_version(void);
@@ -92,6 +93,7 @@ int yb_scale_coords_params(int Hb, int Wb, int src_h, int src_w, float* out3);
 #define YB_OP_DWCONV 4     /* depthwise k x k convolution, one group per channel (MobileNetV3 InvertedResidual)  */
 #define YB_OP_SE 5         /* in-place squeeze-excitation x <- x * hardsigmoid(W2 relu(W1 mean_hw(x) + b1) + b2)  */
 #define YB_OP_AVGPOOL 6    /* global average pool y[n,0,0,c] = mean_hw(x[n,:,:,c]) (nn.AdaptiveAvgPool2d(1))       */
+#define YB_OP_QUANTIZE 7   /* y = RN_satfinite(x / s) to e4m3, one power-of-two scale s per tensor (FP8 plans)      */
 
 #define YB_ACT_NONE 0
 #define YB_ACT_SILU 1
@@ -183,10 +185,34 @@ typedef struct {
  *   weight, bias, residual, decode and chain must be NULL; act and reserved must be 0; ksize, stride, pad, Cin_pad,
  *   Cout_pad and res_cstride are not read.
  * out[n,0,0,c] = round(sum_{y,x} in[n,y,x,c] / (H*W)): the sum is fp32 in a fixed order without atomics (a repeated
- * run gives the same bits), divided once and rounded once to the compute dtype.  in and out must be 16-byte aligned. */
+ * run gives the same bits), divided once and rounded once to the compute dtype.  in and out must be 16-byte aligned.
+ *
+ * FP8 (e4m3) plans.  An e4m3 tensor stores x / s for one power-of-two scale s per tensor (per output channel for conv
+ * weights); every conversion to e4m3 rounds to nearest even and saturates at +-448 (cvt.rn.satfinite: never a NaN).
+ * Channel counts, channel offsets and cstrides of e4m3 views are multiples of 16 (16 bytes), like every 16-byte view.
+ * YB_OP_CONV with dtype YB_F8E4M3 (the FP8 implicit-GEMM kernel) reads the fields as follows:
+ *   in, residual:  e4m3 NHWC views (scales s_in, s_res); Cin, in_cstride and res_cstride multiples of 16
+ *   out:       an e4m3 NHWC view (scale s_out), Cout and out_cstride multiples of 16; or, with reserved bit 4 (bit 5), an
+ *              fp16 (bf16) NHWC view, Cout and out_cstride multiples of 8, that gets the dequantised values (head logits)
+ *   ksize, stride, pad:  1x1/s1/p0, 3x3/s1/p1 or 3x3/s2/p1
+ *   act:       YB_ACT_NONE, SILU, HARDSWISH, LEAKY01 or RELU
+ *   weight:    e4m3 [Cout_pad][ksize*ksize][Cin_pad], Cin_pad a multiple of 32 (the K step), zero padded; row c holds
+ *              w[c] / s_w[c]
+ *   bias:      fp32 [Cout_pad] bias, then fp32 [Cout_pad] multipliers m[c] = s_w[c] * s_in, then {s_res, 1/s_out}
+ *   reserved:  bit 4: fp16 output, bit 5: bf16 output, every other bit zero; decode and chain must be NULL; a residual
+ *              needs the e4m3 output.
+ *   v = act(acc * m[c] + bias[c]) [+ res * s_res] with the e4m3 dot product acc accumulated in fp32, then
+ *   out = RN_satfinite(v * (1/s_out)) (e4m3) or RN(v) (fp16 / bf16).
+ * YB_OP_QUANTIZE: dtype is the SOURCE type (YB_F16 or YB_BF16); in is that NHWC view, out an e4m3 NHWC view of the
+ *   same extent (Ho == H, Wo == W, Cout == Cin, a multiple of 16; in_cstride a multiple of 8, out_cstride of 16);
+ *   bias: fp32 {1/s}; weight, residual, decode and chain NULL; act and reserved 0.  out = RN_satfinite(in * (1/s)).
+ * YB_OP_SPP_POOL and YB_OP_UPSAMPLE2X with dtype YB_F8E4M3: source and destination share one scale, so the pool is a
+ *   max over the decoded values and the upsample a copy, both exact; channel counts and cstrides multiples of 16.
+ * yb_abi_version() stays 1 with FP8: the descriptor layout is unchanged, and the element type, the op kind and the
+ * reserved bits are additions that every earlier descriptor leaves at values it already had to use. */
 typedef struct {
   int32_t kind;
-  int32_t dtype;                /* YB_F16 or YB_BF16 (accumulation is always fp32) */
+  int32_t dtype;                /* YB_F16, YB_BF16 or YB_F8E4M3 (accumulation is always fp32) */
   int32_t N, H, W;              /* input spatial extent                              */
   int32_t Cin, in_cstride;
   const void* in;
@@ -204,7 +230,7 @@ typedef struct {
                                    super-pixel stem matrix [Cout_pad][3][128] (engine.stem_band); bit 2: take the
                                    halo-patch kernel's stride-2 parity-plane variant whatever the channel counts (tests);
                                    bit 3: do not split N over CTAs with resident weights (A/B timing, tests);
-                                   other bits: must be zero */
+                                   e4m3 convolutions: bits 4 / 5 only (see above); other bits: must be zero */
   const yb_head_decode* decode; /* optional (host pointer, copied at plan creation): fused decode epilogue */
   const yb_conv_chain* chain;   /* optional (host pointer, copied at plan creation): chained pointwise tail  */
 } yb_op_desc;
@@ -214,7 +240,7 @@ typedef struct {
 int yb_conv_chain_supported(const yb_op_desc* op);
 
 /* Host-only introspection of how a convolution would be launched (tests, tuning): fills 12 ints
- *   [0] 1 = halo-patch kernel, 0 = im2col / 1x1 kernel   [1] N-tile width   [2] N tiles   [3] weights resident in
+ *   [0] 1 = halo-patch kernel, 0 = im2col / 1x1 kernel, 2 = the e4m3 kernel   [1] N-tile width   [2] N tiles   [3] weights resident in
  *   shared memory   [4] M tiles per weight pass   [5] patch slots (pipeline stages)   [6] weight-ring slabs (k-iterations
  *   per stage)   [7] store-box columns   [8] staging buffers per epilogue group (halo-patch kernel) / epilogue groups
  *   (1x1 / im2col kernel)   [9] dynamic shared memory   [10] grid

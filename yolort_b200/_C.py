@@ -14,9 +14,10 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # YB_LIB_PATH: A/B timing of alternative builds of the same ABI (scripts/ab_step.py); never set in product use
 LIB_PATH = os.environ.get("YB_LIB_PATH") or os.path.join(_HERE, "libyolort_b200.so")
 
-YB_U8, YB_F16, YB_BF16, YB_F32 = 0, 1, 2, 3
+YB_U8, YB_F16, YB_BF16, YB_F32, YB_F8E4M3 = 0, 1, 2, 3, 4
 YB_LAYOUT_NCHW, YB_LAYOUT_S2D16 = 0, 1
 YB_OP_CONV, YB_OP_SPP_POOL, YB_OP_UPSAMPLE2X, YB_OP_ATTENTION, YB_OP_DWCONV, YB_OP_SE, YB_OP_AVGPOOL = 0, 1, 2, 3, 4, 5, 6
+YB_OP_QUANTIZE = 7
 YB_ACT_NONE, YB_ACT_SILU, YB_ACT_HARDSWISH, YB_ACT_LEAKY01, YB_ACT_RELU = 0, 1, 2, 3, 4
 YB_MAX_LEVELS, YB_MAX_ANCHORS = 4, 4
 NMS_TV_AUTO, NMS_EXACT_PER_CLASS, NMS_OFFSET_TRICK = 0, 1, 2
@@ -210,7 +211,8 @@ def check(rc: int, what: str) -> None:
 
 def dtype_code(dt: torch.dtype) -> int:
     try:
-        return {torch.uint8: YB_U8, torch.float16: YB_F16, torch.bfloat16: YB_BF16, torch.float32: YB_F32}[dt]
+        return {torch.uint8: YB_U8, torch.float16: YB_F16, torch.bfloat16: YB_BF16, torch.float32: YB_F32,
+                torch.float8_e4m3fn: YB_F8E4M3}[dt]
     except KeyError:
         raise NativeLibraryError(f"unsupported tensor dtype {dt}") from None
 
@@ -345,6 +347,8 @@ def conv_config(op: "OpDesc") -> dict:
     keys = ("patch_kernel", "block_n", "n_tiles", "weights_resident", "tiles_per_pass", "slots", "ring", "store_cols",
             "store_bufs", "smem_bytes", "grid", "chained")
     cfg = dict(zip(keys, [int(v) for v in info]))
+    cfg["e4m3_kernel"] = int(cfg["patch_kernel"] == 2)   # slot 0 is 2 for the e4m3 kernel (conv_fp8_sm90.cu)
+    cfg["patch_kernel"] = int(cfg["patch_kernel"] == 1)
     if not cfg["patch_kernel"]:     # slot 8 of the 1x1 / im2col kernel: consumer warpgroups (sharing two staging buffers)
         cfg["epilogue_groups"] = cfg.pop("store_bufs")
     return cfg

@@ -23,13 +23,15 @@ using namespace yb;
 struct yb_plan {
   struct Step {
     yb_op_desc desc;
-    ConvOp* conv;       // non-null for YB_OP_CONV
+    ConvOp* conv;       // non-null for YB_OP_CONV at f16 / bf16
+    Fp8ConvOp* fp8;     // non-null for YB_OP_CONV at e4m3
     AttentionOp* attn;  // non-null for YB_OP_ATTENTION
   };
   std::vector<Step> steps;
   ~yb_plan() {
     for (auto& s : steps) {
       if (s.conv) conv_op_destroy(s.conv);
+      if (s.fp8) fp8_conv_op_destroy(s.fp8);
       if (s.attn) attention_op_destroy(s.attn);
     }
   }
@@ -39,7 +41,7 @@ extern "C" const char* yb_last_error(void) { return g_err; }
 extern "C" int yb_abi_version(void) { return 1; }
 
 extern "C" int yb_conv_chain_supported(const yb_op_desc* op) {
-  if (op == nullptr || op->kind != YB_OP_CONV || op->chain == nullptr) return 0;
+  if (op == nullptr || op->kind != YB_OP_CONV || op->chain == nullptr || op->dtype == YB_F8E4M3) return 0;
   const int rc = patch_conv_eligible(*op) ? patch_conv_configure_check(*op) : conv_configure_check(*op);
   return rc == YB_OK ? 1 : 0;
 }
@@ -47,6 +49,7 @@ extern "C" int yb_conv_chain_supported(const yb_op_desc* op) {
 extern "C" int yb_conv_config(const yb_op_desc* op, int32_t* info12) {
   YB_REQUIRE(op != nullptr && info12 != nullptr && op->kind == YB_OP_CONV, "conv_config: needs a convolution op and an output array");
   for (int i = 0; i < 12; ++i) info12[i] = 0;
+  if (op->dtype == YB_F8E4M3) return fp8_conv_configure_check(*op, info12);
   return patch_conv_eligible(*op) ? patch_conv_configure_check(*op, info12) : conv_configure_check(*op, info12);
 }
 
@@ -57,6 +60,7 @@ extern "C" int yb_plan_create(const yb_op_desc* ops, int n_ops, yb_plan** plan_o
     yb_plan::Step st;
     st.desc = ops[i];
     st.conv = nullptr;
+    st.fp8 = nullptr;
     st.attn = nullptr;
     int rc = YB_OK;
     if (ops[i].in == nullptr || ops[i].out == nullptr) {
@@ -66,6 +70,8 @@ extern "C" int yb_plan_create(const yb_op_desc* ops, int n_ops, yb_plan** plan_o
       if (ops[i].weight == nullptr || ops[i].bias == nullptr) {
         set_error("plan_create: conv op %d without weight/bias", i);
         rc = YB_ERR_INVALID;
+      } else if (ops[i].dtype == YB_F8E4M3) {
+        rc = fp8_conv_op_create(ops[i], &st.fp8);   // validates before any driver call
       } else {
         rc = conv_op_create(ops[i], &st.conv);
       }
@@ -77,6 +83,8 @@ extern "C" int yb_plan_create(const yb_op_desc* ops, int n_ops, yb_plan** plan_o
       rc = se_configure_check(ops[i]);
     } else if (ops[i].kind == YB_OP_AVGPOOL) {
       rc = avgpool_configure_check(ops[i]);
+    } else if (ops[i].kind == YB_OP_QUANTIZE) {
+      rc = quantize_configure_check(ops[i]);
     } else if (ops[i].kind == YB_OP_SPP_POOL || ops[i].kind == YB_OP_UPSAMPLE2X) {
       rc = validate_pool_or_upsample(ops[i]);
     } else {
@@ -107,7 +115,7 @@ extern "C" int yb_plan_run_range(yb_plan* plan, int first, int count, void* stre
     int rc;
     switch (st.desc.kind) {
       case YB_OP_CONV:
-        rc = conv_op_launch(st.conv, stream);
+        rc = st.fp8 ? fp8_conv_op_launch(st.fp8, stream) : conv_op_launch(st.conv, stream);
         break;
       case YB_OP_ATTENTION:
         rc = attention_op_launch(st.attn, stream);
@@ -120,6 +128,9 @@ extern "C" int yb_plan_run_range(yb_plan* plan, int first, int count, void* stre
         break;
       case YB_OP_AVGPOOL:
         rc = avgpool_launch(st.desc, stream);
+        break;
+      case YB_OP_QUANTIZE:
+        rc = quantize_launch(st.desc, stream);
         break;
       case YB_OP_SPP_POOL:
         rc = spp_pool_launch(st.desc, stream);

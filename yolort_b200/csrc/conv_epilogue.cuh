@@ -66,10 +66,8 @@ struct FragRows {
   bool ok[2];
 };
 
-// bias -> activation (SiLU / linear, the r3.1 Hardswish / LeakyReLU(0.1), or MobileNetV3's ReLU) -> + shortcut, in fp32
-template <bool kBf16>
-__device__ __forceinline__ uint32_t epilogue_pair(const EpilogueParams& p, float v0, float v1, long long row, bool row_ok,
-                                                  int gcol) {
+// activation (SiLU / linear, the r3.1 Hardswish / LeakyReLU(0.1), or MobileNetV3's ReLU) of a column pair, in fp32
+__device__ __forceinline__ void act_pair(const EpilogueParams& p, float& v0, float& v1) {
   if (p.act == YB_ACT_SILU) {
     v0 = silu(v0);
     v1 = silu(v1);
@@ -83,6 +81,13 @@ __device__ __forceinline__ uint32_t epilogue_pair(const EpilogueParams& p, float
     v0 = fmaxf(v0, v0 * slope);
     v1 = fmaxf(v1, v1 * slope);
   }
+}
+
+// bias -> activation -> + shortcut, in fp32
+template <bool kBf16>
+__device__ __forceinline__ uint32_t epilogue_pair(const EpilogueParams& p, float v0, float v1, long long row, bool row_ok,
+                                                  int gcol) {
+  act_pair(p, v0, v1);
   if (p.residual != nullptr && row_ok && gcol < p.Cout) {   // Cout % 8 == 0: a pair never straddles it
     const uint16_t* r = reinterpret_cast<const uint16_t*>(p.residual) + row * p.res_cstride + gcol;
     const float2 f = unpack2<kBf16>(__ldg(reinterpret_cast<const unsigned int*>(r)));

@@ -401,12 +401,6 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 }
 
 // ---- host side -----------------------------------------------------------------------------------
-typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                                   const cuuint64_t*, const cuuint64_t*, const int*, const int*,
-                                   cuuint32_t, cuuint32_t, const cuuint32_t*, CUtensorMapInterleave,
-                                   CUtensorMapSwizzle, CUtensorMapL2promotion,
-                                   CUtensorMapFloatOOBfill);
-
 EncodeTiledFn g_encode_tiled = nullptr;
 EncodeIm2colFn g_encode_im2col = nullptr;
 
@@ -444,6 +438,12 @@ int mma_n(int n) {
 int encode_tiled_entry(EncodeTiledFn* out) {
   const int rc = load_driver_entry_points();
   if (rc == YB_OK) *out = g_encode_tiled;
+  return rc;
+}
+
+int encode_im2col_entry(EncodeIm2colFn* out) {
+  const int rc = load_driver_entry_points();
+  if (rc == YB_OK) *out = g_encode_im2col;
   return rc;
 }
 

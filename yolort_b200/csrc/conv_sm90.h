@@ -25,8 +25,23 @@ int conv_configure_check(const yb_op_desc& d, int* info = nullptr);         // h
 int conv_op_launch(const ConvOp* op, cudaStream_t stream);
 void conv_op_destroy(ConvOp* op);
 
-// cuTensorMapEncodeTiled from the driver (looked up once)
+typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                   const cuuint64_t*, const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*,
+                                   CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
+                                   CUtensorMapFloatOOBfill);
+
+// cuTensorMapEncodeTiled / cuTensorMapEncodeIm2col from the driver (looked up once)
 int encode_tiled_entry(EncodeTiledFn* out);
+int encode_im2col_entry(EncodeIm2colFn* out);
+
+// e4m3 convolution and the fp16/bf16 -> e4m3 quantisation op (conv_fp8_sm90.cu)
+struct Fp8ConvOp;
+int fp8_conv_configure_check(const yb_op_desc& d, int* info = nullptr);   // host-only validation + tiling (no driver calls)
+int fp8_conv_op_create(const yb_op_desc& d, Fp8ConvOp** out);
+int fp8_conv_op_launch(const Fp8ConvOp* op, cudaStream_t stream);
+void fp8_conv_op_destroy(Fp8ConvOp* op);
+int quantize_configure_check(const yb_op_desc& d);                         // host-only validation (no driver calls)
+int quantize_launch(const yb_op_desc& d, cudaStream_t stream);
 
 // multi-head attention (attention_sm90.cu)
 struct AttentionOp;

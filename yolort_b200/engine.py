@@ -17,6 +17,7 @@ path_aggregation_network.py:199-239, box_head.py:68-82).  Here the module tree i
 Host code only prepares descriptors; all arithmetic happens in csrc/*.cu.
 """
 import ctypes
+import math
 import os
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Tuple
@@ -41,6 +42,7 @@ class _Buf:
     div: int          # spatial divisor w.r.t. the canvas, or GLOBAL
     C: int            # total channels (pixel stride)
     offset: int = 0   # byte offset in the arena
+    esz: int = 2      # bytes per element: 2 (fp16 / bf16), 1 (e4m3 buffers of an FP8 plan)
 
     def hw(self, H: int, W: int) -> Tuple[int, int]:
         """Spatial extent of this buffer on an H x W canvas."""
@@ -77,6 +79,10 @@ class _Op:
     chain_own: int = 0
     chain_extra: Optional[_View] = None
     chain_store: bool = True
+    # FP8 plans (lower_fp8): element type code of the op when it differs from the plan's compute dtype (e4m3 ops; the
+    # QUANTIZE op carries its source type), and the option bits of an e4m3 convolution (16-bit head outputs)
+    dtype: Optional[int] = None
+    reserved: int = 0
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -227,11 +233,15 @@ class _Lowering:
         assert w.shape[1] == src.C * pack and w.shape[0] <= dst.C * pack, (name, tuple(w.shape), src.C, dst.C)
         if pack > 1:
             assert src.ch0 == 0 and src.C == src.buf.C and dst.ch0 == 0 and dst.C == dst.buf.C and residual is None
-        wp, _, co_pad = pack_weight(w, self.dtype, self.device)
-        bp = pack_bias(b, co_pad, self.device)
+        wp, bp = self.pack(w, b)
         if ref_flops_per_pixel is None:
             ref_flops_per_pixel = 2 * w.shape[0] * w.shape[1] * k * k
         self.ops.append(_Op(_C.YB_OP_CONV, src, dst, k, s, p, act, wp, bp, residual, name, ref_flops_per_pixel, pack, force_im2col))
+
+    def pack(self, w: torch.Tensor, b: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Packed weight and fp32 bias of a convolution from its fp64 folded weight and bias."""
+        wp, _, co_pad = pack_weight(w, self.dtype, self.device)
+        return wp, pack_bias(b, co_pad, self.device)
 
     def conv_band(self, name, w_band, b, src: _View, dst: _View, act, ref_flops_per_pixel):
         """Stem on the banded super-pixel weights (stem_band): pack 4, 3x3/s1/p1, handled by the patch kernel's
@@ -519,10 +529,38 @@ class _Lowering:
         return x
 
 
-def lower_yolo(model: nn.Module, dtype: torch.dtype, device: torch.device, stem_variant: str = "auto"):
+class _Fp8Lowering(_Lowering):
+    """The same walk for an FP8 plan (lower_fp8): the stem is packed in the compute dtype and one YB_OP_QUANTIZE
+    converts its output to e4m3; every later convolution packs its weight to e4m3 at once, with one scale per output
+    channel (`s_w[op index]`, fp64).  The activation scales, hence the epilogue multipliers, come later."""
+
+    def __init__(self, dtype: torch.dtype, device: torch.device):
+        super().__init__(dtype, device)
+        self.quantized = False
+        self.s_w: Dict[int, torch.Tensor] = {}
+
+    def pack(self, w: torch.Tensor, b: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+        if not self.quantized:
+            return super().pack(w, b)
+        s_w = e4m3_scales(w.abs().amax(dim=(1, 2, 3)))
+        self.s_w[len(self.ops)] = s_w
+        wq = pack_weight_e4m3(w, s_w, self.device)
+        return wq, pack_bias(b, wq.shape[0], self.device)
+
+    def stem(self, prefix: str, stem: nn.Module, stem_variant: str) -> Tuple[_Buf, _View]:
+        x0, out = super().stem(prefix, stem, stem_variant)
+        q = _View(self.buf(f"{prefix}.0(e4m3)", out.buf.div, out.C), 0, out.C)
+        self.ops.append(_Op(_C.YB_OP_QUANTIZE, out, q, name=f"{prefix}.0(quantize)"))
+        self.quantized = True
+        return x0, q
+
+
+def lower_yolo(model: nn.Module, dtype: torch.dtype, device: torch.device, stem_variant: str = "auto",
+               fp8: bool = False):
     """Walk YOLO.backbone / YOLO.head and emit (lowering, input_buf, head_bufs, features).
-    `stem_variant`: "auto" | "band" | "superpixel" | "im2col" (the last two are kept for parity tests and A/B timing)."""
-    L = _Lowering(dtype, device)
+    `stem_variant`: "auto" | "band" | "superpixel" | "im2col" (the last two are kept for parity tests and A/B timing).
+    `fp8`: the walk of an FP8 plan (_Fp8Lowering; lower_fp8 quantises it)."""
+    L = (_Fp8Lowering if fp8 else _Lowering)(dtype, device)
     bb = model.backbone
     body, pan = bb.body, bb.pan
     ch = list(bb.out_channels)
@@ -585,6 +623,135 @@ def lower_yolo(model: nn.Module, dtype: torch.dtype, device: torch.device, stem_
                _View(hb, 0, co_buf), 1, 1, 0, _C.YB_ACT_NONE)
         head_bufs.append(hb)
     return L, x0, head_bufs, {f"p{l + 3}": r for l, r in enumerate(results)}
+
+
+# ---------------------------------------------------------------------------------------------------
+# FP8 (e4m3) plans
+# ---------------------------------------------------------------------------------------------------
+E4M3_MAX = 448.0
+
+
+def e4m3_scale(amax: float) -> float:
+    """The smallest power of two s with amax / s <= 448 (1 for an all-zero tensor).  Powers of two make every
+    dequantisation and every epilogue multiplier exact."""
+    if not amax > 0:
+        return 1.0
+    s = 2.0 ** math.ceil(math.log2(amax / E4M3_MAX))
+    while amax / s > E4M3_MAX:
+        s *= 2.0
+    while amax / (0.5 * s) <= E4M3_MAX:
+        s *= 0.5
+    return s
+
+
+def e4m3_scales(amax: torch.Tensor) -> torch.Tensor:
+    """e4m3_scale of every element of `amax`, in fp64 (per-output-channel weight scales)."""
+    a = amax.double()
+    s = torch.exp2(torch.ceil(torch.log2(a / E4M3_MAX)))
+    s = torch.where(a / s > E4M3_MAX, 2.0 * s, s)
+    s = torch.where(a / (0.5 * s) <= E4M3_MAX, 0.5 * s, s)
+    return torch.where(a > 0, s, torch.ones_like(s))
+
+
+def e4m3_round(x: torch.Tensor) -> torch.Tensor:
+    """fp64 `x` rounded once to the nearest e4m3 value (ties to even, saturating at +-448), still in fp64."""
+    _, e = torch.frexp(x)
+    q = torch.exp2((torch.clamp(e - 1, min=-6) - 3).to(torch.float64))    # spacing of the binade (subnormals: 2^-9)
+    return torch.clamp(torch.round(x / q) * q, -E4M3_MAX, E4M3_MAX)
+
+
+def pack_weight_e4m3(w: torch.Tensor, s_w: torch.Tensor, device: torch.device) -> torch.Tensor:
+    """[Co,Ci,k,k] fp64 with per-output-channel scales s_w -> e4m3 K-major [Co_pad, k*k, Ci_pad] holding w / s_w,
+    zero padded.  Ci_pad is a multiple of 128 (one 128-byte TMA row) once Ci > 64, else of 32 (the wgmma K step)."""
+    co, ci, kh, kw = w.shape
+    ci_pad, co_pad = (_round_up(ci, 128) if ci > 64 else _round_up(ci, 32)), _round_up(co, 16)
+    p = torch.zeros((co_pad, kh * kw, ci_pad), dtype=torch.float64, device=w.device)
+    p[:co, :, :ci] = e4m3_round(w / s_w.view(-1, 1, 1, 1)).permute(0, 2, 3, 1).reshape(co, kh * kw, ci)
+    return p.to(torch.float8_e4m3fn).to(device).contiguous()
+
+
+def scale_groups(L: _Lowering) -> List[List[_Buf]]:
+    """Buffers that share one activation scale: every channel window of a buffer (so every concat) by construction, and
+    the source and destination of each op that moves values without arithmetic (SPP max-pool, nearest upsample), so
+    that those ops are exact in e4m3.  Union-find over the op list, groups in buffer order."""
+    parent = {id(b): id(b) for b in L.bufs}
+
+    def find(k):
+        while parent[k] != k:
+            parent[k] = parent[parent[k]]
+            k = parent[k]
+        return k
+
+    for op in L.ops:
+        if op.kind in (_C.YB_OP_SPP_POOL, _C.YB_OP_UPSAMPLE2X):
+            parent[find(id(op.src.buf))] = find(id(op.dst.buf))
+    groups: Dict[int, List[_Buf]] = {}
+    for b in L.bufs:
+        groups.setdefault(find(id(b)), []).append(b)
+    return list(groups.values())
+
+
+def fp8_unsupported(model: nn.Module) -> Optional[str]:
+    """Name of the model family when it has no FP8 plan (its ops have no e4m3 kernels), else None."""
+    from .models._classifier import DarkNetClassifier
+    from .models.yolo_lite import BackboneWithFPN
+
+    if isinstance(model, DarkNetClassifier):
+        return f"the DarkNet classifier {type(model).__name__}"
+    if isinstance(getattr(model, "backbone", None), BackboneWithFPN):
+        return "yolov5_mobilenet_v3_small_fpn"
+    if any(isinstance(m, C3TR) for m in model.modules()):
+        return "yolov5ts (C3TR transformer neck)"
+    return None
+
+
+def lower_fp8(model: nn.Module, dtype: torch.dtype, device: torch.device, amax: Dict[str, float],
+              stem_variant: str = "auto"):
+    """The FP8 plan of a YOLOv5 detection model: (lowering, input_buf, head_bufs, features, scale per buffer id).
+
+    The walk is lower_yolo's (_Fp8Lowering).  The stem keeps its fp16 / bf16 kernel and a YB_OP_QUANTIZE converts its
+    output; every later op runs on e4m3 buffers, the heads write fp16 / bf16 logits.  `amax` is the calibrated maximum
+    of |x| per buffer name of the fp16 / bf16 plan (quantization.calibrate_fp8); a scale group takes the largest of its
+    members.  Weights: one scale per output channel from the BN-folded fp64 weight, one rounding to e4m3."""
+    why = fp8_unsupported(model)
+    if why is not None:
+        raise NotImplementedError(f"FP8 inference is not implemented for {why}")
+    L, x0, head_bufs, feats = lower_yolo(model, dtype, device, stem_variant, fp8=True)
+    qi = next(i for i, op in enumerate(L.ops) if op.kind == _C.YB_OP_QUANTIZE)
+    stem_out, stem_q = L.ops[qi].src.buf, L.ops[qi].dst.buf
+    wide = {id(x0), id(stem_out)} | {id(b) for b in head_bufs}
+    for b in L.bufs:
+        if id(b) not in wide:
+            b.esz = 1
+    missing = sorted(b.name for b in L.bufs if b.esz == 1 and b is not stem_q and b.name not in amax)
+    if missing:
+        raise ValueError(f"the calibration has no amax for {missing[:4]}... (calibrated for another architecture?)")
+    scale: Dict[int, float] = {}
+    for group in scale_groups(L):
+        q = [b for b in group if b.esz == 1]
+        if q:
+            s = e4m3_scale(max(amax[stem_out.name if b is stem_q else b.name] for b in q))
+            for b in q:
+                scale[id(b)] = s
+    head_ids = {id(b) for b in head_bufs}
+    for i, op in enumerate(L.ops[qi:], start=qi):
+        if op.kind == _C.YB_OP_QUANTIZE:
+            op.bias = torch.tensor([1.0 / scale[id(op.dst.buf)]], dtype=torch.float32, device=device)
+            continue
+        op.dtype = _C.YB_F8E4M3
+        if op.kind != _C.YB_OP_CONV:
+            continue
+        s_w = L.s_w.pop(i)
+        co, co_pad = s_w.shape[0], op.weight.shape[0]
+        head = id(op.dst.buf) in head_ids
+        tail = torch.zeros((2 * co_pad + 2,), dtype=torch.float64, device=s_w.device)
+        tail[:co_pad] = op.bias.to(s_w.device)        # the fp32 bias
+        tail[co_pad:co_pad + co] = s_w * scale[id(op.src.buf)]
+        tail[2 * co_pad] = scale[id(op.residual.buf)] if op.residual is not None else 0.0
+        tail[2 * co_pad + 1] = 1.0 if head else 1.0 / scale[id(op.dst.buf)]
+        op.bias = tail.to(torch.float32).to(device).contiguous()
+        op.reserved = (32 if dtype == torch.bfloat16 else 16) if head else 0
+    return L, x0, head_bufs, feats, scale
 
 
 def _split_conv_norm_act(name, m: nn.Sequential):
@@ -750,11 +917,17 @@ class Lowered:
     """Shape-independent part of a model's plans: the op list with BN-folded, packed weights on the device.  Built
     once per Engine and shared by every PlanInstance (a plan adds only an activation arena and TMA descriptors)."""
 
-    def __init__(self, model: nn.Module, dtype: torch.dtype, device: torch.device, stem_variant: str = "auto"):
+    def __init__(self, model: nn.Module, dtype: torch.dtype, device: torch.device, stem_variant: str = "auto",
+                 fp8=None):
         from .models._classifier import DarkNetClassifier
         from .models.yolo_lite import BackboneWithFPN
 
-        if isinstance(model, DarkNetClassifier):
+        self.fp8 = fp8 is not None       # fp8: a quantization.Fp8Calibration
+        self.feat_scales: Dict[str, float] = {}
+        if fp8 is not None:
+            self.L, self.x0, self.head_bufs, self.feats, scale = lower_fp8(model, dtype, device, fp8.amax, stem_variant)
+            self.feat_scales = {k: scale[id(v.buf)] for k, v in self.feats.items()}
+        elif isinstance(model, DarkNetClassifier):
             self.L, self.x0, self.head_bufs, self.feats = lower_darknet(model, dtype, device, stem_variant)
         elif isinstance(model.backbone, BackboneWithFPN):
             self.L, self.x0, self.head_bufs, self.feats = lower_lite(model, dtype, device)
@@ -770,13 +943,13 @@ def front_op_count(L: _Lowering) -> int:
     `YOLOv5.predict` can run per image chunk while later chunks are still crossing PCIe."""
     n = 0
     for op in L.ops:
-        if op.dst.buf.div > 8 or op.src.buf.div > 8 or op.kind != _C.YB_OP_CONV:
+        if op.dst.buf.div > 8 or op.src.buf.div > 8 or op.kind not in (_C.YB_OP_CONV, _C.YB_OP_QUANTIZE):
             break
         n += 1
     return n
 
 
-def assign_offsets(L: _Lowering, x0: _Buf, keep: List[_Buf], N: int, H: int, W: int, reuse: bool, esz: int = 2,
+def assign_offsets(L: _Lowering, x0: _Buf, keep: List[_Buf], N: int, H: int, W: int, reuse: bool,
                    front_ops: int = 0, launches: Optional[List[Tuple[int, ...]]] = None):
     """Arena layout for one (N, H, W): byte offset per buffer and the arena size.  `launches` groups the ops that run
     as ONE kernel (chained tails): liveness is tracked per launch, since everything a fused launch touches is live at
@@ -790,7 +963,7 @@ def assign_offsets(L: _Lowering, x0: _Buf, keep: List[_Buf], N: int, H: int, W: 
         launches = [(i,) for i in range(len(L.ops))]
     step_of = {i: t for t, grp in enumerate(launches) for i in grp}
     n_ops = len(launches)          # time is counted in launches
-    size = {id(b): _round_up(N * b.hw(H, W)[0] * b.hw(H, W)[1] * b.C * esz, 1024) for b in L.bufs}
+    size = {id(b): _round_up(N * b.hw(H, W)[0] * b.hw(H, W)[1] * b.C * b.esz, 1024) for b in L.bufs}
     first = {id(b): n_ops for b in L.bufs}
     last = {id(b): -1 for b in L.bufs}
     first[id(x0)] = -1
@@ -879,7 +1052,7 @@ class PlanInstance:
         self.N, self.H, self.W = N, H, W
         self.dtype, self.device = L.dtype, L.device
         self.keep_intermediates = keep_intermediates
-        esz = 2
+        fuse_chains = fuse_chains and not low.fp8      # FP8 plans run every convolution as its own launch
         # the input canvas stays live too, so that a plan can be re-run (timing loops, tests) without re-letterboxing
         keep = [x0] + list(head_bufs) + [v.buf for v in feats.values()]
         # chunked front: 4 chunks when the batch divides (>= 4 images per chunk)
@@ -893,7 +1066,7 @@ class PlanInstance:
             d = _C.OpDesc()
             hi, wi = op.src.buf.hw(H, W)
             ho, wo = op.dst.buf.hw(H, W)
-            d.kind, d.dtype = op.kind, code
+            d.kind, d.dtype = op.kind, code if op.dtype is None else op.dtype
             k = op.pack
             if wi % k or wo % k:
                 raise ValueError(f"{op.name}: width {wi} not divisible by the pixel packing {k}")
@@ -910,9 +1083,13 @@ class PlanInstance:
                     d.Cin_pad = 64     # [Cout_pad, 3, 2 x 64] banded stem matrix: one 64-channel chunk of super-pixels
             elif op.kind in (_C.YB_OP_DWCONV, _C.YB_OP_SE):
                 d.weight, d.bias = op.weight.data_ptr(), op.bias.data_ptr()
+            elif op.kind == _C.YB_OP_QUANTIZE:
+                d.bias = op.bias.data_ptr()
             d.reserved = (1 if op.force_im2col else 0) | (2 if op.band else 0) | (8 if no_nsplit else 0)
-            if op.kind in (_C.YB_OP_ATTENTION, _C.YB_OP_DWCONV, _C.YB_OP_SE, _C.YB_OP_AVGPOOL):
+            if op.kind in (_C.YB_OP_ATTENTION, _C.YB_OP_DWCONV, _C.YB_OP_SE, _C.YB_OP_AVGPOOL, _C.YB_OP_QUANTIZE):
                 d.reserved = 0        # these ops have no option bits
+            if op.dtype == _C.YB_F8E4M3:
+                d.reserved = op.reserved
             if op.residual is not None:
                 d.residual, d.res_cstride = ptr(op.residual), op.residual.buf.C
             return d
@@ -958,15 +1135,15 @@ class PlanInstance:
         step_of = {j: t for t, grp in enumerate(launches) for j in grp}
         self.front_ops = step_of[front_ops - 1] + 1 if front_ops else 0     # in launches (what the run_* methods count)
         self._front_op_count = front_ops                                       # in ops of the lowering
-        offsets, total = assign_offsets(L, x0, keep, N, H, W, reuse=not keep_intermediates, esz=esz,
-                                        front_ops=front_ops, launches=launches)
+        offsets, total = assign_offsets(L, x0, keep, N, H, W, reuse=not keep_intermediates, front_ops=front_ops,
+                                        launches=launches)
         self.arena = torch.zeros((max(total, 1024),), dtype=torch.uint8, device=L.device)
         self.arena_bytes = total
-        self.unshared_bytes = sum(_round_up(N * b.hw(H, W)[0] * b.hw(H, W)[1] * b.C * esz, 1024) for b in L.bufs)
+        self.unshared_bytes = sum(_round_up(N * b.hw(H, W)[0] * b.hw(H, W)[1] * b.C * b.esz, 1024) for b in L.bufs)
         base = self.arena.data_ptr()
 
         def ptr(v: _View) -> int:
-            return base + offsets[id(v.buf)] + v.ch0 * esz
+            return base + offsets[id(v.buf)] + v.ch0 * v.buf.esz
 
         descs = []
         self.op_names = []
@@ -1017,7 +1194,7 @@ class PlanInstance:
             h, w = b.hw(H, W)
             n = N * h * w * b.C
             o = offsets[id(b)]
-            return self.arena[o: o + n * esz].view(L.dtype).view(N, h, w, b.C)
+            return self.arena[o: o + n * b.esz].view(L.dtype if b.esz == 2 else torch.float8_e4m3fn).view(N, h, w, b.C)
 
         self.input = nhwc(x0)                      # [N, H/2, W/2, 16] space-to-depth canvas
         self.heads = [nhwc(b) for b in head_bufs]  # [N, h, w, round_up(3*(nc+5), 16)]
@@ -1029,6 +1206,28 @@ class PlanInstance:
     @property
     def device_bytes(self) -> int:
         return int(self.arena.numel())
+
+    # -- e4m3 features of an FP8 plan (the hook path: YOLO.backbone / YOLO.head) ------------------------------------
+    def dequantized_feature(self, key: str, dtype: torch.dtype) -> torch.Tensor:
+        """Feature map `key` of an FP8 plan as its e4m3 values times their power-of-two scale, in `dtype` (exact for
+        scales of 2^-15 and up in fp16, for any scale in bf16)."""
+        return (self.features[key].to(torch.float32) * self._low.feat_scales[key]).to(dtype)
+
+    def quantize_feature(self, key: str, x_nhwc: torch.Tensor) -> None:
+        """x (NHWC, the plan's compute dtype) -> e4m3 feature buffer `key`, by one YB_OP_QUANTIZE launch with the
+        feature's scale: a feature from dequantized_feature comes back as the same bytes."""
+        x = x_nhwc.to(self.dtype).contiguous()
+        dst = self.features[key]
+        N, h, w, C = dst.shape
+        inv = self.__dict__.setdefault("_inv_scales", {})
+        if key not in inv:
+            inv[key] = torch.tensor([1.0 / self._low.feat_scales[key]], dtype=torch.float32, device=self.device)
+        d = _C.OpDesc()
+        d.kind, d.dtype = _C.YB_OP_QUANTIZE, _C.dtype_code(self.dtype)
+        d.N, d.H, d.W, d.Cin, d.in_cstride, d.in_ = N, h, w, C, C, x.data_ptr()
+        d.Ho, d.Wo, d.Cout, d.out_cstride, d.out = h, w, C, C, dst.data_ptr()
+        d.bias = inv[key].data_ptr()
+        _C.Plan([d], self.device).run()
 
     def run(self, first: int = 0, count: Optional[int] = None) -> None:
         """Backbone + PAN + heads, logits stored in `self.heads`."""
@@ -1060,7 +1259,6 @@ class PlanInstance:
         every tensor pointer advanced by the chunk's images (activations are NHWC, image-major)."""
         L = self._low.L
         c = self.N // self.front_chunks
-        esz = 2
         plans = []
         for k in range(self.front_chunks):
             ds = []
@@ -1071,7 +1269,7 @@ class PlanInstance:
                 d2.N = c
 
                 def adv(view):
-                    return k * c * (self.H // view.buf.div) * (self.W // view.buf.div) * view.buf.C * esz
+                    return k * c * (self.H // view.buf.div) * (self.W // view.buf.div) * view.buf.C * view.buf.esz
 
                 d2.in_ = d.in_ + adv(op.src)
                 d2.out = d.out + adv(op.dst)
@@ -1132,6 +1330,8 @@ class Engine:
         import collections
         self._plans: "collections.OrderedDict[tuple, PlanInstance]" = collections.OrderedDict()
         self._low: Optional[Lowered] = None
+        self._low8: Optional[Lowered] = None      # the FP8 lowering of `fp8`
+        self.fp8 = None          # quantization.Fp8Calibration: plans run in FP8 (YOLO.set_fp8); None: in `dtype`
         self._tensors: List[torch.Tensor] = []
         self._versions: Tuple[int, ...] = ()
         self.max_arena_bytes = max_arena_bytes
@@ -1145,11 +1345,24 @@ class Engine:
     def _fingerprint(self) -> Tuple[int, ...]:
         return tuple(t._version for t in self._tensors)
 
-    def lowered(self) -> Lowered:
+    def lowered(self, fp8: Optional[bool] = None) -> Lowered:
         """The shared lowering; rebuilt (and every plan dropped) when a parameter or BN statistic was modified in
-        place since the last lowering (`_version` counters; `.to()` / `load_state_dict` go through YOLO's hooks)."""
-        if self._low is not None and self._fingerprint() != self._versions:
+        place since the last lowering (`_version` counters; `.to()` / `load_state_dict` go through YOLO's hooks).
+        `fp8`: the FP8 (True) or the `dtype` (False) lowering; default: the one `self.fp8` selects."""
+        if (self._low is not None or self._low8 is not None) and self._fingerprint() != self._versions:
             self.invalidate()
+        use_fp8 = self.fp8 is not None if fp8 is None else fp8
+        if use_fp8:
+            if self.fp8 is None:
+                raise ValueError("an FP8 lowering needs a calibration (set_fp8)")
+            if self._low8 is None:
+                with _C.device_guard(self.device):
+                    if self._low is None:
+                        self._tensors = [t for t in list(self.model.parameters()) + list(self.model.buffers())]
+                        self._versions = self._fingerprint()
+                    self._low8 = Lowered(self.model, self.dtype, self.device, self.stem_variant, fp8=self.fp8)
+                self.lowerings += 1
+            return self._low8
         if self._low is None:
             with _C.device_guard(self.device):
                 self._tensors = [t for t in list(self.model.parameters()) + list(self.model.buffers())]
@@ -1161,6 +1374,16 @@ class Engine:
     def invalidate(self) -> None:
         self._plans.clear()
         self._low = None
+        self._low8 = None
+
+    def set_fp8(self, calib) -> None:
+        """Run plans in FP8 with the scales of `calib` (None: in `dtype`).  FP8 plans are cached apart from the others,
+        so switching back finds the `dtype` plans as they were."""
+        if calib is not self.fp8:
+            self.fp8 = calib
+            self._low8 = None
+            for key in [k for k in self._plans if k[-1]]:
+                del self._plans[key]
 
     # -- plans ---------------------------------------------------------------------------------------------------
     def _budget(self) -> int:
@@ -1175,11 +1398,14 @@ class Engine:
              chunked: bool = False) -> PlanInstance:
         """`chunked`: a plan whose first ops can also run per image chunk (PlanInstance.run_front_chunk; the arena keeps
         the front buffers live, so it is a separate instance from the plain plan of the same shape)."""
+        check_fp8 = getattr(self.model, "_check_fp8", None)     # YOLO: a stale FP8 calibration raises
+        if check_fp8 is not None:
+            check_fp8()
         low = self.lowered()
         pkey = None if post is None else (post["score_thresh"], post["nms_thresh"], post["detections_per_img"],
                                           post["semantics"], post["num_classes"])
         chunked = bool(chunked and N % 4 == 0 and N >= 16 and not keep_intermediates)
-        key = (N, H, W, pkey, bool(keep_intermediates), chunked, bool(self.fuse_chains))
+        key = (N, H, W, pkey, bool(keep_intermediates), chunked, bool(self.fuse_chains), self.fp8 is not None)
         inst = self._plans.get(key)
         if inst is not None:
             self._plans.move_to_end(key)

@@ -91,6 +91,9 @@ class YOLO(nn.Module):
                                        anchors_px=anchor_generator.anchors_px())
         self.post_process = post_process
         self._engine = None
+        self._fp8 = None             # quantization.Fp8Calibration of the FP8 plan (set_fp8), None: fp16 / bf16
+        self._fp8_stale = False
+        self._fp8_versions = ()
         # `backbone(x)` / `head(features)` are callable sub-modules like the reference's (yolo.py:163-166,
         # utils/hooks.py:7-26): they execute the corresponding launch range of this model's plan.  The owner is
         # reached through a list so that it is neither registered as a sub-module nor lost by deepcopy/pickle.
@@ -100,15 +103,25 @@ class YOLO(nn.Module):
         # never calls child.load_state_dict -- it recurses through _load_from_state_dict and fires the post hooks
         # of every sub-module -- so the invalidation is a post hook; `.to()/.half()/.cuda()` reach `_apply`; in-place
         # edits are caught by the engine's parameter-version fingerprint.
+        # The same hook makes an FP8 calibration stale (new weights need new activation ranges).
         self.register_load_state_dict_post_hook(lambda module, incompatible_keys: module._drop_engine())
 
     # -- engine lifetime -----------------------------------------------------------------------------
     def _drop_engine(self) -> None:
         self._engine = None
+        if self._fp8 is not None:
+            self._fp8_stale = True
 
-    def _apply(self, fn, *a, **k):  # .to()/.half()/.cuda() invalidate prepared weights
+    def _apply(self, fn, *a, **k):  # .to()/.half()/.cuda() invalidate prepared weights, and keep an FP8 calibration
         self._engine = None
-        return super()._apply(fn, *a, **k)
+        if self._fp8 is not None and self._param_versions() != self._fp8_versions:
+            self._fp8_stale = True       # edited in place before the move
+        out = super()._apply(fn, *a, **k)
+        self._fp8_versions = self._param_versions()
+        return out
+
+    def _param_versions(self):
+        return tuple(t._version for t in list(self.parameters()) + list(self.buffers()))
 
     def engine(self):
         from ..engine import Engine
@@ -117,7 +130,42 @@ class YOLO(nn.Module):
             p = next(self.parameters())
             dtype = torch.bfloat16 if p.dtype == torch.bfloat16 else torch.float16
             self._engine = Engine(self, dtype, p.device)
+            self._engine.set_fp8(self._fp8)
         return self._engine
+
+    # -- precision -----------------------------------------------------------------------------------
+    @property
+    def precision(self) -> str:
+        """"fp8" when the plans run in FP8 (set_fp8), else the compute dtype of the parameters: "fp16" or "bf16"."""
+        if self._fp8 is not None:
+            return "fp8"
+        return "bf16" if next(self.parameters()).dtype == torch.bfloat16 else "fp16"
+
+    def set_fp8(self, calib) -> None:
+        """Run every later forward on the FP8 (e4m3) plan with the activation ranges of `calib`
+        (quantization.calibrate_fp8), or, with None, on the fp16 / bf16 plan again.  The calibration is not part of
+        `state_dict()`; save `calib.state_dict()` next to the weights.  It goes stale when the weights change
+        (load_state_dict, in-place edits): a forward then raises until set_fp8 is called with a new calibration."""
+        if calib is not None:
+            from ..engine import fp8_unsupported
+            from ..quantization import arch_fingerprint
+
+            why = fp8_unsupported(self)
+            if why is not None:
+                raise NotImplementedError(f"FP8 inference is not implemented for {why}")
+            if calib.fingerprint != arch_fingerprint(self):
+                raise ValueError("this FP8 calibration was made for a different architecture")
+        self._fp8 = calib
+        self._fp8_stale = False
+        self._fp8_versions = self._param_versions()
+        if self._engine is not None:
+            self._engine.set_fp8(calib)
+
+    def _check_fp8(self) -> None:
+        if self._fp8 is not None and (self._fp8_stale or self._param_versions() != self._fp8_versions):
+            self._fp8_stale = True
+            raise RuntimeError("the FP8 calibration is stale: the weights changed after it was set; recalibrate with "
+                               "quantization.calibrate_fp8 and call set_fp8 (or set_fp8(None) for fp16 / bf16)")
 
     # -- stages --------------------------------------------------------------------------------------
     def post_config(self) -> dict:
@@ -138,6 +186,8 @@ class YOLO(nn.Module):
         # The fused decode epilogue (heads emit NMS candidates instead of logits) is functional; opt-in until it is
         # shown to be faster than storing fp16 logits + the stand-alone decode kernel.
         fuse = os.environ.get("YB_FUSED_DECODE", "0") == "1"
+        if fuse and self._fp8 is not None:
+            raise NotImplementedError("the fused decode epilogue (YB_FUSED_DECODE=1) has no FP8 variant")
         return self.engine().plan(N, H, W, self.post_config() if fuse else None, keep_intermediates, chunked and not fuse)
 
     def has_hooks(self) -> bool:
@@ -164,6 +214,9 @@ class YOLO(nn.Module):
         plan = self.get_plan(N, H, W)
         self._write_samples(plan, samples)
         plan.run_backbone()
+        if self._fp8 is not None:       # e4m3 features, dequantised (exactly) into the model's dtype
+            dt = next(self.parameters()).dtype
+            return [plan.dequantized_feature(k, dt).permute(0, 3, 1, 2).contiguous() for k in sorted(plan.features)]
         return [plan.features[k].permute(0, 3, 1, 2).clone() for k in sorted(plan.features)]
 
     def run_head(self, features: List[Tensor]) -> List[Tensor]:
@@ -171,6 +224,7 @@ class YOLO(nn.Module):
         list in training and eval mode."""
         # the canvas is the first feature map times its divisor in the lowering (not strides[0]: the lite model's first
         # map sits at stride 16 while its anchor generator says 8)
+        self._check_fp8()
         low = self.engine().lowered()
         s0 = low.feats[min(low.feats)].buf.div
         N, _, h0, w0 = (int(v) for v in features[0].shape)
@@ -183,7 +237,10 @@ class YOLO(nn.Module):
             if tuple(f.shape) != (dst.shape[0], dst.shape[3], dst.shape[1], dst.shape[2]):
                 raise ValueError(f"feature {k}: expected [N,{dst.shape[3]},{dst.shape[1]},{dst.shape[2]}], got {tuple(f.shape)}")
             _C.require_cuda(f, "head")
-            dst.copy_(f.permute(0, 2, 3, 1))       # layout change only (NCHW caller tensor -> plan NHWC buffer)
+            if self._fp8 is not None:
+                plan.quantize_feature(k, f.permute(0, 2, 3, 1))     # YB_OP_QUANTIZE into the e4m3 feature buffer
+            else:
+                dst.copy_(f.permute(0, 2, 3, 1))       # layout change only (NCHW caller tensor -> plan NHWC buffer)
         plan.run_heads()
         A, K = self.anchor_generator.num_anchors, self.num_classes + 5
         outs = []

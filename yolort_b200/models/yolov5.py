@@ -45,6 +45,16 @@ class YOLOv5(nn.Module):
                                        fill_color=fill_color)
 
     # ---------------------------------------------------------------------------------------------
+    @property
+    def precision(self) -> str:
+        """"fp8", "fp16" or "bf16": what the plans compute in (YOLO.precision)."""
+        return self.model.precision
+
+    def set_fp8(self, calib) -> None:
+        """FP8 inference with the scales of `calib` (quantization.calibrate_fp8), or None for fp16 / bf16 again
+        (YOLO.set_fp8)."""
+        self.model.set_fp8(calib)
+
     def _prepare(self, inputs: List[Tensor], batch_hw: Optional[Tuple[int, int]] = None):
         """Letterbox `inputs` straight into the plan's input canvas; returns (plan, rescale[n,3] on device)."""
         if self.training:
