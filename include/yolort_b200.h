@@ -342,6 +342,56 @@ int yb_batched_nms(const float* boxes_dev, const float* scores_dev, const int64_
                    int64_t* keep_dev, int32_t* n_keep_dev, void* workspace_dev,
                    size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Baseline JPEG decode  (replaces the reference's default loader `read_image(path, mode=RGB)`,
+ * yolort/models/yolov5.py:218-228, for the files it can take; bit-identical to that CPU decoder:
+ * libjpeg's islow IDCT, "fancy" upsampling and integer YCbCr->RGB)
+ * Subset: SOF0/SOF1, 8-bit, Huffman, one interleaved scan holding every component; 1 component (gray,
+ * replicated to RGB) or 3 components libjpeg reads as YCbCr; per-component sampling ratios 1x1, 2x1
+ * (4:2:2) and 2x2 (4:2:0); restart intervals; APPn / COM skipped.  Anything else is reported as
+ * unsupported by yb_jpeg_parse, with the reason.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  int32_t supported;           /* 1: yb_jpeg_decode takes this file; 0: `reason` says why not            */
+  char reason[92];
+  int32_t width, height;
+  int32_t ncomp;               /* 1 or 3                                                                  */
+  int32_t h_samp[3], v_samp[3];
+  int32_t restart_interval;    /* MCUs per restart interval, 0 = no DRI                                  */
+  int32_t mcus_x, mcus_y, blocks_per_mcu;
+  int64_t scan_begin, scan_end; /* the entropy-coded segment: file bytes [scan_begin, scan_end)           */
+  int64_t data_offset;         /* set by the caller: where byte 0 of the file lies in yb_jpeg_decode's src */
+  uint16_t quant[3][64];       /* per component, natural (row-major) order                               */
+  uint8_t dc_bits[3][16], ac_bits[3][16]; /* per component: number of codes of length 1..16             */
+  uint8_t dc_vals[3][16];
+  uint8_t ac_vals[3][256];
+} yb_jpeg_info;
+
+/* status bits of yb_jpeg_decode, per image (0 = decoded cleanly) */
+#define YB_JPEG_ST_HUFFMAN 1   /* a bit pattern that is no code of its table                             */
+#define YB_JPEG_ST_COEF 2      /* a run that moves the coefficient index past 63                          */
+#define YB_JPEG_ST_TRUNCATED 4 /* the data ends before the last MCU, an interval holds the wrong number of
+                                  MCUs, or data follows the last MCU                                      */
+#define YB_JPEG_ST_RESTART 8   /* a restart marker out of sequence, missing or unexpected                 */
+#define YB_JPEG_ST_RANGE 16    /* an IDCT value outside [-512, 511] (or a 16-bit overflow): libjpeg's C and
+                                  SIMD code disagree there, so the CPU decoder is the one to ask          */
+
+/* Host-only: reads the markers of `data` (nothing in it is trusted: every length and table is checked)
+ * and fills `info`.  Returns YB_OK for any input; info->supported says whether the device decoder takes it. */
+int yb_jpeg_parse(const uint8_t* data, int64_t len, yb_jpeg_info* info);
+
+/* Host-only: workspace yb_jpeg_decode needs for these images (all of them supported). */
+size_t yb_jpeg_workspace_bytes(int n, const yb_jpeg_info* infos);
+
+/* Decodes n files on `stream` without a host synchronisation.  `infos` (host) are yb_jpeg_parse results with
+ * data_offset filled in; `src_dev` starts with a copy of infos[0..n) (n * sizeof(yb_jpeg_info) bytes, so one
+ * host-to-device copy carries tables and compressed bytes together) and holds file i at src_dev +
+ * infos[i].data_offset.  dst_dev[i] (a host array of device pointers) receives image i as HWC uint8 RGB,
+ * height x width x 3, rows packed.  status_dev: int32[n], YB_JPEG_ST_* bits per image; a nonzero image's pixels
+ * are undefined.  The kernels touch no byte of dst outside each image's extent. */
+int yb_jpeg_decode(int n, const yb_jpeg_info* infos, const void* src_dev, uint8_t* const* dst_dev,
+                   int32_t* status_dev, void* workspace_dev, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,6 +5,7 @@ PyTorch is used here only as the owner of device memory and streams: every wrapp
 library is missing, or a wrapper is asked to run without a CUDA device, it raises.
 """
 import ctypes
+import itertools
 import os
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -47,6 +48,9 @@ EXPORTED_SYMBOLS = (
     "yb_decode_candidates",
     "yb_batched_nms_workspace_bytes",
     "yb_batched_nms",
+    "yb_jpeg_parse",
+    "yb_jpeg_workspace_bytes",
+    "yb_jpeg_decode",
 )
 
 
@@ -135,6 +139,24 @@ class NmsParams(ctypes.Structure):
     ]
 
 
+class JpegInfo(ctypes.Structure):
+    """yb_jpeg_info: what yb_jpeg_parse reads from a file's markers (include/yolort_b200.h)."""
+    _fields_ = [
+        ("supported", ctypes.c_int32), ("reason", ctypes.c_char * 92),
+        ("width", ctypes.c_int32), ("height", ctypes.c_int32), ("ncomp", ctypes.c_int32),
+        ("h_samp", ctypes.c_int32 * 3), ("v_samp", ctypes.c_int32 * 3),
+        ("restart_interval", ctypes.c_int32),
+        ("mcus_x", ctypes.c_int32), ("mcus_y", ctypes.c_int32), ("blocks_per_mcu", ctypes.c_int32),
+        ("scan_begin", ctypes.c_int64), ("scan_end", ctypes.c_int64), ("data_offset", ctypes.c_int64),
+        ("quant", (ctypes.c_uint16 * 64) * 3),
+        ("dc_bits", (ctypes.c_uint8 * 16) * 3), ("ac_bits", (ctypes.c_uint8 * 16) * 3),
+        ("dc_vals", (ctypes.c_uint8 * 16) * 3),
+        ("ac_vals", (ctypes.c_uint8 * 256) * 3),
+    ]
+
+
+YB_JPEG_ST_HUFFMAN, YB_JPEG_ST_COEF, YB_JPEG_ST_TRUNCATED, YB_JPEG_ST_RESTART, YB_JPEG_ST_RANGE = 1, 2, 4, 8, 16
+
 _lib = None
 
 
@@ -199,6 +221,11 @@ def lib() -> ctypes.CDLL:
     L.yb_batched_nms.argtypes = [
         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_float, ctypes.c_int,
         ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
+    L.yb_jpeg_parse.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.POINTER(JpegInfo)]
+    L.yb_jpeg_workspace_bytes.restype = ctypes.c_size_t
+    L.yb_jpeg_workspace_bytes.argtypes = [ctypes.c_int, ctypes.POINTER(JpegInfo)]
+    L.yb_jpeg_decode.argtypes = [ctypes.c_int, ctypes.POINTER(JpegInfo), ctypes.c_void_p, ctypes.POINTER(ctypes.c_void_p),
+                                 ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
     _lib = L
     return L
 
@@ -602,3 +629,94 @@ def batched_nms(boxes: torch.Tensor, scores: torch.Tensor, labels: torch.Tensor,
                                    int(semantics), int(max_keep), keep.data_ptr(), n_keep.data_ptr(), ws.data_ptr(),
                                    ws.numel(), current_stream_ptr(dev)), "yb_batched_nms")
     return keep[: int(n_keep.item())]
+
+
+# ---------------------------------------------------------------------------------------------------
+# JPEG decode
+# ---------------------------------------------------------------------------------------------------
+def jpeg_parse(data: bytes) -> JpegInfo:
+    """Host-only marker parse (yb_jpeg_parse); `.supported` says whether jpeg_decode takes the file."""
+    info = JpegInfo()
+    buf = (ctypes.c_uint8 * len(data)).from_buffer_copy(data) if len(data) else None
+    check(lib().yb_jpeg_parse(buf, len(data), ctypes.byref(info)), "yb_jpeg_parse")
+    return info
+
+
+_jpeg_staging: Dict[torch.device, dict] = {}
+
+
+def _jpeg_stage(device: torch.device, nbytes: int) -> list:
+    """A pinned host buffer of >= nbytes for the next decode on `device`: two alternate, and the copy out of a buffer
+    must have finished before it is refilled (fresh pinned allocations cost about as much as the decode itself)."""
+    st = _jpeg_staging.setdefault(device, {"slots": [None, None], "next": 0})
+    k = st["next"]
+    st["next"] = k ^ 1
+    slot = st["slots"][k]
+    if slot is not None and slot[1] is not None:
+        slot[1].synchronize()
+    if slot is None or slot[0].numel() < nbytes:
+        slot = [torch.empty((max(nbytes + nbytes // 4, 1 << 20),), dtype=torch.uint8, pin_memory=True), None]
+        st["slots"][k] = slot
+    return slot
+
+
+def jpeg_decode(datas: Sequence, infos: Sequence[JpegInfo], device: torch.device,
+                dst: Optional[Sequence[torch.Tensor]] = None):
+    """Decodes supported JPEG files (bytes, or 1-D uint8 host tensors, with their parse results) on `device`'s
+    current stream.  The infos and the compressed bytes cross PCIe as one copy from pinned memory.  Returns ([3,H,W]
+    uint8 CHW views of HWC memory, status int32 [n] on the device); nothing is synchronised.  `dst` optionally gives
+    the contiguous [H,W,3] uint8 device tensors to write into."""
+    device = torch.device(device)
+    if device.type != "cuda":
+        raise NativeLibraryError("jpeg_decode runs on a CUDA device only (no CPU fallback)")
+    if device.index is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    n = len(datas)
+    isz = ctypes.sizeof(JpegInfo)
+    arr = (JpegInfo * n)()
+    off = (n * isz + 15) // 16 * 16
+    lens = []
+    for i, (d, info) in enumerate(zip(datas, infos)):
+        if not info.supported:
+            raise NativeLibraryError(f"jpeg_decode: image {i} is not supported: {info.reason.decode()}")
+        ctypes.memmove(ctypes.byref(arr[i]), ctypes.byref(info), isz)
+        arr[i].data_offset = off
+        lens.append(int(d.numel()) if isinstance(d, torch.Tensor) else len(d))
+        off += (lens[-1] + 15) // 16 * 16
+    slot = _jpeg_stage(device, off)
+    base = slot[0].data_ptr()
+    ctypes.memmove(base, ctypes.addressof(arr), n * isz)
+    for i, d in enumerate(datas):
+        if isinstance(d, torch.Tensor):
+            if d.is_cuda or d.dtype != torch.uint8 or d.dim() != 1:
+                raise NativeLibraryError("jpeg_decode: file contents must be 1-D uint8 host tensors or bytes")
+            d = d.contiguous()
+            ctypes.memmove(base + int(arr[i].data_offset), d.data_ptr(), lens[i])
+        else:
+            ctypes.memmove(base + int(arr[i].data_offset), bytes(d), lens[i])
+    host = slot[0][:off]
+    ws_bytes = int(lib().yb_jpeg_workspace_bytes(n, arr))
+    with device_guard(device):
+        src = host.to(device, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(device))
+        slot[1] = ev
+        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=device)
+        sizes = [int(a.height) * int(a.width) * 3 for a in arr]
+        if dst is None:
+            out = torch.empty((sum(sizes),), dtype=torch.uint8, device=device)
+            offs = [0] + list(itertools.accumulate(sizes))[:-1]
+            dst = [out[o:o + sz].view(int(a.height), int(a.width), 3) for o, sz, a in zip(offs, sizes, arr)]
+        status = torch.empty((n,), dtype=torch.int32, device=device)
+        ptrs = (ctypes.c_void_p * n)()
+        images = []
+        for i, (a, t) in enumerate(zip(arr, dst)):
+            if (t.device != device or t.dtype != torch.uint8 or not t.is_contiguous()
+                    or tuple(t.shape) != (int(a.height), int(a.width), 3)):
+                raise NativeLibraryError(f"jpeg_decode: dst[{i}] must be a contiguous uint8 [{a.height},{a.width},3] "
+                                         f"tensor on {device}")
+            ptrs[i] = t.data_ptr()
+            images.append(t.permute(2, 0, 1))
+        check(lib().yb_jpeg_decode(n, arr, src.data_ptr(), ptrs, status.data_ptr(), ws.data_ptr(), ws_bytes,
+                                   current_stream_ptr(device)), "yb_jpeg_decode")
+    return images, status

@@ -271,17 +271,51 @@ class YOLOv5(nn.Module):
     _DECODE_THREADS = 8
 
     def _ingest_files(self, paths: List[str], device: torch.device) -> List[Tensor]:
-        """`predict(paths)` fast path: CPU decode (nvJPEG is third-party; torchvision's decoder releases the GIL, so
-        files decode on a small thread pool), the decoder's interleaved HWC bytes are packed into ONE pinned staging
-        buffer and cross PCIe as a single asynchronous copy; the letterbox kernel reads HWC uint8 in place
-        (`yb_letterbox_strided`), so there is no repacking pass on either side and `/255` stays in the kernel."""
+        """`predict(paths)` fast path.  The files are read (and their headers parsed) on a small thread pool.  JPEGs
+        the device decoder takes (yolort_b200.io) cross PCIe compressed, in one copy, and decode on the GPU to the
+        bytes torchvision's CPU decoder gives; every other file is decoded on the CPU as before.  An image whose
+        device decode reports corrupt data is decoded again on the CPU, so it warns, fills or raises exactly as
+        before.  YB_JPEG_DECODE=cpu decodes everything on the CPU (A/B runs)."""
+        import os
+
+        on_gpu = os.environ.get("YB_JPEG_DECODE", "").lower() != "cpu"
+
+        def load(path):
+            if on_gpu:
+                with open(path, "rb") as f:
+                    data = f.read()
+                info = _C.jpeg_parse(data)
+                if info.supported:
+                    return data, info
+            return self.default_loader(path)
+
         if len(paths) > 1:
             from concurrent.futures import ThreadPoolExecutor
 
             with ThreadPoolExecutor(max_workers=min(self._DECODE_THREADS, len(paths))) as pool:
-                decoded = list(pool.map(self.default_loader, paths))
+                loaded = list(pool.map(load, paths))
         else:
-            decoded = [self.default_loader(paths[0])]
+            loaded = [load(paths[0])]
+        out: List[Optional[Tensor]] = [None] * len(paths)
+        jpeg = [i for i, t in enumerate(loaded) if not isinstance(t, Tensor)]
+        if jpeg:
+            images, status = _C.jpeg_decode([loaded[i][0] for i in jpeg], [loaded[i][1] for i in jpeg], device)
+            bad = status.cpu().tolist()        # waits for this stream's decode only
+            for k, i in enumerate(jpeg):
+                if bad[k]:
+                    loaded[i] = self.default_loader(paths[i])
+                else:
+                    out[i] = images[k]
+        cpu = [i for i, t in enumerate(loaded) if isinstance(t, Tensor)]
+        if cpu:
+            for i, t in zip(cpu, self._stage_decoded([loaded[i] for i in cpu], device)):
+                out[i] = t
+        return out
+
+    def _stage_decoded(self, decoded: List[Tensor], device: torch.device) -> List[Tensor]:
+        """CPU-decoded images: the decoder's interleaved HWC bytes are packed into ONE pinned staging buffer and
+        cross PCIe as a single asynchronous copy; the letterbox kernel reads HWC uint8 in place
+        (`yb_letterbox_strided`), so there is no repacking pass on either side and `/255` stays in the kernel."""
         total = sum(t.numel() for t in decoded)
         slots = self.__dict__.setdefault("_ingest_slots", [None, None])   # double-buffered pinned staging
         k = self.__dict__.get("_ingest_next", 0)
