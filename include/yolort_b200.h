@@ -392,6 +392,54 @@ size_t yb_jpeg_workspace_bytes(int n, const yb_jpeg_info* infos);
 int yb_jpeg_decode(int n, const yb_jpeg_info* infos, const void* src_dev, uint8_t* const* dst_dev,
                    int32_t* status_dev, void* workspace_dev, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * COCO box evaluation  (replaces pycocotools' COCOeval.evaluate + accumulate behind the reference's
+ * COCOEvaluator, yolort/data/coco_eval.py:28-217, iouType "bbox"; the protocol is restated rule by rule in
+ * oracle/restate_cocoeval.py and reproduced bit for bit)
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {               /* host struct of device pointers, uploaded once per annotation file          */
+  int32_t n_images;            /* image index i = the i-th smallest image id of the file                      */
+  int32_t n_categories;        /* K; category index k = the k-th smallest category id                         */
+  int32_t n_gt;                /* annotations                                                                 */
+  int32_t max_gt_per_pair;     /* most annotations of one (image, category)                                   */
+  const int32_t* img_start;    /* [n_images+1]: the annotations of image i are [img_start[i], img_start[i+1])  */
+  const int32_t* gt_img;       /* [n_gt] image index                                                          */
+  const int32_t* gt_cat;       /* [n_gt] category index: ascending within an image, file order within a pair  */
+  const double* gt_box;        /* [n_gt][4] x, y, w, h as in the file (16-byte aligned)                       */
+  const double* gt_area;       /* [n_gt] the annotation's `area` field                                        */
+  const uint8_t* gt_flags;     /* [n_gt] YB_COCO_GT_* bits                                                    */
+} yb_coco_gt;
+
+#define YB_COCO_GT_CROWD 1          /* iscrowd != 0: ignored, and its IoU's union is the detection's area      */
+#define YB_COCO_GT_ID_NONZERO 2     /* a match to an annotation whose id is 0 counts as no match               */
+#define YB_COCO_ST_UNKNOWN_IMAGE 1  /* status bit: a detection on an image the file does not have             */
+#define YB_COCO_ST_BAD_LABEL 2      /* status bit: a label outside the label map                               */
+#define YB_COCO_ROW_DROPPED (-2)    /* row_image value: skip the row (its image was evaluated before)          */
+#define YB_COCO_RECORD_INT32 8      /* one stored detection: image, position, category (-1: not evaluated),
+                                       score bits, then x, y, w, h as fp32 bits                               */
+#define YB_COCO_NUM_PARAMS 119      /* float64 iouThrs[10] | recThrs[101] | areaRng[4][2]                     */
+
+/* Appends an n x d padded batch (forward_padded's layout: boxes xyxy fp32 [n,d,4], scores fp32 [n,d], labels
+ * int64 [n,d], counts int32 [n]) as n*d records at records_dev (16-byte aligned).  row_image_dev: int32 [n],
+ * the image index of each row, -1 for an image id the file does not have, or YB_COCO_ROW_DROPPED.
+ * label_map_dev: int32 [n_labels], label -> category index, -1 for a category the file does not have.  Slots
+ * at or past counts[row] are stored as not evaluated.  Errors found in the data are ORed into *status_dev
+ * (YB_COCO_ST_*).  No host synchronisation. */
+int yb_coco_append(int n, int d, const float* boxes_dev, const float* scores_dev, const int64_t* labels_dev,
+                   const int32_t* counts_dev, const int32_t* row_image_dev, const int32_t* label_map_dev,
+                   int32_t n_labels, int32_t* records_dev, int32_t* status_dev, void* stream);
+
+/* Host-only: workspace yb_coco_evaluate needs for n_records records against `gt`. */
+size_t yb_coco_evaluate_workspace_bytes(int64_t n_records, const yb_coco_gt* gt);
+
+/* Evaluates the stored records against `gt` over the images with evaluated_dev[i] != 0 (uint8 [n_images]; every
+ * record must lie on such an image).  params_dev: YB_COCO_NUM_PARAMS float64 values.  Writes COCOeval.eval's
+ * arrays as float64: precision_dev and scores_dev [10][101][K][4][3], recall_dev [10][K][4][3], -1 where
+ * pycocotools leaves -1.  No host synchronisation. */
+int yb_coco_evaluate(const yb_coco_gt* gt, const int32_t* records_dev, int64_t n_records, const uint8_t* evaluated_dev,
+                     const double* params_dev, double* precision_dev, double* recall_dev, double* scores_dev,
+                     void* workspace_dev, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -51,6 +51,9 @@ EXPORTED_SYMBOLS = (
     "yb_jpeg_parse",
     "yb_jpeg_workspace_bytes",
     "yb_jpeg_decode",
+    "yb_coco_append",
+    "yb_coco_evaluate_workspace_bytes",
+    "yb_coco_evaluate",
 )
 
 
@@ -157,6 +160,21 @@ class JpegInfo(ctypes.Structure):
 
 YB_JPEG_ST_HUFFMAN, YB_JPEG_ST_COEF, YB_JPEG_ST_TRUNCATED, YB_JPEG_ST_RESTART, YB_JPEG_ST_RANGE = 1, 2, 4, 8, 16
 
+
+class CocoGt(ctypes.Structure):
+    """yb_coco_gt: an annotation file's GT in the layout the evaluation kernels read (include/yolort_b200.h)."""
+    _fields_ = [
+        ("n_images", ctypes.c_int32), ("n_categories", ctypes.c_int32), ("n_gt", ctypes.c_int32),
+        ("max_gt_per_pair", ctypes.c_int32),
+        ("img_start", ctypes.c_void_p), ("gt_img", ctypes.c_void_p), ("gt_cat", ctypes.c_void_p),
+        ("gt_box", ctypes.c_void_p), ("gt_area", ctypes.c_void_p), ("gt_flags", ctypes.c_void_p),
+    ]
+
+
+YB_COCO_GT_CROWD, YB_COCO_GT_ID_NONZERO = 1, 2
+YB_COCO_ST_UNKNOWN_IMAGE, YB_COCO_ST_BAD_LABEL = 1, 2
+YB_COCO_ROW_DROPPED, YB_COCO_RECORD_INT32, YB_COCO_NUM_PARAMS = -2, 8, 119
+
 _lib = None
 
 
@@ -226,6 +244,12 @@ def lib() -> ctypes.CDLL:
     L.yb_jpeg_workspace_bytes.argtypes = [ctypes.c_int, ctypes.POINTER(JpegInfo)]
     L.yb_jpeg_decode.argtypes = [ctypes.c_int, ctypes.POINTER(JpegInfo), ctypes.c_void_p, ctypes.POINTER(ctypes.c_void_p),
                                  ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
+    L.yb_coco_append.argtypes = [ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 6 + [ctypes.c_int32] + \
+        [ctypes.c_void_p] * 3
+    L.yb_coco_evaluate_workspace_bytes.restype = ctypes.c_size_t
+    L.yb_coco_evaluate_workspace_bytes.argtypes = [ctypes.c_int64, ctypes.POINTER(CocoGt)]
+    L.yb_coco_evaluate.argtypes = [ctypes.POINTER(CocoGt), ctypes.c_void_p, ctypes.c_int64] + [ctypes.c_void_p] * 6 + \
+        [ctypes.c_size_t, ctypes.c_void_p]
     _lib = L
     return L
 
@@ -720,3 +744,55 @@ def jpeg_decode(datas: Sequence, infos: Sequence[JpegInfo], device: torch.device
         check(lib().yb_jpeg_decode(n, arr, src.data_ptr(), ptrs, status.data_ptr(), ws.data_ptr(), ws_bytes,
                                    current_stream_ptr(device)), "yb_jpeg_decode")
     return images, status
+
+
+# ---------------------------------------------------------------------------------------------------
+# COCO box evaluation
+# ---------------------------------------------------------------------------------------------------
+def coco_append(boxes: torch.Tensor, scores: torch.Tensor, labels: torch.Tensor, counts: torch.Tensor,
+                row_image: torch.Tensor, label_map: torch.Tensor, records: torch.Tensor, status: torch.Tensor) -> None:
+    """yb_coco_append on the current stream of `records`' device: boxes fp32 [n,d,4], scores fp32 [n,d], labels int64
+    [n,d], counts int32 [n], row_image int32 [n], label_map int32 [L]; records int32 [n*d, 8]; status int32 [1]."""
+    dev = records.device
+    if dev.type != "cuda":
+        raise NativeLibraryError("coco_append runs on a CUDA device only (no CPU fallback)")
+    n, d = int(scores.shape[0]), int(scores.shape[1])
+    ts = (boxes, scores, labels, counts, row_image, label_map, records, status)
+    want = (torch.float32, torch.float32, torch.int64, torch.int32, torch.int32, torch.int32, torch.int32, torch.int32)
+    for t, dt in zip(ts, want):
+        if t.device != dev or t.dtype != dt or not t.is_contiguous():
+            raise NativeLibraryError(f"coco_append: every tensor must be a contiguous {dt} tensor on {dev}")
+    if tuple(boxes.shape) != (n, d, 4) or tuple(labels.shape) != (n, d) or counts.numel() != n \
+            or row_image.numel() != n or tuple(records.shape) != (n * d, YB_COCO_RECORD_INT32):
+        raise NativeLibraryError("coco_append: shapes do not agree")
+    with device_guard(dev):
+        check(lib().yb_coco_append(n, d, boxes.data_ptr(), scores.data_ptr(), labels.data_ptr(), counts.data_ptr(),
+                                   row_image.data_ptr(), label_map.data_ptr(), label_map.numel(), records.data_ptr(),
+                                   status.data_ptr(), current_stream_ptr(dev)), "yb_coco_append")
+
+
+def coco_evaluate(gt: CocoGt, records: torch.Tensor, evaluated: torch.Tensor, params: torch.Tensor):
+    """yb_coco_evaluate: records int32 [n, 8], evaluated uint8 [n_images], params float64 [119], all on one CUDA device.
+    Returns float64 device tensors precision [10,101,K,4,3], recall [10,K,4,3], scores [10,101,K,4,3]."""
+    dev = records.device
+    if dev.type != "cuda":
+        raise NativeLibraryError("coco_evaluate runs on a CUDA device only (no CPU fallback)")
+    for t, dt in ((records, torch.int32), (evaluated, torch.uint8), (params, torch.float64)):
+        if t.device != dev or t.dtype != dt or not t.is_contiguous():
+            raise NativeLibraryError(f"coco_evaluate: expected a contiguous {dt} tensor on {dev}")
+    if evaluated.numel() != gt.n_images or params.numel() != YB_COCO_NUM_PARAMS:
+        raise NativeLibraryError("coco_evaluate: evaluated / params have the wrong size")
+    n = int(records.shape[0])
+    K = int(gt.n_categories)
+    with device_guard(dev):
+        ws_bytes = int(lib().yb_coco_evaluate_workspace_bytes(n, ctypes.byref(gt)))
+        if ws_bytes == 0:
+            raise NativeLibraryError(f"coco_evaluate: no workspace size for {n} records: {lib().yb_last_error()}")
+        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+        precision = torch.empty((10, 101, K, 4, 3), dtype=torch.float64, device=dev)
+        recall = torch.empty((10, K, 4, 3), dtype=torch.float64, device=dev)
+        scores = torch.empty_like(precision)
+        check(lib().yb_coco_evaluate(ctypes.byref(gt), records.data_ptr() if n else None, n, evaluated.data_ptr(),
+                                     params.data_ptr(), precision.data_ptr(), recall.data_ptr(), scores.data_ptr(),
+                                     ws.data_ptr(), ws_bytes, current_stream_ptr(dev)), "yb_coco_evaluate")
+    return precision, recall, scores
