@@ -440,6 +440,64 @@ int yb_coco_evaluate(const yb_coco_gt* gt, const int32_t* records_dev, int64_t n
                      const double* params_dev, double* precision_dev, double* recall_dev, double* scores_dev,
                      void* workspace_dev, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * YOLOv5 training loss  (the reference's SetCriterion, yolort/models/box_head.py:85-325: target assignment
+ * :233-325, CIoU box loss :190-195 with yolort/models/_utils.py:26-40 / :65-108, objectness :197-217, class
+ * loss :205-212, gains :223-225; restated rule by rule in oracle/restate_loss.py)
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  const void* logits;          /* head output [N, A, H, W, K], contiguous, K = n_classes + 5                   */
+  int32_t dtype;               /* YB_F32 / YB_F16 / YB_BF16                                                   */
+  int32_t H, W;                /* the level's grid (the gain of box_head.py:271 is W, H, W, H)                 */
+  float stride_px;             /* anchors are divided by it in fp32 (box_head.py:167-171)                      */
+  float anchors_px[2 * YB_MAX_ANCHORS];  /* (w, h) per anchor in pixels                                       */
+} yb_loss_level;
+
+typedef struct {
+  int32_t n_images, n_levels, n_anchors, n_classes;  /* N, L <= YB_MAX_LEVELS, A <= YB_MAX_ANCHORS, nc       */
+  float box_gain, cls_gain, obj_gain;  /* box_head.py:223-225                                                 */
+  float cls_pos, obj_pos;      /* BCE pos_weight of the class and objectness terms (:175-176)                  */
+  float anchor_thresh;         /* ratio test max(r, 1/r) < anchor_thresh, compared in fp32 (:278)              */
+  float smooth_pos, smooth_neg;  /* class targets (:140-141, _utils.py:111-114)                               */
+  float gr;                    /* objectness target (1 - gr) + gr * clamp(CIoU, 0) (:203)                      */
+  float balance[YB_MAX_LEVELS];  /* objectness weight per level (:217)                                        */
+} yb_yolo_loss_params;
+
+#define YB_LOSS_ST_IMAGE 1          /* status bit: a target's image index is outside [0, N)                  */
+#define YB_LOSS_ST_CLASS 2          /* status bit: a target's class is outside [0, nc)                        */
+#define YB_LOSS_ST_NONFINITE 4      /* status bit: a target's cx, cy, w or h is not finite                    */
+#define YB_LOSS_MATCH_INT32 24      /* one match record: level, b, a, gj, gi, class, cell, 0, tbox[4] (fp32),
+                                       anchor[2] (fp32, grid units), objectness target, 1 - CIoU, then
+                                       d box loss / d logit[4] and the class BCE sum (fp32), 3 unused words   */
+
+/* Host-only: workspace the loss needs for n_targets targets over these levels (0 for an invalid request). */
+size_t yb_yolo_loss_workspace_bytes(const yb_yolo_loss_params* params, const yb_loss_level* levels,
+                                    int64_t n_targets);
+
+/* Host-only: where the matches live in the workspace.  out[0] = byte offset of the match records
+ * (YB_LOSS_MATCH_INT32 words each, ordered level, then offset, anchor, target as box_head.py:297 does),
+ * out[1] = byte offset of the int32 match counts: element l * 5 * A * n_targets is the index of level l's first
+ * match, element n_levels * 5 * A * n_targets the total.  out[2] = the record capacity. */
+int yb_yolo_loss_layout(const yb_yolo_loss_params* params, const yb_loss_level* levels, int64_t n_targets,
+                        int64_t* out);
+
+/* Forward.  targets_dev: fp32 [n_targets, 6] (image, class, cx, cy, w, h), normalised to the canvas.  Writes
+ * out_losses_dev: fp32 [3 + n_levels] = loss_cls, loss_box, loss_obj (gains applied) and each level's
+ * objectness mean before its balance.  Invalid targets OR YB_LOSS_ST_* bits into *status_dev and take no part; no
+ * thread reads outside the arrays.  No host synchronisation, no float atomics: a repeated call gives the same bits.
+ * The workspace keeps what yb_yolo_loss_backward needs. */
+int yb_yolo_loss_forward(const yb_yolo_loss_params* params, const yb_loss_level* levels, const float* targets_dev,
+                         int64_t n_targets, float* out_losses_dev, int32_t* status_dev, void* workspace_dev,
+                         size_t workspace_bytes, void* stream);
+
+/* Backward of the forward call that filled `workspace_dev` (same params, levels and n_targets).  grad_losses_dev:
+ * fp32 [3], the incoming gradients of loss_cls, loss_box, loss_obj.  grad_out_levels[l] (host array of device
+ * pointers) receives d loss / d logits of level l, in that level's dtype and layout, every element written once,
+ * computed in fp32 and rounded once.  Matches that share a cell are summed in match order. */
+int yb_yolo_loss_backward(const yb_yolo_loss_params* params, const yb_loss_level* levels, int64_t n_targets,
+                          const float* grad_losses_dev, void* const* grad_out_levels, void* workspace_dev,
+                          size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -54,6 +54,10 @@ EXPORTED_SYMBOLS = (
     "yb_coco_append",
     "yb_coco_evaluate_workspace_bytes",
     "yb_coco_evaluate",
+    "yb_yolo_loss_workspace_bytes",
+    "yb_yolo_loss_layout",
+    "yb_yolo_loss_forward",
+    "yb_yolo_loss_backward",
 )
 
 
@@ -175,6 +179,30 @@ YB_COCO_GT_CROWD, YB_COCO_GT_ID_NONZERO = 1, 2
 YB_COCO_ST_UNKNOWN_IMAGE, YB_COCO_ST_BAD_LABEL = 1, 2
 YB_COCO_ROW_DROPPED, YB_COCO_RECORD_INT32, YB_COCO_NUM_PARAMS = -2, 8, 119
 
+
+class LossLevel(ctypes.Structure):
+    """yb_loss_level: one head output of the training loss (include/yolort_b200.h)."""
+    _fields_ = [
+        ("logits", ctypes.c_void_p), ("dtype", ctypes.c_int32), ("H", ctypes.c_int32), ("W", ctypes.c_int32),
+        ("stride_px", ctypes.c_float), ("anchors_px", ctypes.c_float * (2 * YB_MAX_ANCHORS)),
+    ]
+
+
+class YoloLossParams(ctypes.Structure):
+    """yb_yolo_loss_params: SetCriterion's hyperparameters (include/yolort_b200.h)."""
+    _fields_ = [
+        ("n_images", ctypes.c_int32), ("n_levels", ctypes.c_int32), ("n_anchors", ctypes.c_int32),
+        ("n_classes", ctypes.c_int32),
+        ("box_gain", ctypes.c_float), ("cls_gain", ctypes.c_float), ("obj_gain", ctypes.c_float),
+        ("cls_pos", ctypes.c_float), ("obj_pos", ctypes.c_float), ("anchor_thresh", ctypes.c_float),
+        ("smooth_pos", ctypes.c_float), ("smooth_neg", ctypes.c_float), ("gr", ctypes.c_float),
+        ("balance", ctypes.c_float * YB_MAX_LEVELS),
+    ]
+
+
+YB_LOSS_ST_IMAGE, YB_LOSS_ST_CLASS, YB_LOSS_ST_NONFINITE = 1, 2, 4
+YB_LOSS_MATCH_INT32 = 24
+
 _lib = None
 
 
@@ -250,6 +278,16 @@ def lib() -> ctypes.CDLL:
     L.yb_coco_evaluate_workspace_bytes.argtypes = [ctypes.c_int64, ctypes.POINTER(CocoGt)]
     L.yb_coco_evaluate.argtypes = [ctypes.POINTER(CocoGt), ctypes.c_void_p, ctypes.c_int64] + [ctypes.c_void_p] * 6 + \
         [ctypes.c_size_t, ctypes.c_void_p]
+    L.yb_yolo_loss_workspace_bytes.restype = ctypes.c_size_t
+    L.yb_yolo_loss_workspace_bytes.argtypes = [ctypes.POINTER(YoloLossParams), ctypes.POINTER(LossLevel), ctypes.c_int64]
+    L.yb_yolo_loss_layout.argtypes = [ctypes.POINTER(YoloLossParams), ctypes.POINTER(LossLevel), ctypes.c_int64,
+                                      ctypes.POINTER(ctypes.c_int64)]
+    L.yb_yolo_loss_forward.argtypes = [ctypes.POINTER(YoloLossParams), ctypes.POINTER(LossLevel), ctypes.c_void_p,
+                                       ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t,
+                                       ctypes.c_void_p]
+    L.yb_yolo_loss_backward.argtypes = [ctypes.POINTER(YoloLossParams), ctypes.POINTER(LossLevel), ctypes.c_int64,
+                                        ctypes.c_void_p, ctypes.POINTER(ctypes.c_void_p), ctypes.c_void_p,
+                                        ctypes.c_size_t, ctypes.c_void_p]
     _lib = L
     return L
 
@@ -796,3 +834,62 @@ def coco_evaluate(gt: CocoGt, records: torch.Tensor, evaluated: torch.Tensor, pa
                                      params.data_ptr(), precision.data_ptr(), recall.data_ptr(), scores.data_ptr(),
                                      ws.data_ptr(), ws_bytes, current_stream_ptr(dev)), "yb_coco_evaluate")
     return precision, recall, scores
+
+
+# ---------------------------------------------------------------------------------------------------
+# YOLOv5 training loss
+# ---------------------------------------------------------------------------------------------------
+def yolo_loss_levels(head_outputs: Sequence[torch.Tensor], strides: Sequence[int],
+                     anchors_px: Sequence[Sequence[float]]):
+    """yb_loss_level array over contiguous [N, A, H, W, K] head outputs (one dtype, one device)."""
+    levels = (LossLevel * len(head_outputs))()
+    for i, t in enumerate(head_outputs):
+        lv = levels[i]
+        lv.logits = t.data_ptr()
+        lv.dtype = dtype_code(t.dtype)
+        lv.H, lv.W = int(t.shape[2]), int(t.shape[3])
+        lv.stride_px = float(strides[i])
+        for j, v in enumerate(anchors_px[i]):
+            lv.anchors_px[j] = float(v)
+    return levels
+
+
+def yolo_loss_forward(params: YoloLossParams, levels, targets: torch.Tensor, device: torch.device):
+    """yb_yolo_loss_forward on `device`'s current stream.  targets: contiguous fp32 [T, 6] on the device.  Returns
+    (losses fp32 [3 + L], status int32 [1], workspace uint8); nothing is synchronised."""
+    n = int(targets.shape[0])
+    ws_bytes = int(lib().yb_yolo_loss_workspace_bytes(ctypes.byref(params), levels, n))
+    if ws_bytes == 0:
+        raise NativeLibraryError(f"yolo_loss: {lib().yb_last_error().decode('utf-8', 'replace')}")
+    with device_guard(device):
+        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=device)
+        out = torch.empty((3 + params.n_levels,), dtype=torch.float32, device=device)
+        status = torch.zeros((1,), dtype=torch.int32, device=device)
+        check(lib().yb_yolo_loss_forward(ctypes.byref(params), levels, targets.data_ptr() if n else None, n,
+                                         out.data_ptr(), status.data_ptr(), ws.data_ptr(), ws_bytes,
+                                         current_stream_ptr(device)), "yb_yolo_loss_forward")
+    return out, status, ws
+
+
+def yolo_loss_backward(params: YoloLossParams, levels, n_targets: int, grad_losses: torch.Tensor, ws: torch.Tensor,
+                       grads: Sequence[torch.Tensor]) -> None:
+    """yb_yolo_loss_backward: writes d loss / d logits into `grads` (contiguous, shaped and typed as the head
+    outputs) from grad_losses fp32 [3] on the device."""
+    dev = ws.device
+    ptrs = (ctypes.c_void_p * len(grads))(*[g.data_ptr() for g in grads])
+    with device_guard(dev):
+        check(lib().yb_yolo_loss_backward(ctypes.byref(params), levels, int(n_targets), grad_losses.data_ptr(), ptrs,
+                                          ws.data_ptr(), ws.numel(), current_stream_ptr(dev)), "yb_yolo_loss_backward")
+
+
+def yolo_loss_matches(params: YoloLossParams, levels, n_targets: int, ws: torch.Tensor):
+    """The matches a forward call left in `ws` (test and debugging aid; synchronises): (records int32 [M, 24],
+    start index of each level's matches + the total, as a list)."""
+    out = (ctypes.c_int64 * 3)()
+    check(lib().yb_yolo_loss_layout(ctypes.byref(params), levels, int(n_targets), out), "yb_yolo_loss_layout")
+    cap = int(out[2])
+    per_level = cap // params.n_levels if params.n_levels else 0
+    pos = ws[int(out[1]): int(out[1]) + 4 * (cap + 1)].view(torch.int32).cpu()
+    bounds = [int(pos[l * per_level]) for l in range(params.n_levels)] + [int(pos[cap])]
+    rec = ws[int(out[0]): int(out[0]) + 4 * YB_LOSS_MATCH_INT32 * bounds[-1]].view(torch.int32)
+    return rec.view(-1, YB_LOSS_MATCH_INT32).cpu(), bounds

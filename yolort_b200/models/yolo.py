@@ -303,12 +303,13 @@ class YOLO(nn.Module):
             features = self.backbone(samples)
             head_outputs = self.head(features)
             if self.training:
-                # the training-mode output of the head is the raw per-level list; the loss itself (SetCriterion,
-                # box_head.py:85-325) is out of scope, a caller-supplied criterion receives what the reference passes
+                # the training-mode output of the head is the raw per-level list; the criterion (opt-in, e.g.
+                # box_head.SetCriterion, box_head.py:85-325) receives what the reference passes
                 if self.compute_loss is None:
                     raise NotImplementedError(
-                        "training mode returns criterion(targets, head_outputs); SetCriterion is out of scope of this "
-                        "build -- construct YOLO(..., criterion=...) or call model.head(model.backbone(x)) directly")
+                        "training mode returns criterion(targets, head_outputs) and no criterion is set -- construct "
+                        "YOLO(..., criterion=SetCriterion(strides, anchor_grids, num_classes)) or call "
+                        "model.head(model.backbone(x)) directly")
                 return self.compute_loss(targets, head_outputs)
             return self.post_process(head_outputs, None, None)
         if targets is not None:
