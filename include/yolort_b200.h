@@ -230,7 +230,9 @@ typedef struct {
                                    super-pixel stem matrix [Cout_pad][3][128] (engine.stem_band); bit 2: take the
                                    halo-patch kernel's stride-2 parity-plane variant whatever the channel counts (tests);
                                    bit 3: do not split N over CTAs with resident weights (A/B timing, tests);
-                                   e4m3 convolutions: bits 4 / 5 only (see above); other bits: must be zero */
+                                   bit 4: keep one CTA per SM where the shape would take two (tests compare the two
+                                   launches bit for bit); e4m3 convolutions: bits 4 / 5 only (see above), with their
+                                   own meaning; other bits: must be zero */
   const yb_head_decode* decode; /* optional (host pointer, copied at plan creation): fused decode epilogue */
   const yb_conv_chain* chain;   /* optional (host pointer, copied at plan creation): chained pointwise tail  */
 } yb_op_desc;
@@ -244,7 +246,11 @@ int yb_conv_chain_supported(const yb_op_desc* op);
  *   shared memory   [4] M tiles per weight pass   [5] patch slots (pipeline stages)   [6] weight-ring slabs (k-iterations
  *   per stage)   [7] store-box columns   [8] staging buffers per epilogue group (halo-patch kernel) / epilogue groups
  *   (1x1 / im2col kernel)   [9] dynamic shared memory   [10] grid
- *   [11] chained tail fused.  Pure host logic. */
+ *   [11] flags: bit 0 chained tail fused; bit 1 two CTAs resident per SM (else one).  A convolution takes two CTAs
+ *   per SM when its kernel has a two-CTA instance for the N tile (1x1 / im2col: N <= 64 with no tail or a tail of at
+ *   most 64 columns; halo patch: N = 32 or 64, or 32 with a 64-column tail, single-tile tasks, resident weights in
+ *   one N tile, no banded stem), its plan fits half of
+ *   the SM's shared memory and it has at least 2 x SMs tiles; the grid is then up to 2 x SMs.  Pure host logic. */
 int yb_conv_config(const yb_op_desc* op, int32_t* info12);
 
 typedef struct yb_plan yb_plan;

@@ -436,6 +436,8 @@ def conv_config(op: "OpDesc") -> dict:
     keys = ("patch_kernel", "block_n", "n_tiles", "weights_resident", "tiles_per_pass", "slots", "ring", "store_cols",
             "store_bufs", "smem_bytes", "grid", "chained")
     cfg = dict(zip(keys, [int(v) for v in info]))
+    cfg["ctas_per_sm"] = 2 if cfg["chained"] & 2 else 1   # slot 11: bit 0 chained tail, bit 1 two CTAs per SM
+    cfg["chained"] &= 1
     cfg["e4m3_kernel"] = int(cfg["patch_kernel"] == 2)   # slot 0 is 2 for the e4m3 kernel (conv_fp8_sm90.cu)
     cfg["patch_kernel"] = int(cfg["patch_kernel"] == 1)
     if not cfg["patch_kernel"]:     # slot 8 of the 1x1 / im2col kernel: consumer warpgroups (sharing two staging buffers)

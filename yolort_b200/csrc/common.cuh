@@ -48,6 +48,48 @@ static inline int num_sms() {
   return n;
 }
 
+// Shared memory of one SM of the CURRENT device (228 KB on the H100) that resident CTAs share; the hardware reserves
+// kSmemReservedPerCta of it for every resident CTA.
+constexpr size_t kSmemReservedPerCta = 1024;
+static inline size_t smem_per_sm() {
+  static int cache[64] = {0};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= 64) dev = 0;
+  int n = cache[dev];
+  if (n == 0) {
+    cudaDeviceGetAttribute(&n, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
+    if (n <= 0) n = 228 * 1024;
+    cache[dev] = n;
+  }
+  return static_cast<size_t>(n);
+}
+
+// Shared-memory attributes of a conv kernel instance planned for `ctas` CTAs per SM.  A two-CTA plan asks for the
+// largest shared-memory carveout, and the occupancy the driver reports must confirm both CTAs: a plan that would
+// silently run one CTA per SM is an error.
+static inline int set_smem_attributes(const void* fn, size_t max_dynamic, int ctas, size_t smem_bytes, int threads,
+                                      const char* who) {
+  cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(max_dynamic));
+  if (e == cudaSuccess && ctas > 1)
+    e = cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  if (e != cudaSuccess) {
+    set_error("%s: cudaFuncSetAttribute failed: %s", who, cudaGetErrorString(e));
+    return YB_ERR_CUDA;
+  }
+  if (ctas > 1) {
+    int per_sm = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, smem_bytes);
+    if (e != cudaSuccess) {
+      set_error("%s: cudaOccupancyMaxActiveBlocksPerMultiprocessor failed: %s", who, cudaGetErrorString(e));
+      return YB_ERR_CUDA;
+    }
+    YB_REQUIRE(per_sm >= ctas, "%s: planned %d CTAs per SM with %zu bytes of shared memory, the device fits %d", who, ctas,
+               smem_bytes, per_sm);
+  }
+  return YB_OK;
+}
+
 #ifdef __CUDACC__
 // ---- small device utilities -------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -288,9 +330,22 @@ __device__ __forceinline__ void wgmma_mma(float* d, uint64_t da, uint64_t db, bo
 
 // Warpgroup register budgets: the producer warpgroup (TMA issue only) hands registers to the two consumer warpgroups,
 // whose fp32 accumulators (up to 128 per thread) must stay in registers for wgmma to run asynchronously.  Every warp of
-// a warpgroup executes the same instruction.  40 x 128 + 232 x 256 <= 64 K registers.
-__device__ __forceinline__ void regs_producer() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory"); }
-__device__ __forceinline__ void regs_consumer() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory"); }
+// a warpgroup executes the same instruction.  kCtas = CTAs of 384 threads resident per SM (__launch_bounds__):
+//   1: ptxas gives every thread 168 registers; 40 x 128 + 232 x 256 <= 384 x 168 (64 K registers per SM).
+//   2: ptxas gives every thread 80 registers (the cap it reports for __launch_bounds__(384, 2));
+//      24 x 128 + 104 x 256 <= 384 x 80, 104 being the largest multiple of 8 that fits.
+template <int kCtas>
+__device__ __forceinline__ void regs_producer() {
+  static_assert(kCtas == 1 || kCtas == 2, "1 or 2 CTAs per SM");
+  if constexpr (kCtas == 1) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+  else asm volatile("setmaxnreg.dec.sync.aligned.u32 24;\n" ::: "memory");
+}
+template <int kCtas>
+__device__ __forceinline__ void regs_consumer() {
+  static_assert(kCtas == 1 || kCtas == 2, "1 or 2 CTAs per SM");
+  if constexpr (kCtas == 1) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+  else asm volatile("setmaxnreg.inc.sync.aligned.u32 104;\n" ::: "memory");
+}
 
 // Role loops: warp-uniform with one elected issuing lane.  TMA instructions take uniform-register operands; inside a
 // one-lane branch ptxas wraps each of them in an elect/branch convergence loop.

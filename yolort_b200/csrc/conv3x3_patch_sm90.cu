@@ -18,7 +18,7 @@
 // pair-column to the left, dx = 1 the even plane, dx = 2 the odd plane; consecutive output pixels are consecutive
 // pair-columns (rows of a view stay contiguous) and consecutive output rows are two patch rows apart (SBO = 18 rows).
 //
-// Roles (one persistent CTA per SM, 384 threads): warp 0 = patch (A) producer, warp 2 = weight (B) producer (unless
+// Roles (one persistent CTA per SM, two for the narrow shallow levels, see patch_conv_configure; 384 threads): warp 0 = patch (A) producer, warp 2 = weight (B) producer (unless
 // the weights are resident in shared memory), warpgroups 1-2 = consumers: each multiplies 64 of the tile's 128
 // accumulator rows with wgmma (fp32 accumulators in registers) and runs the epilogue on its fragment.
 #include <cstdlib>
@@ -37,6 +37,7 @@ constexpr int kThreads = 128 * (1 + kConsumers);   // 384
 constexpr int kStageBufBytes = 128 * 128;
 constexpr int kMaxBlockN = 128;
 constexpr size_t kSmemBudget = 216 * 1024;
+constexpr size_t kStaticSmem = (2 * kMaxA + 2 * kMaxB + 2) * 8 + 2 * kMaxBlockN * 4;   // barriers + bias vectors (ptxas -v)
 constexpr uint32_t kConsumerBar = 1;               // named barrier of the 256 consumer threads
 
 // Tile geometry.  An output tile is 128 accumulator rows = 16 groups of 8 horizontally adjacent pixels.
@@ -65,6 +66,7 @@ struct PatchParams {
                           // the accumulators of both tiles (N tile <= 128)
   int s2;                 // 1: stride-2 convolution over two column-parity planes (H, W are the OUTPUT extent)
   int band;               // 1: banded super-pixel weights (stem), see the band MMA loop
+  int ctas;               // CTAs per SM the launch is planned for (1 or 2): selects the kernel instance
   int store_cols, store_bufs, bias_len;
   int stage_buf_bytes;    // bytes between the staging buffers (16 KB; 8 KB for the N-split variant)
   int kk_last;            // K=16 steps of the last channel chunk (TMA zero-fills past Cin, the MMA skips)
@@ -111,9 +113,9 @@ __device__ __forceinline__ void tile_coords(const PatchParams& p, int m_tile, in
 __device__ __forceinline__ void consumer_sync() { named_bar_sync(kConsumerBar, 128 * kConsumers); }
 
 // The K=16 steps of one filter tap over one channel chunk.
-//   mode 0: one tile; 1: two tiles sharing the weight slab (second accumulator at acc + kN / 2, kN <= 64);
+//   mode 0: one tile; 1: two tiles sharing the weight slab (second accumulator at acc + kN / 2, kPair instances only);
 //   2: stride 2, one accumulator, the tap picks its column-parity plane (a0 = even plane, a1 = odd plane).
-template <bool kBf16, int kN>
+template <bool kBf16, int kN, bool kPair>
 __device__ __forceinline__ void issue_tap(int mode, int tap, int kc, bool first, float* acc, uint32_t a0, uint32_t a1,
                                           uint32_t a_hi, uint32_t b_lo, uint32_t b_hi) {
   for (int k = 0; k < kc; ++k) {
@@ -123,7 +125,7 @@ __device__ __forceinline__ void issue_tap(int mode, int tap, int kc, bool first,
       wgmma_mma<kBf16, kN>(acc, desc_lohi(((tap % 3) == 1 ? a0 : a1) + 2 * k, a_hi), db, accum);
     } else {
       wgmma_mma<kBf16, kN>(acc, desc_lohi(a0 + 2 * k, a_hi), db, accum);
-      if constexpr (kN <= 64) {
+      if constexpr (kPair) {
         if (mode == 1) wgmma_mma<kBf16, kN>(acc + kN / 2, desc_lohi(a1 + 2 * k, a_hi), db, accum);
       }
     }
@@ -157,23 +159,31 @@ __device__ __forceinline__ void store_tile(const PatchParams& p, const CUtensorM
   }
 }
 
-// kN: the wgmma N of the tile (= block_n; pair tasks, kN <= 64, hold two tiles' accumulators).  kN2 != 0: a pointwise
+// kN: the wgmma N of the tile (= block_n; pair tasks hold two tiles' accumulators, see kPair).  kN2 != 0: a pointwise
 // tail of kN2 columns is chained onto every tile (conv_chain.cuh):
 // tmap_w2 = its weights, tmap_x = its optional second operand block (C3: the cv2 half of the concat, fetched per tile
-// with the output tile's box), tmap_out2 = its output.
-template <bool kBf16, int kN, int kN2>
-__global__ void __launch_bounds__(kThreads, 1)
+// with the output tile's box), tmap_out2 = its output.  kCtas: CTAs resident per SM (1 or 2, see regs_producer); with
+// two, one CTA's epilogue and barrier waits overlap the other CTA's MMAs and patch loads.
+template <bool kBf16, int kN, int kN2, int kCtas>
+__global__ void __launch_bounds__(kThreads, kCtas)
 conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                      const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_w2,
                      const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_out2,
                      const PatchParams p) {
   constexpr bool kChain = kN2 != 0;
-  constexpr int kTileAcc = kN <= 64 ? kN : kN / 2;   // accumulator registers per thread: two tiles when kN <= 64
+  // Pair tasks (two tiles per weight pass) need the accumulators of two tiles: one-CTA instances with kN <= 64.  The
+  // two-CTA instances only run single-tile tasks (patch_conv_plan) and hold one tile's accumulators.
+  constexpr bool kPair = kCtas == 1 && kN <= 64;
+  constexpr int kTileAcc = kPair ? kN : kN / 2;   // accumulator registers per thread
+  // Two-CTA plans (patch_conv_plan) always have resident weights in one N tile, single-tile tasks and no banded stem:
+  // those instances drop the other paths at compile time, which keeps their consumers within 104 registers.
+  constexpr bool kLean = kCtas == 2;
   // Register budget.  The N = 128 instance and the N = 64 instances with a chained tail spill within the 168 registers
   // that __launch_bounds__ gives every thread, so their producers hand registers to the consumers (40 / 232).  The
   // other instances fit in 168 without spilling and keep the even split: with 232 registers ptxas builds a schedule for
-  // them that runs 1-2.5 % slower on the H100 (pair-task and stride-2 launches).
-  constexpr bool kRealloc = kN == 128 || (kChain && kN == 64);
+  // them that runs 1-2.5 % slower on the H100 (pair-task and stride-2 launches).  With two CTAs per SM the even split
+  // is 80 registers, too few for the consumers: every two-CTA instance takes the 24 / 104 split.
+  constexpr bool kRealloc = kCtas == 2 || kN == 128 || (kChain && kN == 64);
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t a_full[kMaxA], a_empty[kMaxA];
   __shared__ __align__(8) uint64_t b_full[kMaxB], b_empty[kMaxB];
@@ -218,7 +228,7 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
   // Each role raises or lowers its register budget on a path of its own: the producer warps return before the consumer
   // code, so ptxas never reaches the consumers from the 40-register budget.
   if constexpr (kRealloc) {
-    if (warp < 4) regs_producer();
+    if (warp < 4) regs_producer<kCtas>();
   }
 
   if (warp == 0) {
@@ -294,7 +304,7 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
     return;
   }
   if (warp < 4) return;
-  if constexpr (kRealloc) regs_consumer();
+  if constexpr (kRealloc) regs_consumer<kCtas>();
 
   // ===================== consumers: MMA + epilogue of 64 accumulator rows each =====================
   const int g = (warp >> 2) - 1;
@@ -337,9 +347,9 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
   if constexpr (kChain) {   // the tail has a single N tile: one bias vector for every task
     for (int i = ctid; i < p.ch.n2; i += 128 * kConsumers) s_bias2[i] = (i < p.ch.bias2_len) ? __ldg(p.ch.bias2 + i) : 0.f;
   }
-  const bool fixed_n = (gridDim.x % p.n_tiles) == 0;
+  const bool fixed_n = kLean || (gridDim.x % p.n_tiles) == 0;
   if (fixed_n) {
-    const int n0f = (blockIdx.x % p.n_tiles) * p.block_n;
+    const int n0f = kLean ? 0 : (blockIdx.x % p.n_tiles) * p.block_n;
     for (int i = ctid; i < p.block_n; i += 128 * kConsumers) s_bias[i] = (n0f + i < p.bias_len) ? __ldg(p.bias + n0f + i) : 0.f;
   }
   consumer_sync();
@@ -349,9 +359,9 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
   int ka = 0, kb = 0, store_idx = 0;
   uint32_t xph = 0;
   for (int task = blockIdx.x; task < p.num_tasks; task += gridDim.x) {
-    const int m_first = (task / p.n_tiles) * p.pair;
-    const int cnt = p.s2 ? 2 : min(p.pair, p.m_tiles - m_first);
-    const int n0 = (task % p.n_tiles) * p.block_n;
+    const int m_first = kLean ? task : (task / p.n_tiles) * p.pair;
+    const int cnt = p.s2 ? 2 : (kLean ? 1 : min(p.pair, p.m_tiles - m_first));
+    const int n0 = kLean ? 0 : (task % p.n_tiles) * p.block_n;
     if (!fixed_n) {
       consumer_sync();
       for (int i = ctid; i < p.block_n; i += 128 * kConsumers) s_bias[i] = (n0 + i < p.bias_len) ? __ldg(p.bias + n0 + i) : 0.f;
@@ -365,7 +375,7 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
       const uint32_t a_lo1 = smem_lo16(a_buf + static_cast<size_t>(sa1) * p.a_stride) + a_wg16;
       const bool first_chunk = c == 0;
       wgmma_fence();
-      if (p.band) {
+      if (!kLean && p.band) {
         // Super-pixel stem (engine.stem_superpixel, pack 4, 16 channels per pixel, one 64-channel chunk): the expanded
         // weight matrix is block-banded -- a group of 4 output pixels reads, per filter row, exactly the 6 input pixels
         // x 16 channels that sit in 192 CONTIGUOUS bytes of the patch, starting 96 bytes into the left neighbour
@@ -382,11 +392,11 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
         wgmma_commit();
       } else {
         const int kc = c == p.chunks - 1 ? p.kk_last : kk;
-        if (p.b_resident) {
+        if (kLean || p.b_resident) {
           // all nine weight slabs are in shared memory
           const uint32_t b_lo_chunk = b_res_lo0 + static_cast<uint32_t>(c * 9) * b_step16;
           for (int tap = 0; tap < 9; ++tap)
-            issue_tap<kBf16, kN>(tmode, tap, kc, first_chunk && tap == 0, acc, a_lo0 + tap_off16(tap), a_lo1 + tap_off16(tap),
+            issue_tap<kBf16, kN, kPair>(tmode, tap, kc, first_chunk && tap == 0, acc, a_lo0 + tap_off16(tap), a_lo1 + tap_off16(tap),
                              a_hi, b_lo_chunk + tap * b_step16, b_hi);
           wgmma_commit();
         } else {
@@ -396,7 +406,7 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
           for (int tap = 0; tap < 9; ++tap, ++kb) {
             const int sb = kb % p.b_stages;
             mbar_wait(&b_full[sb], (kb / p.b_stages) & 1);
-            issue_tap<kBf16, kN>(tmode, tap, kc, first_chunk && tap == 0, acc, a_lo0 + tap_off16(tap), a_lo1 + tap_off16(tap),
+            issue_tap<kBf16, kN, kPair>(tmode, tap, kc, first_chunk && tap == 0, acc, a_lo0 + tap_off16(tap), a_lo1 + tap_off16(tap),
                              a_hi, b_res_lo0 + static_cast<uint32_t>(sb) * b_step16, b_hi);
             wgmma_commit();
             wgmma_wait<1>();
@@ -417,7 +427,7 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
     fence_acc<kTileAcc>(acc);
     if (!fixed_n) consumer_sync();   // bias visible
 
-    const int n_tiles_here = p.pair == 2 ? cnt : 1;
+    const int n_tiles_here = kPair && p.pair == 2 ? cnt : 1;
     int x0 = 0, y0 = 0, n_img = 0;
     for (int tsel = 0; tsel < n_tiles_here; ++tsel) {
       tile_coords(p, m_first + tsel, n_img, y0, x0);
@@ -441,7 +451,7 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
       }
       if (tsel == 0)
         store_tile<kBf16, kChain, kN>(p, &tmap_out, acc, s_bias, fr, n0, x0, y0, n_img, staging, store_idx, issuer, lane);
-      else if constexpr (kN <= 64)
+      else if constexpr (kPair)
         store_tile<kBf16, kChain, kN>(p, &tmap_out, acc + kN / 2, s_bias, fr, n0, x0, y0, n_img, staging, store_idx, issuer, lane);
     }
     if constexpr (kChain) {
@@ -492,18 +502,28 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
 using PatchKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
                                const CUtensorMap, const PatchParams);
 
-// One kernel per (dtype, N tile, chained tail N): the MMA width and the accumulator size are compile-time constants of
-// every instance.  patch_conv_configure admits exactly these shapes.
+// One kernel per (dtype, N tile, chained tail N, CTAs per SM): the MMA width and the accumulator size are compile-time
+// constants of every instance.  patch_conv_configure admits exactly these shapes.
 template <bool kBf16>
 PatchKernelFn select_patch_kernel_t(const PatchParams& kp) {
+  if (kp.ctas == 2) {
+    // two CTAs per SM: the instances whose consumers fit in 104 registers without spilling (N = 32 / 64, N = 32 with a
+    // 64-column tail; DESIGN.md section 3)
+    if (kp.ch.on) return kp.block_n == 32 && kp.ch.n2 == 64 ? conv3x3_patch_kernel<kBf16, 32, 64, 2> : nullptr;
+    switch (kp.block_n) {
+      case 32: return conv3x3_patch_kernel<kBf16, 32, 0, 2>;
+      case 64: return conv3x3_patch_kernel<kBf16, 64, 0, 2>;
+      default: return nullptr;
+    }
+  }
   if (kp.ch.on) {
-    if (kp.block_n == 32) return kp.ch.n2 == 64 ? conv3x3_patch_kernel<kBf16, 32, 64> : conv3x3_patch_kernel<kBf16, 32, 128>;
-    return kp.ch.n2 == 64 ? conv3x3_patch_kernel<kBf16, 64, 64> : conv3x3_patch_kernel<kBf16, 64, 128>;
+    if (kp.block_n == 32) return kp.ch.n2 == 64 ? conv3x3_patch_kernel<kBf16, 32, 64, 1> : conv3x3_patch_kernel<kBf16, 32, 128, 1>;
+    return kp.ch.n2 == 64 ? conv3x3_patch_kernel<kBf16, 64, 64, 1> : conv3x3_patch_kernel<kBf16, 64, 128, 1>;
   }
   switch (kp.block_n) {
-    case 32: return conv3x3_patch_kernel<kBf16, 32, 0>;
-    case 64: return conv3x3_patch_kernel<kBf16, 64, 0>;
-    default: return conv3x3_patch_kernel<kBf16, 128, 0>;
+    case 32: return conv3x3_patch_kernel<kBf16, 32, 0, 1>;
+    case 64: return conv3x3_patch_kernel<kBf16, 64, 0, 1>;
+    default: return conv3x3_patch_kernel<kBf16, 128, 0, 1>;
   }
 }
 PatchKernelFn select_patch_kernel(const PatchParams& kp) {
@@ -566,9 +586,23 @@ bool patch_conv_eligible(const yb_op_desc& d) {
   return eff >= 0.7;
 }
 
-// Pure host logic: tiling, shared-memory layout and launch shape (no driver calls).
+static int patch_conv_plan(const yb_op_desc& d, int ctas, PatchParams& kp, dim3& grid, size_t& smem_bytes);
+
+// Pure host logic: tiling, shared-memory layout and launch shape (no driver calls).  Two CTAs per SM when the shape has
+// a two-CTA instance, its plan fits half of the SM's shared memory with resident weights and there are tasks for both
+// (reserved bit 4 keeps one CTA per SM: tests compare the two launches bit for bit).
 static int patch_conv_configure(const yb_op_desc& d, PatchParams& kp, dim3& grid, size_t& smem_bytes) {
+  if (!(d.reserved & 16) && patch_conv_plan(d, 2, kp, grid, smem_bytes) == YB_OK) return YB_OK;
+  return patch_conv_plan(d, 1, kp, grid, smem_bytes);
+}
+
+// The plan for `ctas` CTAs per SM.  With ctas = 2 it gets half of the SM's shared memory, less the per-CTA reservation
+// and the kernel's static shared memory, and fails unless the weights stay resident in one N tile, the tasks are single
+// tiles, the shape has a two-CTA instance and there are at least 2 x SMs tasks.
+static int patch_conv_plan(const yb_op_desc& d, int ctas, PatchParams& kp, dim3& grid, size_t& smem_bytes) {
+  const size_t budget = ctas == 2 ? smem_per_sm() / 2 - kSmemReservedPerCta - kStaticSmem : kSmemBudget;
   kp = PatchParams();
+  kp.ctas = ctas;
   kp.N = d.N;
   kp.s2 = d.stride == 2 ? 1 : 0;
   kp.H = d.Ho;     // the kernel tiles the OUTPUT map (equal to the input extent at stride 1)
@@ -605,9 +639,9 @@ static int patch_conv_configure(const yb_op_desc& d, PatchParams& kp, dim3& grid
     const int kc = d.chain->own_C >= 64 ? 64 : d.chain->own_C;
     const int chunks2 = kc > 0 ? d.chain->K_pad / kc : 0;
     chain_bytes = static_cast<size_t>(chunks2) * ((static_cast<size_t>(mma_n(d.chain->Cout_pad)) * kc * 2 + 1023) & ~static_cast<size_t>(1023));
-    YB_REQUIRE(chain_bytes + staging + 1024 + 64 * 1024 < kSmemBudget, "patch conv: chained tail weights (%zu bytes) do not fit", chain_bytes);
+    YB_REQUIRE(chain_bytes + staging + 1024 + 64 * 1024 < budget, "patch conv: chained tail weights (%zu bytes) do not fit", chain_bytes);
   }
-  const size_t avail = kSmemBudget - staging - 1024 - chain_bytes;
+  const size_t avail = budget - staging - 1024 - chain_bytes;
   uint32_t b_sub = (static_cast<uint32_t>(block_n * kp.block_k * 2) + 1023u) & ~1023u;
   size_t b_total = static_cast<size_t>(kp.band ? 6 : 9 * kp.chunks) * b_sub;
   kp.b_resident = (n_tiles == 1 && b_total + 2 * kp.a_stride <= avail) ? 1 : 0;
@@ -634,7 +668,7 @@ static int patch_conv_configure(const yb_op_desc& d, PatchParams& kp, dim3& grid
         const size_t stg = static_cast<size_t>(opt_bufs[o]) * buf_bytes;
         // at least three patch slots: with two, a task that needs both (two channel chunks) cannot prefetch the next
         // task's patch and every task pays the L2 latency
-        if (bt + 3 * kp.a_stride + stg + 1024 > kSmemBudget) continue;
+        if (bt + 3 * kp.a_stride + stg + 1024 > budget) continue;
         n_tiles = ns;
         block_n = bn;
         b_sub = bs;
@@ -648,7 +682,7 @@ static int patch_conv_configure(const yb_op_desc& d, PatchParams& kp, dim3& grid
       }
     }
   }
-  const size_t avail_ns = kSmemBudget - staging_ns - 1024 - chain_bytes;
+  const size_t avail_ns = budget - staging_ns - 1024 - chain_bytes;
   // Weights that do not fit in shared memory are streamed from L2 for every task; two M tiles per weight pass halve
   // that stream (the bound of the deep layers: 128 -> 128 at 40 x 40 re-reads 295 KB per 128 output pixels).  Pair
   // tasks hold the accumulators of two tiles in registers, so their N tile is at most 64 columns (stride-2 tasks with
@@ -693,6 +727,10 @@ static int patch_conv_configure(const yb_op_desc& d, PatchParams& kp, dim3& grid
     kp.ch.extra_bytes = static_cast<uint32_t>(tg.tile_w * tg.tile_h) * static_cast<uint32_t>(kp.ch.extra_row_bytes);
   }
   kp.b_res_bytes = kp.b_resident ? static_cast<uint32_t>(b_total) : 0u;
+  kp.ep.is_bf16 = d.dtype == YB_BF16;
+  if (ctas == 2 && !(kp.b_resident && n_tiles == 1 && kp.pair == 1 && !kp.band && kp.num_tasks >= 2 * sms &&
+                     select_patch_kernel(kp) != nullptr))
+    return YB_ERR_INVALID;
   if (kp.b_resident) {
     int a_st = static_cast<int>((avail_ns - b_total) / kp.a_stride);
     kp.a_slots = a_st > kMaxA ? kMaxA : a_st;
@@ -716,15 +754,15 @@ static int patch_conv_configure(const yb_op_desc& d, PatchParams& kp, dim3& grid
   YB_REQUIRE(kp.a_slots >= 2, "patch conv: fewer than two patch slots fit in shared memory (block_n=%d)", block_n);
   kp.ep.Cout = d.Cout;
   kp.ep.act = d.act;
-  kp.ep.is_bf16 = d.dtype == YB_BF16;
   kp.ep.residual = d.residual;
   kp.ep.res_cstride = d.res_cstride;
   kp.bias = d.bias;
-  grid = dim3(kp.num_tasks < sms ? kp.num_tasks : sms, 1, 1);
+  const int max_grid = ctas * sms;
+  grid = dim3(kp.num_tasks < max_grid ? kp.num_tasks : max_grid, 1, 1);
   YB_REQUIRE(!(kp.b_resident && n_tiles > 1) || grid.x % n_tiles == 0, "patch conv: N-split grid %u not a multiple of %d", grid.x, n_tiles);
   const size_t b_region = kp.b_resident ? kp.b_res_bytes : static_cast<size_t>(kp.b_stages) * kp.b_sub_bytes;
   const size_t smem = static_cast<size_t>(kp.a_slots) * kp.a_stride + b_region + staging_ns + chain_bytes + 1024;
-  YB_REQUIRE(smem <= kSmemBudget, "patch conv: %zu bytes of shared memory needed, %zu available", smem, kSmemBudget);
+  YB_REQUIRE(smem <= budget, "patch conv: %zu bytes of shared memory needed, %zu available", smem, budget);
   smem_bytes = smem;
   return YB_OK;
 }
@@ -746,7 +784,7 @@ int patch_conv_configure_check(const yb_op_desc& d, int* info) {
     info[8] = kp.store_bufs;
     info[9] = static_cast<int>(smem);
     info[10] = static_cast<int>(grid.x);
-    info[11] = kp.ch.on;
+    info[11] = kp.ch.on | (kp.ctas == 2 ? 2 : 0);
   }
   return rc;
 }
@@ -866,11 +904,10 @@ int patch_conv_create(const yb_op_desc& d, EncodeTiledFn encode_tiled, PatchConv
     }
   }
   op->fn = select_patch_kernel(kp);
-  cudaError_t e = cudaFuncSetAttribute(op->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kSmemBudget));
-  if (e != cudaSuccess) {
-    set_error("patch conv: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
+  rc = set_smem_attributes(reinterpret_cast<const void*>(op->fn), kSmemBudget, kp.ctas, op->smem_bytes, kThreads, "patch conv");
+  if (rc != YB_OK) {
     delete op;
-    return YB_ERR_CUDA;
+    return rc;
   }
   *out = op;
   return YB_OK;

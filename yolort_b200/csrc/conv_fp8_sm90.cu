@@ -150,7 +150,7 @@ conv_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
   if (warp < 4) {
-    regs_producer();
+    regs_producer<1>();
     if (warp != 0) return;
     // ===================== TMA producer (warp-uniform loop, one elected lane issues) =====================
     const uint32_t a_bytes = kBlockM * p.block_k, b_bytes = p.block_n * p.block_k;
@@ -198,7 +198,7 @@ conv_fp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   }
 
   // ===================== consumers: MMA + epilogue of 64 rows each =====================
-  regs_consumer();
+  regs_consumer<1>();
   const int g = (warp >> 2) - 1;
   const int wq = warp & 3;
   const bool issuer = threadIdx.x == 128;

@@ -6,7 +6,8 @@
 // Replaces the arithmetic of yolort/v5/models/common.py:42-73 (Conv = conv2d -> BN(eps 1e-3) -> SiLU),
 // :94-116 (Bottleneck residual) and the 1x1 head convs of yolort/models/box_head.py:35-37,68-82.
 //
-// Persistent kernel, one CTA per SM, static round-robin over 128 x block_n output tiles, 384 threads:
+// Persistent kernel, one CTA per SM (two for the narrow shallow layers, see conv_configure), static round-robin over
+// 128 x block_n output tiles, 384 threads:
 //   warpgroup 0 (producer, 40 registers): warp 0 issues the TMA loads.  A tiles come from a 4-D im2col tensor map (the
 //                TMA engine walks 128 output pixels, applies padding/stride and zero-fills the halo) or, for 1x1/s1
 //                convs, from a 2-D tiled map; B tiles (weights) from a 2-D tiled map.  Both land in shared memory in the
@@ -38,6 +39,7 @@ constexpr int kStageBufBytes = 128 * 128;  // 128 rows x (up to) 64 columns x 2 
 constexpr int kStageBufs = 2;              // staging boxes, shared by the two consumer warpgroups
 constexpr int kMaxBlockN = 256;
 constexpr size_t kSmemBudget = 216 * 1024;  // dynamic shared memory per CTA (227 KB limit minus static)
+constexpr size_t kStaticSmem = (2 * kMaxStages + 2) * 8 + 2 * kMaxBlockN * 4;   // barriers + bias vectors (ptxas -v)
 constexpr uint32_t kConsumerBar = 1;        // named barrier of the 256 consumer threads
 
 struct ConvKernelParams {
@@ -50,6 +52,7 @@ struct ConvKernelParams {
   int b_resident;  // weights of the (single) N tile stay in shared memory for the CTA's lifetime
   uint32_t b_res_bytes;
   int n_tiles, num_tiles;
+  int ctas;        // CTAs per SM the launch is planned for (1 or 2): selects the kernel instance
   int store_cols;  // columns per TMA store box: 64 / 32 / 16
   int bias_len;    // length of the (padded) bias vector
   int kk_last;     // K=16 steps of the LAST channel chunk (Cin need not fill it: TMA zero-fills, the MMA skips)
@@ -154,9 +157,10 @@ __device__ __forceinline__ void decode_fragment(const yb_head_decode& D, const f
 
 // kN: the wgmma N of the tile (= block_n; kN / 2 accumulator registers per thread).  kDecode: detection head with the
 // fused decode (nothing stored).  kN2 != 0: a
-// pointwise tail is chained onto every tile (conv_chain.cuh).
-template <bool kBf16, int kN, bool kDecode, int kN2>
-__global__ void __launch_bounds__(kThreads, 1)
+// pointwise tail is chained onto every tile (conv_chain.cuh).  kCtas: CTAs resident per SM (1 or 2, see
+// regs_producer); with two, one CTA's epilogue and barrier waits overlap the other CTA's MMAs and loads.
+template <bool kBf16, int kN, bool kDecode, int kN2, int kCtas>
+__global__ void __launch_bounds__(kThreads, kCtas)
 conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_w2,
                   const __grid_constant__ CUtensorMap tmap_out2, const ConvKernelParams p) {
@@ -218,7 +222,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
   if (warp < 4) {
-    regs_producer();
+    regs_producer<kCtas>();
     if (warp != 0) return;
     // ===================== TMA producer (warp-uniform loop, one elected lane issues) =====================
     const uint32_t a_bytes = kBlockM * p.block_k * 2, b_bytes = p.block_n * p.block_k * 2;
@@ -266,7 +270,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   }
 
   // ===================== consumers: MMA + epilogue of 64 rows each =====================
-  regs_consumer();
+  regs_consumer<kCtas>();
   const int g = (warp >> 2) - 1;
   const int wq = warp & 3;
   const bool issuer = threadIdx.x == 128;
@@ -450,25 +454,41 @@ int encode_im2col_entry(EncodeIm2colFn* out) {
 using ConvKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
                               const ConvKernelParams);
 
-// One kernel per (dtype, N tile, fused decode, chained tail N): the MMA width and the accumulator size are compile-time
-// constants of every instance, so the accumulators stay in registers while the wgmma instructions are in flight.
-// conv_configure admits exactly these shapes.
+// One kernel per (dtype, N tile, fused decode, chained tail N, CTAs per SM): the MMA width and the accumulator size are
+// compile-time constants of every instance, so the accumulators stay in registers while the wgmma instructions are in
+// flight.  conv_configure admits exactly these shapes.
 template <bool kBf16>
 ConvKernelFn select_conv_kernel_t(const ConvKernelParams& kp) {
-  if (kp.decode_on) return conv_wgmma_kernel<kBf16, 256, true, 0>;
+  if (kp.ctas == 2) {
+    // two CTAs per SM: the instances whose consumers fit in 104 registers without spilling (N <= 64, tails of at most
+    // 64 columns; DESIGN.md section 3)
+    if (kp.decode_on) return nullptr;
+    if (kp.ch.on) {
+      if (kp.block_n != 64) return nullptr;
+      return kp.ch.n2 == 32 ? conv_wgmma_kernel<kBf16, 64, false, 32, 2>
+                            : (kp.ch.n2 == 64 ? conv_wgmma_kernel<kBf16, 64, false, 64, 2> : nullptr);
+    }
+    switch (kp.block_n) {
+      case 16: return conv_wgmma_kernel<kBf16, 16, false, 0, 2>;
+      case 32: return conv_wgmma_kernel<kBf16, 32, false, 0, 2>;
+      case 64: return conv_wgmma_kernel<kBf16, 64, false, 0, 2>;
+      default: return nullptr;
+    }
+  }
+  if (kp.decode_on) return conv_wgmma_kernel<kBf16, 256, true, 0, 1>;
   if (kp.ch.on) {
     if (kp.block_n == 64)
-      return kp.ch.n2 == 32 ? conv_wgmma_kernel<kBf16, 64, false, 32>
-                            : (kp.ch.n2 == 64 ? conv_wgmma_kernel<kBf16, 64, false, 64> : conv_wgmma_kernel<kBf16, 64, false, 128>);
-    return kp.ch.n2 == 32 ? conv_wgmma_kernel<kBf16, 128, false, 32>
-                          : (kp.ch.n2 == 64 ? conv_wgmma_kernel<kBf16, 128, false, 64> : conv_wgmma_kernel<kBf16, 128, false, 128>);
+      return kp.ch.n2 == 32 ? conv_wgmma_kernel<kBf16, 64, false, 32, 1>
+                            : (kp.ch.n2 == 64 ? conv_wgmma_kernel<kBf16, 64, false, 64, 1> : conv_wgmma_kernel<kBf16, 64, false, 128, 1>);
+    return kp.ch.n2 == 32 ? conv_wgmma_kernel<kBf16, 128, false, 32, 1>
+                          : (kp.ch.n2 == 64 ? conv_wgmma_kernel<kBf16, 128, false, 64, 1> : conv_wgmma_kernel<kBf16, 128, false, 128, 1>);
   }
   switch (kp.block_n) {
-    case 16: return conv_wgmma_kernel<kBf16, 16, false, 0>;
-    case 32: return conv_wgmma_kernel<kBf16, 32, false, 0>;
-    case 64: return conv_wgmma_kernel<kBf16, 64, false, 0>;
-    case 128: return conv_wgmma_kernel<kBf16, 128, false, 0>;
-    default: return conv_wgmma_kernel<kBf16, 256, false, 0>;
+    case 16: return conv_wgmma_kernel<kBf16, 16, false, 0, 1>;
+    case 32: return conv_wgmma_kernel<kBf16, 32, false, 0, 1>;
+    case 64: return conv_wgmma_kernel<kBf16, 64, false, 0, 1>;
+    case 128: return conv_wgmma_kernel<kBf16, 128, false, 0, 1>;
+    default: return conv_wgmma_kernel<kBf16, 256, false, 0, 1>;
   }
 }
 ConvKernelFn select_conv_kernel(const ConvKernelParams& kp) {
@@ -484,11 +504,13 @@ struct ConvOp {
   size_t smem_bytes;
 };
 
+static int conv_plan(const yb_op_desc& d, int ctas, ConvKernelParams& kp, dim3& grid, size_t& smem_bytes);
+
 // Pure host logic: validates the op and derives tiling, pipeline depth, shared-memory layout and launch shape
 // (no driver calls: yb_conv_chain_supported runs this without a GPU).
 static int conv_configure(const yb_op_desc& d, ConvKernelParams& kp, dim3& grid, size_t& smem_bytes) {
   YB_REQUIRE(d.dtype == YB_F16 || d.dtype == YB_BF16, "conv: dtype must be f16 or bf16");
-  YB_REQUIRE((d.reserved & ~15) == 0, "conv: reserved bits 4 and up must be zero, got 0x%x", d.reserved);
+  YB_REQUIRE((d.reserved & ~31) == 0, "conv: reserved bits 5 and up must be zero, got 0x%x", d.reserved);
   YB_REQUIRE(d.ksize >= 1 && d.ksize <= 7 && d.stride >= 1 && d.stride <= 2, "conv: ksize/stride");
   YB_REQUIRE(d.act >= YB_ACT_NONE && d.act <= YB_ACT_RELU, "conv: unknown activation %d", d.act);
   YB_REQUIRE(d.Cin % 8 == 0 && d.in_cstride % 8 == 0 && d.in_cstride >= d.Cin,
@@ -515,7 +537,22 @@ static int conv_configure(const yb_op_desc& d, ConvKernelParams& kp, dim3& grid,
              "conv: banded stem weights (reserved bit 1) need the halo-patch kernel, which this %dx%d map does not qualify for",
              d.H, d.W);
   if (patch_conv_eligible(d)) return YB_OK;   // configured by patch_conv_configure
+  // Two CTAs per SM when the shape has a two-CTA instance, its plan fits half of the SM's shared memory and there are
+  // tiles for both (reserved bit 4 keeps one CTA per SM: tests compare the two launches bit for bit).
+  if (!(d.reserved & 16) && conv_plan(d, 2, kp, grid, smem_bytes) == YB_OK) return YB_OK;
+  return conv_plan(d, 1, kp, grid, smem_bytes);
+}
+
+// Tiling, pipeline depth, shared-memory layout and launch shape for `ctas` CTAs per SM (conv_configure has validated the
+// descriptor).  With ctas = 2 the plan gets half of the SM's shared memory, less the per-CTA reservation and the
+// kernel's static shared memory, and fails when it does not fit there, when the shape has no two-CTA instance or when
+// there are fewer tiles than 2 x SMs.
+static int conv_plan(const yb_op_desc& d, int ctas, ConvKernelParams& kp, dim3& grid, size_t& smem_bytes) {
+  const int Ho = d.Ho, Wo = d.Wo;
+  const long long M_ll = static_cast<long long>(d.N) * Ho * Wo;
+  const size_t budget = ctas == 2 ? smem_per_sm() / 2 - kSmemReservedPerCta - kStaticSmem : kSmemBudget;
   kp = ConvKernelParams();
+  kp.ctas = ctas;
   kp.M = static_cast<int>(M_ll);
   kp.ep.Cout = d.Cout;
   const int m_tiles = (kp.M + kBlockM - 1) / kBlockM;
@@ -589,8 +626,8 @@ static int conv_configure(const yb_op_desc& d, ConvKernelParams& kp, dim3& grid,
   // k-iterations per pipeline stage: aim at ~32 KB per stage so that one mbarrier round trip moves
   // enough bytes (a 16-channel tap is only 4 KB), in near-equal groups.
   const uint32_t per_iter = kp.a_stage_bytes + (kp.b_resident ? 0u : kp.b_stage_bytes);
-  YB_REQUIRE(kSmemBudget > fixed + kp.b_res_bytes + 2 * per_iter, "conv: shared memory budget exceeded (block_n=%d)", kp.block_n);
-  const size_t avail = kSmemBudget - fixed - kp.b_res_bytes;
+  YB_REQUIRE(budget > fixed + kp.b_res_bytes + 2 * per_iter, "conv: shared memory budget exceeded (block_n=%d)", kp.block_n);
+  const size_t avail = budget - fixed - kp.b_res_bytes;
   const size_t target = avail / 3 < 32 * 1024 ? avail / 3 : 32 * 1024;   // keep at least three stages in flight
   int kpg_max = static_cast<int>(target / per_iter);
   if (kpg_max < 1) kpg_max = 1;
@@ -607,9 +644,12 @@ static int conv_configure(const yb_op_desc& d, ConvKernelParams& kp, dim3& grid,
   kp.bias = d.bias;
   kp.ep.residual = d.residual;
   kp.ep.res_cstride = d.res_cstride;
-  grid = dim3(kp.num_tiles < sms ? kp.num_tiles : sms, 1, 1);
+  // two CTAs per SM: only with an instance built for it and at least one tile for each of the 2 x SMs CTAs
+  if (ctas == 2 && (select_conv_kernel(kp) == nullptr || kp.num_tiles < 2 * sms)) return YB_ERR_INVALID;
+  const int max_grid = ctas * sms;   // every two-CTA instance has one N tile: any grid keeps the N tile fixed per CTA
+  grid = dim3(kp.num_tiles < max_grid ? kp.num_tiles : max_grid, 1, 1);
   const size_t smem = static_cast<size_t>(stages) * stage_bytes + kp.b_res_bytes + fixed;
-  YB_REQUIRE(smem <= kSmemBudget, "conv: %zu bytes of shared memory needed, %zu available", smem, kSmemBudget);
+  YB_REQUIRE(smem <= budget, "conv: %zu bytes of shared memory needed, %zu available", smem, budget);
   smem_bytes = smem;
   return YB_OK;
 }
@@ -631,7 +671,7 @@ int conv_configure_check(const yb_op_desc& d, int* info) {
     info[8] = kConsumers;         // (im2col / 1x1 kernel: consumer warpgroups; they share two staging buffers)
     info[9] = static_cast<int>(smem);
     info[10] = static_cast<int>(grid.x);
-    info[11] = kp.ch.on;
+    info[11] = kp.ch.on | (kp.ctas == 2 ? 2 : 0);
   }
   return rc;
 }
@@ -755,11 +795,10 @@ int conv_op_create(const yb_op_desc& d, ConvOp** out) {
     }
   }
   op->fn = select_conv_kernel(kp);
-  cudaError_t e = cudaFuncSetAttribute(op->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kSmemBudget));
-  if (e != cudaSuccess) {
-    set_error("conv: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
+  rc = set_smem_attributes(reinterpret_cast<const void*>(op->fn), kSmemBudget, kp.ctas, op->smem_bytes, kThreads, "conv");
+  if (rc != YB_OK) {
     delete op;
-    return YB_ERR_CUDA;
+    return rc;
   }
   *out = op;
   return YB_OK;
