@@ -504,6 +504,54 @@ int yb_yolo_loss_backward(const yb_yolo_loss_params* params, const yb_loss_level
                           const float* grad_losses_dev, void* const* grad_out_levels, void* workspace_dev,
                           size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Training augmentations (the reference's yolort/data/transforms.py:21-336 on uint8 tensor images, with
+ * torchvision's tensor arithmetic; restated in oracle/restate_augment.py).  Each image carries its recipe: the ops
+ * its transforms drew, in call order.  Every parameter is drawn on the host; the kernels only compute pixels.
+ * ---------------------------------------------------------------------------------------------- */
+#define YB_AUG_MAX_OPS 16
+#define YB_AUG_MAX_CONTRAST 4      /* contrast ops per image (one mean launch each)                          */
+#define YB_AUG_BRIGHTNESS 1        /* factor, one_minus                                                      */
+#define YB_AUG_CONTRAST 2          /* factor, one_minus; arg = round, h, w of the image the op sees          */
+#define YB_AUG_SATURATION 3        /* factor, one_minus                                                      */
+#define YB_AUG_HUE 4               /* factor                                                                 */
+#define YB_AUG_PERMUTE 5           /* arg = source channel of output channel 0, 1, 2                         */
+#define YB_AUG_ZOOM_OUT 6          /* arg = top, left, h, w of the image on the canvas, canvas h, w,
+                                      fill (r | g<<8 | b<<16)                                                */
+#define YB_AUG_CROP 7              /* arg = top, left, h, w of the window                                    */
+#define YB_AUG_HFLIP 8             /* arg = width                                                            */
+
+typedef struct {
+  int32_t kind;                /* YB_AUG_*                                                                    */
+  int32_t arg[7];
+  float factor;                /* the drawn factor (an fp32 value)                                            */
+  float one_minus;             /* 1.0 - factor computed in double, rounded to fp32 (torchvision's _blend)      */
+} yb_aug_op;
+
+typedef struct {
+  const uint8_t* src;          /* uint8 [3, src_h, src_w] with these element strides                          */
+  int64_t stride_c, stride_y, stride_x;
+  int32_t src_h, src_w, out_h, out_w;
+  int64_t out_offset;          /* elements from the output base to this image's contiguous [3, out_h, out_w]   */
+  int32_t n_ops, n_contrast;
+  int32_t out_block_start;     /* filled by yb_augment_prepare                                                */
+  int32_t mean_block_start[YB_AUG_MAX_CONTRAST];
+  int32_t reserved;
+  yb_aug_op ops[YB_AUG_MAX_OPS];
+} yb_aug_image;
+
+/* Host-only: checks the recipes (out_h / out_w and each contrast op's h, w must be the sizes the ops give; crops
+ * lie inside their image) and fills n_contrast and the block starts.  totals[0] = output blocks, totals[1 + j] =
+ * blocks of mean round j, for YB_AUG_MAX_CONTRAST rounds. */
+int yb_augment_prepare(int n_images, yb_aug_image* images, int64_t* totals);
+
+/* Computes every image's output.  images_host: the prepared descriptors; images_dev: the same bytes on the device.
+ * out_dtype YB_U8, or YB_F32 for the fused byte / 255.0f (IEEE division).  sums_dev: uint64
+ * [n_images * YB_AUG_MAX_CONTRAST], the exact grayscale sums of the contrast ops (zeroed here).  One mean launch per
+ * contrast round that any image has, then one output launch.  No host synchronisation; deterministic. */
+int yb_augment(int n_images, const yb_aug_image* images_host, const yb_aug_image* images_dev, void* out_dev,
+               int32_t out_dtype, uint64_t* sums_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -58,6 +58,8 @@ EXPORTED_SYMBOLS = (
     "yb_yolo_loss_layout",
     "yb_yolo_loss_forward",
     "yb_yolo_loss_backward",
+    "yb_augment_prepare",
+    "yb_augment",
 )
 
 
@@ -201,6 +203,27 @@ class YoloLossParams(ctypes.Structure):
 
 
 YB_LOSS_ST_IMAGE, YB_LOSS_ST_CLASS, YB_LOSS_ST_NONFINITE = 1, 2, 4
+YB_AUG_MAX_OPS, YB_AUG_MAX_CONTRAST = 16, 4
+(YB_AUG_BRIGHTNESS, YB_AUG_CONTRAST, YB_AUG_SATURATION, YB_AUG_HUE, YB_AUG_PERMUTE, YB_AUG_ZOOM_OUT, YB_AUG_CROP,
+ YB_AUG_HFLIP) = range(1, 9)
+
+
+class AugOp(ctypes.Structure):
+    """yb_aug_op: one op of an image's augmentation recipe (include/yolort_b200.h)."""
+    _fields_ = [("kind", ctypes.c_int32), ("arg", ctypes.c_int32 * 7), ("factor", ctypes.c_float),
+                ("one_minus", ctypes.c_float)]
+
+
+class AugImage(ctypes.Structure):
+    """yb_aug_image: one image, its recipe and where its output goes (include/yolort_b200.h)."""
+    _fields_ = [
+        ("src", ctypes.c_void_p), ("stride_c", ctypes.c_int64), ("stride_y", ctypes.c_int64),
+        ("stride_x", ctypes.c_int64),
+        ("src_h", ctypes.c_int32), ("src_w", ctypes.c_int32), ("out_h", ctypes.c_int32), ("out_w", ctypes.c_int32),
+        ("out_offset", ctypes.c_int64), ("n_ops", ctypes.c_int32), ("n_contrast", ctypes.c_int32),
+        ("out_block_start", ctypes.c_int32), ("mean_block_start", ctypes.c_int32 * YB_AUG_MAX_CONTRAST),
+        ("reserved", ctypes.c_int32), ("ops", AugOp * YB_AUG_MAX_OPS),
+    ]
 YB_LOSS_MATCH_INT32 = 24
 
 _lib = None
@@ -288,6 +311,9 @@ def lib() -> ctypes.CDLL:
     L.yb_yolo_loss_backward.argtypes = [ctypes.POINTER(YoloLossParams), ctypes.POINTER(LossLevel), ctypes.c_int64,
                                         ctypes.c_void_p, ctypes.POINTER(ctypes.c_void_p), ctypes.c_void_p,
                                         ctypes.c_size_t, ctypes.c_void_p]
+    L.yb_augment_prepare.argtypes = [ctypes.c_int, ctypes.POINTER(AugImage), ctypes.POINTER(ctypes.c_int64)]
+    L.yb_augment.argtypes = [ctypes.c_int, ctypes.POINTER(AugImage), ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
+                             ctypes.c_void_p, ctypes.c_void_p]
     _lib = L
     return L
 
@@ -895,3 +921,30 @@ def yolo_loss_matches(params: YoloLossParams, levels, n_targets: int, ws: torch.
     bounds = [int(pos[l * per_level]) for l in range(params.n_levels)] + [int(pos[cap])]
     rec = ws[int(out[0]): int(out[0]) + 4 * YB_LOSS_MATCH_INT32 * bounds[-1]].view(torch.int32)
     return rec.view(-1, YB_LOSS_MATCH_INT32).cpu(), bounds
+
+
+# ---------------------------------------------------------------------------------------------------
+# training augmentations
+# ---------------------------------------------------------------------------------------------------
+def augment(descs, out: torch.Tensor, sources: Sequence[torch.Tensor]) -> torch.Tensor:
+    """Runs the prepared-here recipes `descs` (AugImage array, src pointers set) into `out` (uint8 or float32, on the
+    sources' device).  The descriptors cross to the device in one asynchronous copy from pinned memory."""
+    n = len(descs)
+    dev = out.device
+    require_cuda(out, "augment")
+    totals = (ctypes.c_int64 * (1 + YB_AUG_MAX_CONTRAST))()
+    check(lib().yb_augment_prepare(n, descs, totals), "yb_augment_prepare")
+    raw = torch.frombuffer(bytearray(ctypes.string_at(ctypes.addressof(descs), ctypes.sizeof(descs))), dtype=torch.uint8)
+    with device_guard(dev):
+        d_descs = raw.pin_memory().to(dev, non_blocking=True)
+        sums = torch.empty((n * YB_AUG_MAX_CONTRAST,), dtype=torch.int64, device=dev)
+        check(lib().yb_augment(n, descs, d_descs.data_ptr(), out.data_ptr(), dtype_code(out.dtype), sums.data_ptr(),
+                               current_stream_ptr(dev)), "yb_augment")
+        stream = torch.cuda.current_stream(dev)
+        seen = set()
+        for im in sources:
+            key = im.untyped_storage().data_ptr()
+            if key not in seen:
+                seen.add(key)
+                im.record_stream(stream)
+    return out

@@ -1,4 +1,5 @@
-"""Dataset-side tools of the reference's `yolort.data` that the inference path needs: COCO box evaluation."""
+"""Dataset-side tools of the reference's `yolort.data`: COCO box evaluation and the training augmentations."""
+from . import transforms
 from .coco_eval import COCOEvaluator
 
-__all__ = ["COCOEvaluator"]
+__all__ = ["COCOEvaluator", "transforms"]

@@ -1,9 +1,9 @@
 """`YOLOTransform`: the letterbox front-end, backed by the native kernel.
 
 Same constructor and call contract as the reference class (yolort/models/transform.py:100-351):
-`forward(images)` returns a `NestedTensor` (padded batch + resized sizes).  The resize/pad arithmetic is
-`yb_letterbox_geometry` (host, csrc/letterbox.cu) + `yb_letterbox` (device).  Extension: images may be
-uint8 [3,H,W] tensors, in which case the `/255` of the default loader (yolov5.py:228) is fused.
+`forward(images, targets=None)` returns a `NestedTensor` (padded batch + resized sizes) and the target batch.  The
+resize/pad arithmetic is `yb_letterbox_geometry` (host, csrc/letterbox.cu) + `yb_letterbox` (device).  Extension:
+images may be uint8 [3,H,W] tensors, in which case the `/255` of the default loader (yolov5.py:228) is fused.
 """
 from typing import Dict, List, NamedTuple, Optional, Tuple
 
@@ -43,15 +43,40 @@ class YOLOTransform(nn.Module):
 
     # -- reference call contract -------------------------------------------------------------------
     def forward(self, images: List[Tensor], targets: Optional[List[Dict[str, Tensor]]] = None):
-        if targets is not None:
-            raise NotImplementedError("target transformation belongs to the training path (out of scope)")
         images = list(images)
         geoms, (Hb, Wb) = self.geometry(images)
         dt = images[0].dtype if images[0].is_floating_point() else torch.float32
         out = torch.empty((len(images), 3, Hb, Wb), dtype=dt, device=images[0].device)
         self.letterbox_into(images, geoms, Hb, Wb, out, _C.YB_LAYOUT_NCHW)
         sizes = [(int(g.new_h), int(g.new_w)) for g in geoms]
-        return NestedTensor(out, sizes), None
+        if targets is None:
+            return NestedTensor(out, sizes), None
+        return NestedTensor(out, sizes), self.batch_targets(images, targets)
+
+    def batch_targets(self, images: List[Tensor], targets: List[Dict[str, Tensor]]) -> Tensor:
+        """The reference's target batch (transform.py:205-219 with normalize_boxes :370-381): each image's xyxy boxes
+        divided by its PRE-resize (h, w) in fp32 (IEEE division, as the reference's tensor-by-tensor division), then
+        cx = (x0 + x1) / 2, cy = (y0 + y1) / 2, w = x1 - x0, h = y1 - y0; rows (image, label, cx, cy, w, h) on the
+        images' device, [0, 6] when there are no boxes.  As in the reference the boxes ignore the letterbox's
+        padding offset.  No host synchronisation: the per-row image index and divisors cross in one copy."""
+        if len(targets) != len(images):
+            raise ValueError(f"{len(images)} images and {len(targets)} targets")
+        dev = images[0].device
+        counts = [int(t["labels"].shape[0]) for t in targets]
+        if sum(counts) == 0:
+            return torch.zeros((0, 6), dtype=torch.float32, device=dev)
+        host = torch.empty((sum(counts), 5), dtype=torch.float32)
+        row = 0
+        for i, (im, c) in enumerate(zip(images, counts)):
+            h, w = float(im.shape[-2]), float(im.shape[-1])
+            host[row:row + c] = torch.tensor([i, w, h, w, h], dtype=torch.float32)
+            row += c
+        host = host.pin_memory().to(dev, non_blocking=True) if dev.type == "cuda" else host.to(dev)
+        boxes = torch.cat([t["boxes"].to(dev, torch.float32) for t, c in zip(targets, counts) if c])
+        labels = torch.cat([t["labels"].to(dev) for t, c in zip(targets, counts) if c]).to(torch.float32)
+        b = boxes / host[:, 1:]
+        x0, y0, x1, y1 = b.unbind(1)
+        return torch.stack([host[:, 0], labels, (x0 + x1) / 2, (y0 + y1) / 2, x1 - x0, y1 - y0], 1)
 
     def batch_images(self, images: List[Tensor]) -> Tensor:
         """Pad already-resized images into one batch (transform.py:297-330): run the kernel with an

@@ -71,16 +71,14 @@ class YOLOv5(nn.Module):
 
     def forward(self, inputs: List[Tensor], targets: Optional[List[Dict[str, Tensor]]] = None):
         if self.training or self.model.has_hooks():
-            # The reference's own staging (yolov5.py:160-189): transform -> model (backbone -> head -> post-process
-            # through the callable sub-modules, so forward hooks fire) -> rescale.  Training mode returns what the
-            # caller's criterion returns; target resizing (transform.py:86-97) belongs to the out-of-scope loss path.
-            if targets is not None and self.training:
-                raise NotImplementedError("target transformation / SetCriterion are out of scope; call model.model(samples, "
-                                          "targets) with a criterion on pre-letterboxed batches")
+            # The reference's own staging (yolov5.py:155-189): transform -> model (backbone -> head -> post-process
+            # through the callable sub-modules, so forward hooks fire) -> rescale.  Training mode letterboxes the
+            # images, batches the normalised targets (transform.py:205-250) and returns what the model's criterion
+            # returns (YOLO(..., criterion=SetCriterion(...)); without one YOLO.forward raises).
             inputs = list(inputs)
             original_image_sizes = [(int(im.shape[-2]), int(im.shape[-1])) for im in inputs]
-            samples, _ = self.transform(inputs, None)
-            outputs = self.model(samples.tensors, None)
+            samples, targets_batched = self.transform(inputs, targets if self.training else None)
+            outputs = self.model(samples.tensors, targets_batched)
             if self.training:
                 return outputs
             hb, wb = int(samples.tensors.shape[-2]), int(samples.tensors.shape[-1])
