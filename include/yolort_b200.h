@@ -505,6 +505,44 @@ int yb_yolo_loss_backward(const yb_yolo_loss_params* params, const yb_loss_level
                           size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Weight gradient of 1x1 convolutions  (the backward of the detection head's nn.Conv2d layers,
+ * yolort/models/box_head.py:35-37,68-82, with respect to weight and bias)
+ *   dW[co][ci] = sum_p dY[p][co] * X[p][ci]      db[co] = sum_p dY[p][co]
+ * over the P = N*H*W pixels of NHWC rows.  Sums are fp32 in a fixed order (split-K partial tiles in the workspace,
+ * then an ordered reduction), rounded once to out_dtype; no float atomics, so a repeated call on the same device gives
+ * the same bits.  Up to YB_WGRAD_MAX_PROBLEMS problems (e.g. the levels of a head) share one launch pair.
+ * ---------------------------------------------------------------------------------------------- */
+#define YB_WGRAD_MAX_PROBLEMS 8
+
+typedef struct {
+  int32_t dtype;               /* YB_F16 / YB_BF16: dy and x (every problem of a call has the same)            */
+  int32_t out_dtype;           /* YB_F32 / YB_F16 / YB_BF16: dw and db                                          */
+  int64_t P;                   /* pixels (rows of dy and x), 1 <= P < 2^31                                      */
+  int32_t Cout, Cin;           /* dw is [Cout][Cin] row-major (the nn.Conv2d weight [Cout, Cin, 1, 1])          */
+  const void* dy;              /* [P][dy_stride], 16-byte aligned; Cout <= dy_stride, dy_stride % 8 == 0        */
+  int64_t dy_stride;
+  const void* x;               /* [P][x_stride], 16-byte aligned; Cin <= x_stride, x_stride % 8 == 0            */
+  int64_t x_stride;
+  void* dw;                    /* [Cout][Cin], aligned to its element size                                      */
+  void* db;                    /* optional [Cout], may be NULL                                                  */
+} yb_wgrad_problem;
+
+/* Host-only: workspace bytes yb_conv_wgrad needs for these problems (0 for an invalid request). */
+size_t yb_conv_wgrad_workspace_bytes(const yb_wgrad_problem* problems, int n);
+
+/* Host-only introspection of the launch (tests, tuning).  `info` receives 8 + 4 * n ints:
+ *   [0] work items (CTA tiles)  [1] grid  [2] dynamic shared memory  [3] pipeline stages  [4] pixels per stage
+ *   [5] output rows per tile  [6] maximum input channels per tile  [7] blocks of 256 outputs in the reduction
+ *   then per problem q at 8 + 4q: output-row tiles, input-channel tiles, pixel slices, pixels per slice.
+ * Slice s of problem q covers pixels [s * len, min((s + 1) * len, P)); every slice is non-empty. */
+int yb_conv_wgrad_config(const yb_wgrad_problem* problems, int n, int32_t* info);
+
+/* Enqueues the partial-tile launch and the reduction launch on `stream`.  No host synchronisation, no allocation.
+ * Argument errors return YB_ERR_INVALID before anything touches the device; a workspace smaller than
+ * yb_conv_wgrad_workspace_bytes returns YB_ERR_WORKSPACE. */
+int yb_conv_wgrad(const yb_wgrad_problem* problems, int n, void* workspace_dev, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Training augmentations (the reference's yolort/data/transforms.py:21-336 on uint8 tensor images, with
  * torchvision's tensor arithmetic; restated in oracle/restate_augment.py).  Each image carries its recipe: the ops
  * its transforms drew, in call order.  Every parameter is drawn on the host; the kernels only compute pixels.

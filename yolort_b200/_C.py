@@ -60,6 +60,9 @@ EXPORTED_SYMBOLS = (
     "yb_yolo_loss_backward",
     "yb_augment_prepare",
     "yb_augment",
+    "yb_conv_wgrad_workspace_bytes",
+    "yb_conv_wgrad_config",
+    "yb_conv_wgrad",
 )
 
 
@@ -225,6 +228,17 @@ class AugImage(ctypes.Structure):
         ("reserved", ctypes.c_int32), ("ops", AugOp * YB_AUG_MAX_OPS),
     ]
 YB_LOSS_MATCH_INT32 = 24
+YB_WGRAD_MAX_PROBLEMS = 8
+
+
+class WgradProblem(ctypes.Structure):
+    """yb_wgrad_problem: one 1x1-convolution weight gradient (include/yolort_b200.h)."""
+    _fields_ = [
+        ("dtype", ctypes.c_int32), ("out_dtype", ctypes.c_int32), ("P", ctypes.c_int64), ("Cout", ctypes.c_int32),
+        ("Cin", ctypes.c_int32), ("dy", ctypes.c_void_p), ("dy_stride", ctypes.c_int64), ("x", ctypes.c_void_p),
+        ("x_stride", ctypes.c_int64), ("dw", ctypes.c_void_p), ("db", ctypes.c_void_p),
+    ]
+
 
 _lib = None
 
@@ -314,6 +328,11 @@ def lib() -> ctypes.CDLL:
     L.yb_augment_prepare.argtypes = [ctypes.c_int, ctypes.POINTER(AugImage), ctypes.POINTER(ctypes.c_int64)]
     L.yb_augment.argtypes = [ctypes.c_int, ctypes.POINTER(AugImage), ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
                              ctypes.c_void_p, ctypes.c_void_p]
+    L.yb_conv_wgrad_workspace_bytes.restype = ctypes.c_size_t
+    L.yb_conv_wgrad_workspace_bytes.argtypes = [ctypes.POINTER(WgradProblem), ctypes.c_int]
+    L.yb_conv_wgrad_config.argtypes = [ctypes.POINTER(WgradProblem), ctypes.c_int, ctypes.POINTER(ctypes.c_int32)]
+    L.yb_conv_wgrad.argtypes = [ctypes.POINTER(WgradProblem), ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
+                                ctypes.c_void_p]
     _lib = L
     return L
 
@@ -948,3 +967,55 @@ def augment(descs, out: torch.Tensor, sources: Sequence[torch.Tensor]) -> torch.
                 seen.add(key)
                 im.record_stream(stream)
     return out
+
+
+# ---------------------------------------------------------------------------------------------------
+# weight gradient of 1x1 convolutions
+# ---------------------------------------------------------------------------------------------------
+def wgrad_problems(specs) -> "ctypes.Array":
+    """yb_wgrad_problem array from (dy [P, >= Cout], x [P, >= Cin], dw [Cout, Cin], db [Cout] or None) tuples of
+    row-major device tensors (unit column stride); dtypes are read from the tensors."""
+    probs = (WgradProblem * len(specs))()
+    for pr, (dy, x, dw, db) in zip(probs, specs):
+        for t, what in ((dy, "dy"), (x, "x")):
+            if t.dim() != 2 or t.stride(1) != 1:
+                raise ValueError(f"conv_wgrad: {what} must be a [P, C] view with unit column stride")
+        if not dw.is_contiguous() or (db is not None and not db.is_contiguous()):
+            raise ValueError("conv_wgrad: dw and db must be contiguous")
+        pr.dtype, pr.out_dtype = dtype_code(dy.dtype), dtype_code(dw.dtype)
+        pr.P, pr.Cout, pr.Cin = int(dy.shape[0]), int(dw.shape[0]), int(dw.shape[1])
+        pr.dy, pr.dy_stride = dy.data_ptr(), int(dy.stride(0))
+        pr.x, pr.x_stride = x.data_ptr(), int(x.stride(0))
+        pr.dw, pr.db = dw.data_ptr(), (db.data_ptr() if db is not None else None)
+        if int(x.shape[0]) != pr.P or dy.dtype != x.dtype:
+            raise ValueError("conv_wgrad: dy and x must have the same rows and dtype")
+        if db is not None and db.dtype != dw.dtype:
+            raise ValueError("conv_wgrad: db must have the dtype of dw")
+    return probs
+
+
+def conv_wgrad_config(probs) -> dict:
+    """How yb_conv_wgrad splits these problems (host-only): launch shape and, per problem, tiles and pixel slices."""
+    n = len(probs)
+    info = (ctypes.c_int32 * (8 + 4 * n))()
+    check(lib().yb_conv_wgrad_config(probs, n, info), "yb_conv_wgrad_config")
+    v = [int(x) for x in info]
+    keys = ("items", "grid", "smem_bytes", "stages", "stage_pixels", "tile_rows", "tile_cols", "reduce_blocks")
+    cfg = dict(zip(keys, v[:8]))
+    cfg["problems"] = [dict(zip(("co_tiles", "ci_tiles", "slices", "slice_len"), v[8 + 4 * q: 12 + 4 * q]))
+                       for q in range(n)]
+    cfg["workspace_bytes"] = int(lib().yb_conv_wgrad_workspace_bytes(probs, n))
+    return cfg
+
+
+def conv_wgrad(specs, device: torch.device) -> None:
+    """yb_conv_wgrad on `device`'s current stream: writes dw (and db) of every (dy, x, dw, db) problem; the fp32
+    workspace comes from torch's caching allocator.  Nothing is synchronised."""
+    probs = wgrad_problems(specs)
+    n = len(probs)
+    ws_bytes = int(lib().yb_conv_wgrad_workspace_bytes(probs, n))
+    if ws_bytes == 0:
+        raise NativeLibraryError(f"conv_wgrad: {lib().yb_last_error().decode('utf-8', 'replace')}")
+    with device_guard(device):
+        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=device)
+        check(lib().yb_conv_wgrad(probs, n, ws.data_ptr(), ws_bytes, current_stream_ptr(device)), "yb_conv_wgrad")

@@ -934,8 +934,40 @@ class Lowered:
         else:
             self.L, self.x0, self.head_bufs, self.feats = lower_yolo(model, dtype, device, stem_variant)
         self.n_heads = len(self.head_bufs)
+        self._model = model
         self.weight_bytes = sum(op.weight.numel() * op.weight.element_size() + op.bias.numel() * 4
                                 for op in self.L.ops if op.weight is not None)
+
+    def head_convs(self) -> Optional[List[nn.Conv2d]]:
+        """The detection head's nn.Conv2d layers in level order when the last n_heads ops of this (non-FP8) lowering are
+        exactly them (YOLO models), else None."""
+        head = getattr(getattr(self._model, "head", None), "head", None)
+        if self.fp8 or not isinstance(head, nn.ModuleList) or len(head) != self.n_heads:
+            return None
+        ops = self.L.ops[len(self.L.ops) - self.n_heads:]
+        if any(op.name != f"head.head.{i}" for i, op in enumerate(ops)):
+            return None
+        return list(head)
+
+    def head_weights(self) -> List[torch.Tensor]:
+        """fp64 [Cout, Cin] weights of the head convolutions (from the parameters)."""
+        return [c.weight.detach().double().view(c.out_channels, c.in_channels) for c in self.head_convs()]
+
+    def refresh_head(self) -> None:
+        """Re-pack and round the head weights and biases from the parameters INTO the tensors every plan points at:
+        the plain and fused-decode launch lists, the chunked front plans, captured CUDA graphs and the feature-gradient
+        packs stay valid.  The bits equal those of a fresh lowering."""
+        convs = self.head_convs()
+        ops = self.L.ops[len(self.L.ops) - self.n_heads:]
+        for op, conv in zip(ops, convs):
+            wp, bp = self.L.pack(conv.weight.detach().double(), conv.bias.detach().double())
+            op.weight.copy_(wp)
+            op.bias.copy_(bp)
+        packs = self.__dict__.get("_head_dgrad_w")
+        if packs is not None:
+            for (wt, _), w in zip(packs, self.head_weights()):
+                wt.copy_(self.L.pack(w.t()[:, :, None, None], torch.zeros(w.shape[1], dtype=torch.float64,
+                                                                            device=w.device))[0])
 
 
 def front_op_count(L: _Lowering) -> int:
@@ -1311,6 +1343,56 @@ class PlanInstance:
         self.plan_fused.run()
 
 
+class _HeadDgrad:
+    """Feature gradient of head level `lvl` for one (N, h, w): dX = dY . W as a one-op plan (1x1 convolution, K = C_pad,
+    no activation) on the conv kernel over the transposed, zero-padded head weight.  `dy` is the plan's input
+    [N, h, w, C_pad] (the caller fills it, pad channels zero); run() returns a fresh [N, h, w, Cin] gradient."""
+
+    def __init__(self, low: "Lowered", lvl: int, N: int, h: int, w: int, cin: int):
+        L = low.L
+        wt, bias = head_dgrad_weights(low)[lvl]
+        head = L.ops[len(L.ops) - low.n_heads + lvl]
+        cpad = head.dst.buf.C
+        self.dy = torch.zeros((N, h, w, cpad), dtype=L.dtype, device=L.device)
+        self.dx = torch.empty((N, h, w, cin), dtype=L.dtype, device=L.device)
+        d = _C.OpDesc()
+        d.kind, d.dtype = _C.YB_OP_CONV, _C.dtype_code(L.dtype)
+        d.N, d.H, d.W, d.Cin, d.in_cstride, d.in_ = N, h, w, cpad, cpad, self.dy.data_ptr()
+        d.Ho, d.Wo, d.Cout, d.out_cstride, d.out = h, w, cin, cin, self.dx.data_ptr()
+        d.ksize, d.stride, d.pad, d.act = 1, 1, 0, _C.YB_ACT_NONE
+        d.weight, d.bias = wt.data_ptr(), bias.data_ptr()
+        d.Cout_pad, _, d.Cin_pad = wt.shape
+        self.plan = _C.Plan([d], L.device)
+        self._keep = (wt, bias)
+
+    def run(self) -> torch.Tensor:
+        self.plan.run()
+        return self.dx.clone()
+
+
+def head_dgrad_weights(low: "Lowered") -> List[Tuple[torch.Tensor, torch.Tensor]]:
+    """Per head level: the transposed head weight W^T [Cin, Cout] packed for the conv kernel, and a zero bias.  Built
+    once per lowering from the fp64 parameters, with the rounding of the forward's packed weights; refreshed in place
+    with them (Engine._refresh_head)."""
+    packs = low.__dict__.get("_head_dgrad_w")
+    if packs is None:
+        packs = [low.L.pack(w.t()[:, :, None, None], torch.zeros(w.shape[1], dtype=torch.float64, device=w.device))
+                 for w in low.head_weights()]
+        low.__dict__["_head_dgrad_w"] = packs
+    return packs
+
+
+def head_dgrad(low: "Lowered", lvl: int, N: int, h: int, w: int, cin: int) -> _HeadDgrad:
+    """The cached _HeadDgrad of (level, N, h, w) on this lowering."""
+    cache = low.__dict__.setdefault("_head_dgrad", {})
+    key = (lvl, N, h, w)
+    inst = cache.get(key)
+    if inst is None:
+        with _C.device_guard(low.L.device):
+            inst = cache[key] = _HeadDgrad(low, lvl, N, h, w, cin)
+    return inst
+
+
 class Engine:
     """Per-model state of the native path: the weights lowered ONCE (BN folded, packed, on the device) and an LRU
     cache of plan instances keyed by (N, H, W).  A new shape costs an arena allocation plus descriptor encoding
@@ -1336,6 +1418,7 @@ class Engine:
         self._versions: Tuple[int, ...] = ()
         self.max_arena_bytes = max_arena_bytes
         self.lowerings = 0       # how many times the weights were folded/packed (tests: stays 1 across shapes)
+        self.head_refreshes = 0  # in-place refreshes of the head weights after head-only parameter edits
         self.stem_variant = "auto"
         self.graphs = False      # replay plans as CUDA graphs (PlanInstance.run_graph)
         # chained pointwise tails (yb_conv_chain); YB_NO_CHAIN=1 keeps every convolution its own launch (A/B timing)
@@ -1350,7 +1433,8 @@ class Engine:
         place since the last lowering (`_version` counters; `.to()` / `load_state_dict` go through YOLO's hooks).
         `fp8`: the FP8 (True) or the `dtype` (False) lowering; default: the one `self.fp8` selects."""
         if (self._low is not None or self._low8 is not None) and self._fingerprint() != self._versions:
-            self.invalidate()
+            if not self._refresh_head():
+                self.invalidate()
         use_fp8 = self.fp8 is not None if fp8 is None else fp8
         if use_fp8:
             if self.fp8 is None:
@@ -1370,6 +1454,28 @@ class Engine:
                 self._low = Lowered(self.model, self.dtype, self.device, self.stem_variant)
             self.lowerings += 1
         return self._low
+
+    def _refresh_head(self) -> bool:
+        """Head fine-tuning: after in-place edits of the head parameters only (an optimizer step) on a model whose
+        other parameters are all frozen (requires_grad False), refresh the packed head weights in place instead of
+        re-lowering; True when that was done.  Any other change, any change while a backbone or neck parameter still
+        requires grad, and any change while an FP8 lowering exists take the full invalidation."""
+        if self._low is None or self._low8 is not None or self.fp8 is not None:
+            return False
+        convs = self._low.head_convs()
+        if convs is None:
+            return False
+        head_ids = {id(t) for c in convs for t in (c.weight, c.bias)}
+        if any(p.requires_grad for p in self.model.parameters() if id(p) not in head_ids):
+            return False
+        cur = self._fingerprint()
+        if any(a != b and id(t) not in head_ids for t, a, b in zip(self._tensors, cur, self._versions)):
+            return False
+        with _C.device_guard(self.device):
+            self._low.refresh_head()
+        self._versions = cur
+        self.head_refreshes += 1
+        return True
 
     def invalidate(self) -> None:
         self._plans.clear()

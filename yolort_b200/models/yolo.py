@@ -6,6 +6,7 @@ batch to the plan's input layout with the letterbox kernel (identity geometry), 
 decode+NMS kernels; nothing is computed by PyTorch ops.
 """
 import os
+import warnings
 from typing import Any, Callable, Dict, List, Optional
 
 import torch
@@ -221,7 +222,23 @@ class YOLO(nn.Module):
 
     def run_head(self, features: List[Tensor]) -> List[Tensor]:
         """`head(features)`: the raw per-level logits [N, A, H, W, nc+5] (yolort/models/box_head.py:68-82); the same
-        list in training and eval mode."""
+        list in training and eval mode.  Differentiable like the reference's nn.Conv2d head when autograd records (grad
+        enabled and a head parameter or a feature requires grad): the logits then carry a grad_fn whose backward
+        computes the head's weight and bias gradients (csrc/conv_wgrad_sm90.cu) and, for features that require grad,
+        the feature gradients.  FP8 plans (set_fp8) keep the logits non-differentiable."""
+        features = list(features)
+        params = self._head_params()
+        if (torch.is_grad_enabled() and self._fp8 is None
+                and (any(p.requires_grad for p in params) or any(f.requires_grad for f in features))):
+            return list(_HeadFunction.apply(self, len(features), *features, *params))
+        return self._run_head_plan(features)
+
+    def _head_params(self) -> List[Tensor]:
+        """weight, bias of every level's 1x1 convolution, in level order."""
+        return [t for conv in self.head.head for t in (conv.weight, conv.bias)]
+
+    def _run_head_plan(self, features: List[Tensor]) -> List[Tensor]:
+        """The head launch range of the plan over `features`; the logits have no grad_fn."""
         # the canvas is the first feature map times its divisor in the lowering (not strides[0]: the lite model's first
         # map sits at stride 16 while its anchor generator says 8)
         self._check_fp8()
@@ -248,6 +265,57 @@ class YOLO(nn.Module):
             n, h, w, _ = hbuf.shape
             outs.append(hbuf[..., : A * K].view(n, h, w, A, K).permute(0, 3, 1, 2, 4).contiguous())
         return outs
+
+    def _head_backward(self, features: List[Tensor], grads: List[Optional[Tensor]], need_params: bool,
+                       need_features: List[bool]):
+        """Gradients of the head launch range: (feature gradients, [dW, db] per level).  The incoming gradients go
+        into zero-padded [P, C_pad] rows of the compute dtype; one yb_conv_wgrad call computes every level's weight and
+        bias gradient in the parameters' dtype; a feature gradient is the 1x1 convolution dY . W on the plan's conv
+        kernel (one-op plans cached per shape on the lowering)."""
+        if any(p.requires_grad for p in self.backbone.parameters()) and not self.__dict__.get("_yb_warned_backbone"):
+            self.__dict__["_yb_warned_backbone"] = True
+            warnings.warn(
+                "only the detection head is trained: the backbone and neck run on the native plan with their running "
+                "BatchNorm statistics and receive no gradient (backward through them is not implemented).  Freeze them "
+                "to state this: model.model.backbone.requires_grad_(False) (model.backbone on a YOLO)", UserWarning,
+                stacklevel=3)
+        from ..engine import head_dgrad
+
+        low = self.engine().lowered()
+        dt = low.L.dtype
+        A, K = self.anchor_generator.num_anchors, self.num_classes + 5
+        convs = list(self.head.head)
+        dys, specs, gparams = [], [], []
+        for lvl, (f, g, conv) in enumerate(zip(features, grads, convs)):
+            n, c, h, w = (int(v) for v in f.shape)
+            co = conv.out_channels
+            dy = head_dgrad(low, lvl, n, h, w, conv.in_channels).dy if need_features[lvl] else \
+                torch.empty((n, h, w, (co + 15) // 16 * 16), dtype=dt, device=f.device)
+            if dy.shape[3] > co:
+                dy[..., co:].zero_()        # pad channels: the dgrad multiplies them by zero weights, NaN must not reach it
+            if g is None:
+                dy[..., :co].zero_()
+            else:
+                dy[..., :co].view(n, h, w, A, K).copy_(g.permute(0, 2, 3, 1, 4))
+            dys.append(dy)
+            if need_params:
+                x = f.permute(0, 2, 3, 1)
+                if x.dtype != dt or not x.is_contiguous():
+                    x = x.to(dt).contiguous()
+                dw = torch.empty((co, c), dtype=conv.weight.dtype, device=f.device)
+                db = torch.empty((co,), dtype=conv.bias.dtype, device=f.device)
+                specs.append((dy.view(-1, dy.shape[3]), x.reshape(-1, c), dw, db))
+                gparams += [dw.view(co, c, 1, 1), db]
+        if need_params:
+            _C.conv_wgrad(specs, features[0].device)
+        gfeats = []
+        for lvl, f in enumerate(features):
+            if not need_features[lvl]:
+                gfeats.append(None)
+                continue
+            n, c, h, w = (int(v) for v in f.shape)
+            gfeats.append(head_dgrad(low, lvl, n, h, w, c).run().permute(0, 3, 1, 2))
+        return gfeats, gparams
 
     def run_plan(self, plan) -> List[Tensor]:
         """backbone + PAN + head on the prepared input canvas; returns the raw head logits (NHWC)."""
@@ -331,6 +399,31 @@ class YOLO(nn.Module):
                     score_thresh=score_thresh, nms_thresh=nms_thresh, post_process=post_process)
         model.load_state_dict(info["state_dict"])
         return model
+
+
+class _HeadFunction(torch.autograd.Function):
+    """The plan's head launch range as an autograd node.  Saves the feature tensors it received (never plan arena
+    buffers, which the next forward overwrites)."""
+
+    @staticmethod
+    def forward(ctx, model: "YOLO", n_feats: int, *args: Tensor):
+        feats = list(args[:n_feats])
+        outs = model._run_head_plan(feats)
+        ctx.model, ctx.n_feats = model, n_feats
+        ctx.save_for_backward(*feats)
+        return tuple(outs)
+
+    @staticmethod
+    def backward(ctx, *grads: Optional[Tensor]):
+        feats = list(ctx.saved_tensors)
+        n = ctx.n_feats
+        need = ctx.needs_input_grad
+        need_features = [bool(need[2 + i]) for i in range(n)]
+        need_params = any(need[2 + n:])
+        gfeats, gparams = ctx.model._head_backward(feats, list(grads), need_params, need_features)
+        if not need_params:
+            gparams = [None] * (len(need) - 2 - n)
+        return (None, None, *gfeats, *gparams)
 
 
 def build_model(backbone_name: str, depth_multiple: float, width_multiple: float, version: str,
