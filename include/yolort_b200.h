@@ -246,11 +246,16 @@ int yb_conv_chain_supported(const yb_op_desc* op);
  *   shared memory   [4] M tiles per weight pass   [5] patch slots (pipeline stages)   [6] weight-ring slabs (k-iterations
  *   per stage)   [7] store-box columns   [8] staging buffers per epilogue group (halo-patch kernel) / epilogue groups
  *   (1x1 / im2col kernel)   [9] dynamic shared memory   [10] grid
- *   [11] flags: bit 0 chained tail fused; bit 1 two CTAs resident per SM (else one).  A convolution takes two CTAs
- *   per SM when its kernel has a two-CTA instance for the N tile (1x1 / im2col: N <= 64 with no tail or a tail of at
- *   most 64 columns; halo patch: N = 32 or 64, or 32 with a 64-column tail, single-tile tasks, resident weights in
- *   one N tile, no banded stem), its plan fits half of
- *   the SM's shared memory and it has at least 2 x SMs tiles; the grid is then up to 2 x SMs.  Pure host logic. */
+ *   [11] flags: bit 0 chained tail fused; bit 1 two CTAs resident per SM (else one); bit 2 two CTAs resident per
+ *   SM of ONE consumer warpgroup each (1x1 / im2col kernel, 64-row tiles; [8] is then 1).  A convolution takes two
+ *   CTAs per SM (bit 1) when its kernel has a two-CTA instance for the N tile (1x1 / im2col: N <= 64 with no tail or
+ *   a tail of at most 64 columns; halo patch: N = 32 or 64, or 32 with a 64-column tail, single-tile tasks, resident
+ *   weights in one N tile, no banded stem), its plan fits half of
+ *   the SM's shared memory and it has at least 2 x SMs tiles; the grid is then up to 2 x SMs.  Otherwise a 1x1 /
+ *   im2col convolution takes two one-warpgroup CTAs per SM (bit 2) when its one-CTA plan has a 256-column N tile and
+ *   no chained tail and it has at least 3 x SMs 128-row tiles: it then runs as two 128-column N tiles ([1], [2])
+ *   whose weights stay resident (at most 80 KB per N tile, one N tile per CTA), in half of the SM's shared memory,
+ *   on a grid of 2 x SMs.  Pure host logic. */
 int yb_conv_config(const yb_op_desc* op, int32_t* info12);
 
 typedef struct yb_plan yb_plan;

@@ -481,7 +481,12 @@ def conv_config(op: "OpDesc") -> dict:
     keys = ("patch_kernel", "block_n", "n_tiles", "weights_resident", "tiles_per_pass", "slots", "ring", "store_cols",
             "store_bufs", "smem_bytes", "grid", "chained")
     cfg = dict(zip(keys, [int(v) for v in info]))
-    cfg["ctas_per_sm"] = 2 if cfg["chained"] & 2 else 1   # slot 11: bit 0 chained tail, bit 1 two CTAs per SM
+    # slot 11: bit 0 chained tail, bit 1 two CTAs per SM of the 104-register instances, bit 2 two CTAs per SM of one
+    # consumer warpgroup each.  "ctas_per_sm" keeps naming the 104-register layout; "resident_ctas" counts both.
+    flags = cfg["chained"]
+    cfg["ctas_per_sm"] = 2 if flags & 2 else 1
+    cfg["resident_ctas"] = 2 if flags & 6 else 1
+    cfg["layout"] = "2x2" if flags & 2 else ("2x1" if flags & 4 else "1x2")   # CTAs per SM x consumer warpgroups
     cfg["chained"] &= 1
     cfg["e4m3_kernel"] = int(cfg["patch_kernel"] == 2)   # slot 0 is 2 for the e4m3 kernel (conv_fp8_sm90.cu)
     cfg["patch_kernel"] = int(cfg["patch_kernel"] == 1)

@@ -334,16 +334,20 @@ __device__ __forceinline__ void wgmma_mma(float* d, uint64_t da, uint64_t db, bo
 //   1: ptxas gives every thread 168 registers; 40 x 128 + 232 x 256 <= 384 x 168 (64 K registers per SM).
 //   2: ptxas gives every thread 80 registers (the cap it reports for __launch_bounds__(384, 2));
 //      24 x 128 + 104 x 256 <= 384 x 80, 104 being the largest multiple of 8 that fits.
-template <int kCtas>
+// kGroups = 1 (conv_sm90.cu: one consumer warpgroup, 256 threads, two CTAs per SM): __launch_bounds__(256, 2) gives every
+// thread 128 registers; 24 x 128 + 232 x 128 = 256 x 128, the one-CTA consumers' budget.
+template <int kCtas, int kGroups = 2>
 __device__ __forceinline__ void regs_producer() {
   static_assert(kCtas == 1 || kCtas == 2, "1 or 2 CTAs per SM");
+  static_assert(kGroups == 2 || kCtas == 2, "one consumer warpgroup runs two CTAs per SM");
   if constexpr (kCtas == 1) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
   else asm volatile("setmaxnreg.dec.sync.aligned.u32 24;\n" ::: "memory");
 }
-template <int kCtas>
+template <int kCtas, int kGroups = 2>
 __device__ __forceinline__ void regs_consumer() {
   static_assert(kCtas == 1 || kCtas == 2, "1 or 2 CTAs per SM");
-  if constexpr (kCtas == 1) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+  static_assert(kGroups == 2 || kCtas == 2, "one consumer warpgroup runs two CTAs per SM");
+  if constexpr (kCtas == 1 || kGroups == 1) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
   else asm volatile("setmaxnreg.inc.sync.aligned.u32 104;\n" ::: "memory");
 }
 

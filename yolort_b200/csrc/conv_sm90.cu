@@ -16,6 +16,9 @@
 //                accumulators in registers), then runs the epilogue on its fragment: +bias -> activation -> (+residual)
 //                -> fp16/bf16 -> swizzled shared-memory staging -> TMA store into the NHWC destination view (a channel
 //                window of a concat buffer is just a strided tensor map; ragged M is clipped by the TMA unit).
+// Instances with ONE consumer warpgroup (256 threads, 64-row tiles, two CTAs per SM at the consumers' 232 registers) run
+// the same protocol with half the participants: the two co-resident CTAs take the place of the two consumer warpgroups,
+// and one CTA's epilogue overlaps the other's MMAs.
 // The kernel is a template over (dtype, activation family, fused decode, chained tail).  A chained tail
 // (conv_chain.cuh) is a second, pointwise GEMM over the tile the epilogue has just staged: the consumers multiply the
 // staged boxes with the resident tail weights and a second epilogue pass stores the result.
@@ -31,16 +34,17 @@ namespace yb {
 
 namespace {
 
-constexpr int kBlockM = 128;
 constexpr int kMaxStages = 12;
-constexpr int kConsumers = 2;                         // consumer warpgroups (64 accumulator rows each)
-constexpr int kThreads = 128 * (1 + kConsumers);
-constexpr int kStageBufBytes = 128 * 128;  // 128 rows x (up to) 64 columns x 2 B
-constexpr int kStageBufs = 2;              // staging boxes, shared by the two consumer warpgroups
+// consumer warpgroups per CTA (64 accumulator rows each): 2, or 1 in the 64-row-tile instances
+__host__ __device__ constexpr int tile_rows(int groups) { return 64 * groups; }
+__host__ __device__ constexpr int cta_threads(int groups) { return 128 * (1 + groups); }
+// staging box: the tile's rows x (up to) 64 columns x 2 B
+__host__ __device__ constexpr int stage_buf_bytes(int groups) { return tile_rows(groups) * 128; }
+constexpr int kStageBufs = 2;              // staging boxes, shared by the consumer warpgroups
 constexpr int kMaxBlockN = 256;
 constexpr size_t kSmemBudget = 216 * 1024;  // dynamic shared memory per CTA (227 KB limit minus static)
 constexpr size_t kStaticSmem = (2 * kMaxStages + 2) * 8 + 2 * kMaxBlockN * 4;   // barriers + bias vectors (ptxas -v)
-constexpr uint32_t kConsumerBar = 1;        // named barrier of the 256 consumer threads
+constexpr uint32_t kConsumerBar = 1;        // named barrier of the consumer threads
 
 struct ConvKernelParams {
   int M, block_n, block_k;
@@ -53,6 +57,7 @@ struct ConvKernelParams {
   uint32_t b_res_bytes;
   int n_tiles, num_tiles;
   int ctas;        // CTAs per SM the launch is planned for (1 or 2): selects the kernel instance
+  int groups;      // consumer warpgroups per CTA (2, or 1 with two CTAs per SM): selects the kernel instance
   int store_cols;  // columns per TMA store box: 64 / 32 / 16
   int bias_len;    // length of the (padded) bias vector
   int kk_last;     // K=16 steps of the LAST channel chunk (Cin need not fill it: TMA zero-fills, the MMA skips)
@@ -65,7 +70,8 @@ struct ConvKernelParams {
   yb_head_decode dec;   // copied from the op descriptor
 };
 
-__device__ __forceinline__ void consumer_sync() { named_bar_sync(kConsumerBar, 128 * kConsumers); }
+template <int kGroups>
+__device__ __forceinline__ void consumer_sync() { named_bar_sync(kConsumerBar, 128 * kGroups); }
 
 // Fused post-processing front end (yolort/models/box_head.py:328-360,418) on the head's accumulator fragment.  Objectness
 // and box logits of every (row, anchor) go through a small shared-memory table (they sit in other lanes' registers);
@@ -158,14 +164,18 @@ __device__ __forceinline__ void decode_fragment(const yb_head_decode& D, const f
 // kN: the wgmma N of the tile (= block_n; kN / 2 accumulator registers per thread).  kDecode: detection head with the
 // fused decode (nothing stored).  kN2 != 0: a
 // pointwise tail is chained onto every tile (conv_chain.cuh).  kCtas: CTAs resident per SM (1 or 2, see
-// regs_producer); with two, one CTA's epilogue and barrier waits overlap the other CTA's MMAs and loads.
-template <bool kBf16, int kN, bool kDecode, int kN2, int kCtas>
-__global__ void __launch_bounds__(kThreads, kCtas)
+// regs_producer); with two, one CTA's epilogue and barrier waits overlap the other CTA's MMAs and loads.  kGroups:
+// consumer warpgroups per CTA (2: 128-row tiles; 1: 64-row tiles, two CTAs per SM with 232 consumer registers).
+template <bool kBf16, int kN, bool kDecode, int kN2, int kCtas, int kGroups = 2>
+__global__ void __launch_bounds__(cta_threads(kGroups), kCtas)
 conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_w2,
                   const __grid_constant__ CUtensorMap tmap_out2, const ConvKernelParams p) {
+  static_assert(kGroups == 2 || (kGroups == 1 && kCtas == 2 && !kDecode), "one consumer warpgroup: two CTAs, no decode");
   constexpr bool kChain = kN2 != 0;
   constexpr int kAcc = (kN > kN2 ? kN : kN2) / 2;   // accumulator registers per thread
+  constexpr int kBlockM = tile_rows(kGroups);
+  constexpr int kStageBufBytes = stage_buf_bytes(kGroups);
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
@@ -192,7 +202,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     tma_prefetch_desc(&tmap_out);
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kConsumers);   // one arrival per consumer warpgroup
+      mbar_init(&empty_bar[s], kGroups);   // one arrival per consumer warpgroup
     }
     mbar_init(&b_full, 1);
     mbar_init(&w2_full, 1);
@@ -203,11 +213,12 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   // Programmatic dependent launch: everything above overlapped the tail of the previous kernel in the stream.
   // Resident weights do not depend on the previous kernel: their loads are issued BEFORE the grid-dependency wait
   // and stream in while the previous kernel drains.
-  if (threadIdx.x == 0 && p.b_resident) {
+  if (threadIdx.x == 0 && p.b_resident) {   // the CTA's one N tile (conv_plan: the grid is a multiple of n_tiles)
     const uint32_t b_bytes = p.block_n * p.block_k * 2;
+    const int n0 = (blockIdx.x % p.n_tiles) * p.block_n;
     mbar_expect_tx(&b_full, p.num_k_iters * b_bytes);
     for (int it = 0; it < p.num_k_iters; ++it)
-      tma_load_2d(&tmap_b, &b_full, b_res + it * p.b_stage_bytes, it * p.block_k, 0);
+      tma_load_2d(&tmap_b, &b_full, b_res + it * p.b_stage_bytes, it * p.block_k, n0);
   }
   if constexpr (kChain) {
     if (threadIdx.x == 0) {   // tail weights: [n2][kc] chunks, resident for the CTA's lifetime
@@ -222,7 +233,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
   if (warp < 4) {
-    regs_producer<kCtas>();
+    regs_producer<kCtas, kGroups>();
     if (warp != 0) return;
     // ===================== TMA producer (warp-uniform loop, one elected lane issues) =====================
     const uint32_t a_bytes = kBlockM * p.block_k * 2, b_bytes = p.block_n * p.block_k * 2;
@@ -270,7 +281,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   }
 
   // ===================== consumers: MMA + epilogue of 64 rows each =====================
-  regs_consumer<kCtas>();
+  regs_consumer<kCtas, kGroups>();
   const int g = (warp >> 2) - 1;
   const int wq = warp & 3;
   const bool issuer = threadIdx.x == 128;
@@ -289,16 +300,16 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   float acc[kAcc];
 
   if constexpr (kChain) {   // the tail has a single N tile: its bias is the same for every tile
-    for (int i = ctid; i < p.ch.n2; i += 128 * kConsumers) s_bias2[i] = (i < p.ch.bias2_len) ? __ldg(p.ch.bias2 + i) : 0.f;
+    for (int i = ctid; i < p.ch.n2; i += 128 * kGroups) s_bias2[i] = (i < p.ch.bias2_len) ? __ldg(p.ch.bias2 + i) : 0.f;
   }
   // Every tile of this CTA has the same N tile when the grid is a multiple of the N-tile count (always with one N
   // tile): the bias is then loaded ONCE instead of per tile.
   const bool fixed_n = (gridDim.x % p.n_tiles) == 0;
   if (fixed_n) {
     const int n0f = (blockIdx.x % p.n_tiles) * p.block_n;
-    for (int i = ctid; i < p.block_n; i += 128 * kConsumers) s_bias[i] = (n0f + i < p.bias_len) ? __ldg(p.bias + n0f + i) : 0.f;
+    for (int i = ctid; i < p.block_n; i += 128 * kGroups) s_bias[i] = (n0f + i < p.bias_len) ? __ldg(p.bias + n0f + i) : 0.f;
   }
-  consumer_sync();
+  consumer_sync<kGroups>();
   if (p.b_resident) mbar_wait(&b_full, 0);
   if constexpr (kChain) mbar_wait(&w2_full, 0);
 
@@ -308,8 +319,8 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     const int n0 = (tile - m_tile * p.n_tiles) * p.block_n;
     const int m0 = m_tile * kBlockM;
     if (!fixed_n) {   // the previous tile's epilogue has finished with the bias (and the staging boxes)
-      consumer_sync();
-      for (int i = ctid; i < p.block_n; i += 128 * kConsumers) s_bias[i] = (n0 + i < p.bias_len) ? __ldg(p.bias + n0 + i) : 0.f;
+      consumer_sync<kGroups>();
+      for (int i = ctid; i < p.block_n; i += 128 * kGroups) s_bias[i] = (n0 + i < p.bias_len) ? __ldg(p.bias + n0 + i) : 0.f;
     }
 
     // ---- main loop: stage s is released once the MMAs that read it have completed (one stage in flight) ----
@@ -338,7 +349,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     wgmma_wait<0>();
     fence_acc<kN / 2>(acc);
     if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev_s]);
-    if (!fixed_n) consumer_sync();   // bias visible
+    if (!fixed_n) consumer_sync<kGroups>();   // bias visible
 
     fr.row[0] = static_cast<long long>(m0) + fr.loc[0];
     fr.row[1] = static_cast<long long>(m0) + fr.loc[1];
@@ -351,7 +362,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       // chain tiles index the staging buffers by box (box b of the tile stays in buffer b until the tail GEMM has read
       // it), so the previous tile's stores must have drained both buffers before this tile writes them
       if (issuer) tma_store_wait_read<0>();
-      consumer_sync();
+      consumer_sync<kGroups>();
     }
     for (int c0 = 0; c0 < bn; c0 += store_cols, ++store_idx) {
       // Two staging buffers, one barrier per box: before the barrier below the issuer waits until the PREVIOUS
@@ -362,7 +373,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       if constexpr (!kChain) {
         if (issuer) tma_store_wait_read<0>();
       }
-      consumer_sync();
+      consumer_sync<kGroups>();
       if (issuer) {
         if ((!kChain || p.ch.store_first) && n0 + c0 < p.ep.Cout) tma_store_2d(&tmap_out, buf, n0 + c0, m0);
         tma_store_commit();
@@ -385,14 +396,14 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       // the tail's boxes reuse the staging buffers: the operand boxes are dead (both warpgroups' tail GEMMs have
       // completed), but the stores of the first output may still be reading them
       if (issuer) tma_store_wait_read<0>();
-      consumer_sync();
+      consumer_sync<kGroups>();
       const int s2 = chain_store2_cols(p.ch.n2);
       for (int c0 = 0; c0 < p.ch.n2; c0 += s2) {
         uint8_t* buf = staging + ((c0 / s2) & 1) * kStageBufBytes;
         epilogue_box<kBf16, kChain ? kN2 : 16>(p.ch.ep2, acc, c0, s2, s_bias2, fr, 0, buf, lane);
         fence_proxy_async_smem();
         if (issuer) tma_store_wait_read<0>();   // box k + 1 overwrites the buffer of box k - 1
-        consumer_sync();
+        consumer_sync<kGroups>();
         if (issuer) {
           if (c0 < p.ch.ep2.Cout) tma_store_2d(&tmap_out2, buf, c0, m0);
           tma_store_commit();
@@ -454,11 +465,18 @@ int encode_im2col_entry(EncodeIm2colFn* out) {
 using ConvKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
                               const ConvKernelParams);
 
-// One kernel per (dtype, N tile, fused decode, chained tail N, CTAs per SM): the MMA width and the accumulator size are
-// compile-time constants of every instance, so the accumulators stay in registers while the wgmma instructions are in
-// flight.  conv_configure admits exactly these shapes.
+// One kernel per (dtype, N tile, fused decode, chained tail N, CTAs per SM, consumer warpgroups): the MMA width and the
+// accumulator size are compile-time constants of every instance, so the accumulators stay in registers while the wgmma
+// instructions are in flight.  conv_configure admits exactly these shapes.
 template <bool kBf16>
 ConvKernelFn select_conv_kernel_t(const ConvKernelParams& kp) {
+  if (kp.groups == 1) {
+    // one consumer warpgroup, two CTAs per SM, at the one-CTA instances' 232 consumer registers: the 256-column layers,
+    // as two 128-column N tiles (conv_plan).  No N = 256 instance: ptxas allocates against the 128 registers of
+    // __launch_bounds__(256, 2), and one m64n256 wgmma needs 128 accumulators plus its operands.
+    if (kp.ctas != 2 || kp.decode_on || kp.ch.on) return nullptr;
+    return kp.block_n == 128 ? conv_wgmma_kernel<kBf16, 128, false, 0, 2, 1> : nullptr;
+  }
   if (kp.ctas == 2) {
     // two CTAs per SM: the instances whose consumers fit in 104 registers without spilling (N <= 64, tails of at most
     // 64 columns; DESIGN.md section 3)
@@ -504,7 +522,7 @@ struct ConvOp {
   size_t smem_bytes;
 };
 
-static int conv_plan(const yb_op_desc& d, int ctas, ConvKernelParams& kp, dim3& grid, size_t& smem_bytes);
+static int conv_plan(const yb_op_desc& d, int ctas, int groups, ConvKernelParams& kp, dim3& grid, size_t& smem_bytes);
 
 // Pure host logic: validates the op and derives tiling, pipeline depth, shared-memory layout and launch shape
 // (no driver calls: yb_conv_chain_supported runs this without a GPU).
@@ -537,31 +555,47 @@ static int conv_configure(const yb_op_desc& d, ConvKernelParams& kp, dim3& grid,
              "conv: banded stem weights (reserved bit 1) need the halo-patch kernel, which this %dx%d map does not qualify for",
              d.H, d.W);
   if (patch_conv_eligible(d)) return YB_OK;   // configured by patch_conv_configure
-  // Two CTAs per SM when the shape has a two-CTA instance, its plan fits half of the SM's shared memory and there are
-  // tiles for both (reserved bit 4 keeps one CTA per SM: tests compare the two launches bit for bit).
-  if (!(d.reserved & 16) && conv_plan(d, 2, kp, grid, smem_bytes) == YB_OK) return YB_OK;
-  return conv_plan(d, 1, kp, grid, smem_bytes);
+  // Three layouts, tried in this order:
+  //   two CTAs of two consumer warpgroups (104 registers) when the shape has such an instance;
+  //   otherwise two CTAs of ONE consumer warpgroup (64-row tiles, 232 registers) when the shape has that instance;
+  //   one CTA of two consumer warpgroups.
+  // Each two-CTA plan must fit half of the SM's shared memory and have a tile for each of the 2 x SMs CTAs.  Reserved
+  // bit 4 keeps the last layout (tests compare the launches bit for bit).
+  if (!(d.reserved & 16) &&
+      (conv_plan(d, 2, 2, kp, grid, smem_bytes) == YB_OK || conv_plan(d, 2, 1, kp, grid, smem_bytes) == YB_OK))
+    return YB_OK;
+  return conv_plan(d, 1, 2, kp, grid, smem_bytes);
 }
 
-// Tiling, pipeline depth, shared-memory layout and launch shape for `ctas` CTAs per SM (conv_configure has validated the
-// descriptor).  With ctas = 2 the plan gets half of the SM's shared memory, less the per-CTA reservation and the
-// kernel's static shared memory, and fails when it does not fit there, when the shape has no two-CTA instance or when
-// there are fewer tiles than 2 x SMs.
-static int conv_plan(const yb_op_desc& d, int ctas, ConvKernelParams& kp, dim3& grid, size_t& smem_bytes) {
+// Tiling, pipeline depth, shared-memory layout and launch shape for `ctas` CTAs per SM of `groups` consumer warpgroups
+// (conv_configure has validated the descriptor).  With ctas = 2 the plan gets half of the SM's shared memory, less the
+// per-CTA reservation and the kernel's static shared memory, and fails when it does not fit there, when the layout has
+// no instance for the shape or when there are fewer tiles than 2 x SMs.  One consumer warpgroup is only planned for
+// shapes without a 104-register two-CTA instance.
+static int conv_plan(const yb_op_desc& d, int ctas, int groups, ConvKernelParams& kp, dim3& grid, size_t& smem_bytes) {
   const int Ho = d.Ho, Wo = d.Wo;
   const long long M_ll = static_cast<long long>(d.N) * Ho * Wo;
   const size_t budget = ctas == 2 ? smem_per_sm() / 2 - kSmemReservedPerCta - kStaticSmem : kSmemBudget;
+  const int block_m = tile_rows(groups);
   kp = ConvKernelParams();
   kp.ctas = ctas;
+  kp.groups = groups;
   kp.M = static_cast<int>(M_ll);
   kp.ep.Cout = d.Cout;
-  const int m_tiles = (kp.M + kBlockM - 1) / kBlockM;
+  const int m_tiles = (kp.M + block_m - 1) / block_m;
   const int sms = num_sms();
   // N tile: the whole Cout up to 256 columns (fewest A re-reads); halve it when that leaves fewer
-  // than two tiles per SM so the persistent grid balances better.
+  // than two 128-row tiles per SM so the persistent grid balances better (the same N tile in every layout).
   int n_tiles = (d.Cout + kMaxBlockN - 1) / kMaxBlockN;
   int block_n = mma_n((d.Cout + n_tiles - 1) / n_tiles);
-  if (m_tiles * n_tiles < 2 * sms && block_n > 128 && d.chain == nullptr) block_n /= 2;
+  const int m_tiles128 = (kp.M + tile_rows(2) - 1) / tile_rows(2);
+  if (m_tiles128 * n_tiles < 2 * sms && block_n > 128 && d.chain == nullptr) block_n /= 2;
+  if (groups == 1) {
+    // one consumer warpgroup: only layers whose one-CTA plan has a 256-column N tile, split into two 128-column ones,
+    // with at least 3 x SMs 128-row tiles (DESIGN.md section 3: measured gains at 400 and 1600 such tiles, none at 100)
+    if (block_n != 256 || d.chain != nullptr || m_tiles128 < 3 * sms) return YB_ERR_INVALID;
+    block_n = 128;
+  }
   n_tiles = (d.Cout + block_n - 1) / block_n;
   YB_REQUIRE(mma_n(block_n) == block_n && block_n <= kMaxBlockN, "conv: N tile %d is not a wgmma N", block_n);
   kp.block_n = block_n;
@@ -602,7 +636,7 @@ static int conv_plan(const yb_op_desc& d, int ctas, ConvKernelParams& kp, dim3& 
   kp.kk_last = (d.Cin - (kp.chunks - 1) * kp.block_k + 15) / 16;
   if (kp.kk_last < 1) kp.kk_last = 1;
   if (kp.kk_last > (kp.block_k >> 4)) kp.kk_last = kp.block_k >> 4;
-  kp.a_stage_bytes = kBlockM * kp.block_k * 2;
+  kp.a_stage_bytes = block_m * kp.block_k * 2;
   kp.b_stage_bytes = (static_cast<uint32_t>(kp.block_n * kp.block_k * 2) + 1023u) & ~1023u;
   kp.ch.on = 0;
   size_t chain_bytes = 0;
@@ -618,10 +652,13 @@ static int conv_plan(const yb_op_desc& d, int ctas, ConvKernelParams& kp, dim3& 
     chain_bytes = static_cast<size_t>(kp.ch.w2_chunks) * kp.ch.w2_sub_bytes;
   }
   // Weights stay resident in shared memory when the layer has a single N tile and they are small:
-  // the persistent CTA then streams only activations (halves the L2->SM traffic of the shallow layers).
-  const size_t fixed = static_cast<size_t>(kStageBufs) * kStageBufBytes + 1024 + chain_bytes;
+  // the persistent CTA then streams only activations (halves the L2->SM traffic of the shallow layers).  A one-group
+  // plan (grid 2 x SMs) also keeps them resident over several N tiles when the grid is a multiple of the N tiles: every
+  // CTA then has one N tile and holds its weights.
+  const size_t fixed = static_cast<size_t>(kStageBufs) * stage_buf_bytes(groups) + 1024 + chain_bytes;
   const size_t b_total = static_cast<size_t>(kp.num_k_iters) * kp.b_stage_bytes;
-  kp.b_resident = (n_tiles == 1 && b_total <= 80 * 1024) ? 1 : 0;
+  const bool fixed_n = n_tiles == 1 || (groups == 1 && (2 * sms) % n_tiles == 0);
+  kp.b_resident = (fixed_n && b_total <= 80 * 1024) ? 1 : 0;
   kp.b_res_bytes = kp.b_resident ? static_cast<uint32_t>(b_total) : 0u;
   // k-iterations per pipeline stage: aim at ~32 KB per stage so that one mbarrier round trip moves
   // enough bytes (a 16-channel tap is only 4 KB), in near-equal groups.
@@ -632,8 +669,8 @@ static int conv_plan(const yb_op_desc& d, int ctas, ConvKernelParams& kp, dim3& 
   int kpg_max = static_cast<int>(target / per_iter);
   if (kpg_max < 1) kpg_max = 1;
   if (kpg_max > kp.num_k_iters) kpg_max = kp.num_k_iters;
-  const int groups = (kp.num_k_iters + kpg_max - 1) / kpg_max;
-  kp.kpg = (kp.num_k_iters + groups - 1) / groups;
+  const int kgroups = (kp.num_k_iters + kpg_max - 1) / kpg_max;
+  kp.kpg = (kp.num_k_iters + kgroups - 1) / kgroups;
   const uint32_t stage_bytes = kp.kpg * per_iter;
   int stages = static_cast<int>(avail / stage_bytes);
   if (stages > kMaxStages) stages = kMaxStages;
@@ -646,7 +683,12 @@ static int conv_plan(const yb_op_desc& d, int ctas, ConvKernelParams& kp, dim3& 
   kp.ep.res_cstride = d.res_cstride;
   // two CTAs per SM: only with an instance built for it and at least one tile for each of the 2 x SMs CTAs
   if (ctas == 2 && (select_conv_kernel(kp) == nullptr || kp.num_tiles < 2 * sms)) return YB_ERR_INVALID;
-  const int max_grid = ctas * sms;   // every two-CTA instance has one N tile: any grid keeps the N tile fixed per CTA
+  if (groups == 1) {   // only with resident weights, and where the shape has no 104-register two-CTA instance
+    ConvKernelParams two = kp;
+    two.groups = 2;
+    if (!kp.b_resident || select_conv_kernel(two) != nullptr) return YB_ERR_INVALID;
+  }
+  const int max_grid = ctas * sms;   // a grid that is not a multiple of the N tiles loads the bias per tile
   grid = dim3(kp.num_tiles < max_grid ? kp.num_tiles : max_grid, 1, 1);
   const size_t smem = static_cast<size_t>(stages) * stage_bytes + kp.b_res_bytes + fixed;
   YB_REQUIRE(smem <= budget, "conv: %zu bytes of shared memory needed, %zu available", smem, budget);
@@ -668,10 +710,11 @@ int conv_configure_check(const yb_op_desc& d, int* info) {
     info[5] = kp.stages;
     info[6] = kp.kpg;
     info[7] = kp.store_cols;
-    info[8] = kConsumers;         // (im2col / 1x1 kernel: consumer warpgroups; they share two staging buffers)
+    info[8] = kp.groups;          // (im2col / 1x1 kernel: consumer warpgroups; they share two staging buffers)
     info[9] = static_cast<int>(smem);
     info[10] = static_cast<int>(grid.x);
-    info[11] = kp.ch.on | (kp.ctas == 2 ? 2 : 0);
+    // bit 1: two CTAs of the 104-register instances; bit 2: two CTAs of one consumer warpgroup
+    info[11] = kp.ch.on | (kp.ctas == 2 ? (kp.groups == 2 ? 2 : 4) : 0);
   }
   return rc;
 }
@@ -697,6 +740,7 @@ int conv_op_create(const yb_op_desc& d, ConvOp** out) {
   ConvKernelParams& kp = op->kp;
   const int Ho = d.Ho, Wo = d.Wo;
   (void)Ho; (void)Wo;
+  const cuuint32_t block_m = tile_rows(kp.groups);   // rows of the A, output and tail-output boxes
 
   const CUtensorMapDataType dt =
       kp.ep.is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
@@ -705,7 +749,7 @@ int conv_op_create(const yb_op_desc& d, ConvOp** out) {
   if (kp.mode == 0) {
     cuuint64_t dims[2] = {static_cast<cuuint64_t>(d.Cin), static_cast<cuuint64_t>(kp.M)};
     cuuint64_t strides[1] = {static_cast<cuuint64_t>(d.in_cstride) * 2};
-    cuuint32_t box[2] = {static_cast<cuuint32_t>(kp.block_k), kBlockM};
+    cuuint32_t box[2] = {static_cast<cuuint32_t>(kp.block_k), block_m};
     cuuint32_t estr[2] = {1, 1};
     cr = g_encode_tiled(&op->tmap_a, dt, 2, const_cast<void*>(d.in), dims, strides, box, estr,
                         CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
@@ -720,7 +764,7 @@ int conv_op_create(const yb_op_desc& d, ConvOp** out) {
     int upper[2] = {d.pad - (d.ksize - 1), d.pad - (d.ksize - 1)};
     cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(d.stride), static_cast<cuuint32_t>(d.stride), 1};
     cr = g_encode_im2col(&op->tmap_a, dt, 4, const_cast<void*>(d.in), dims, strides, lower, upper,
-                         static_cast<cuuint32_t>(kp.block_k), kBlockM, estr,
+                         static_cast<cuuint32_t>(kp.block_k), block_m, estr,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     // Driver workaround also applied by CUTLASS (copy_traits_sm90_im2col.hpp): for tensors smaller
@@ -755,10 +799,10 @@ int conv_op_create(const yb_op_desc& d, ConvOp** out) {
     }
   }
   {
-    // destination view [M rows, Cout channels], row pitch = out_cstride; boxes of 128 rows x store_cols
+    // destination view [M rows, Cout channels], row pitch = out_cstride; boxes of block_m rows x store_cols
     cuuint64_t dims[2] = {static_cast<cuuint64_t>(d.Cout), static_cast<cuuint64_t>(kp.M)};
     cuuint64_t strides[1] = {static_cast<cuuint64_t>(d.out_cstride) * 2};
-    cuuint32_t box[2] = {static_cast<cuuint32_t>(kp.store_cols), kBlockM};
+    cuuint32_t box[2] = {static_cast<cuuint32_t>(kp.store_cols), block_m};
     cuuint32_t estr[2] = {1, 1};
     cr = g_encode_tiled(&op->tmap_out, dt, 2, d.out, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                         swizzle_for_row_bytes(kp.store_cols * 2), CU_TENSOR_MAP_L2_PROMOTION_NONE,
@@ -784,7 +828,7 @@ int conv_op_create(const yb_op_desc& d, ConvOp** out) {
       const int s2 = chain_store2_cols(kp.ch.n2);
       cuuint64_t odims[2] = {static_cast<cuuint64_t>(c.Cout), static_cast<cuuint64_t>(kp.M)};
       cuuint64_t ostrides[1] = {static_cast<cuuint64_t>(c.out_cstride) * 2};
-      cuuint32_t obox[2] = {static_cast<cuuint32_t>(s2), kBlockM};
+      cuuint32_t obox[2] = {static_cast<cuuint32_t>(s2), block_m};
       cr = g_encode_tiled(&op->tmap_out2, dt, 2, c.out, odims, ostrides, obox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                           swizzle_for_row_bytes(s2 * 2), CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     }
@@ -795,7 +839,8 @@ int conv_op_create(const yb_op_desc& d, ConvOp** out) {
     }
   }
   op->fn = select_conv_kernel(kp);
-  rc = set_smem_attributes(reinterpret_cast<const void*>(op->fn), kSmemBudget, kp.ctas, op->smem_bytes, kThreads, "conv");
+  rc = set_smem_attributes(reinterpret_cast<const void*>(op->fn), kSmemBudget, kp.ctas, op->smem_bytes, cta_threads(kp.groups),
+                           "conv");
   if (rc != YB_OK) {
     delete op;
     return rc;
@@ -808,7 +853,7 @@ int conv_op_launch(const ConvOp* op, cudaStream_t stream) {
   if (op->patch) return patch_conv_launch(op->patch, stream);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = op->grid;
-  cfg.blockDim = dim3(kThreads, 1, 1);
+  cfg.blockDim = dim3(cta_threads(op->kp.groups), 1, 1);
   cfg.dynamicSmemBytes = op->smem_bytes;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
