@@ -595,6 +595,42 @@ int yb_augment_prepare(int n_images, yb_aug_image* images, int64_t* totals);
 int yb_augment(int n_images, const yb_aug_image* images_host, const yb_aug_image* images_dev, void* out_dev,
                int32_t out_dtype, uint64_t* sums_dev, void* stream);
 
+/* The device parameter sampler (Compose.apply_batch(..., generator=)): the transforms of a Compose, each drawn from
+ * Philox4x32-10 with key = the call's 64-bit draw and counter = (image, transform index, a, b).  The rules are
+ * restated in oracle/sample_augment.py. */
+#define YB_AUG_MAX_TRANSFORMS 16
+#define YB_AUG_MAX_OPTIONS 16
+#define YB_AUG_CROP_ROUNDS 1024    /* IoU-crop rounds before an image gives up                               */
+#define YB_AUG_S_NONE 0            /* PILToTensor, ConvertImageDtype: no draw                                */
+#define YB_AUG_S_PHOTOMETRIC 1     /* p; jitter bit j: range j (brightness, contrast, saturation, hue) drawn  */
+#define YB_AUG_S_ZOOM_OUT 2        /* p; range 0 = side range; fill                                          */
+#define YB_AUG_S_IOU_CROP 3        /* range 0 = scale; aspect bounds; options; trials                        */
+#define YB_AUG_S_HFLIP 4           /* p                                                                      */
+#define YB_AUG_ST_CROP_ROUNDS 1    /* status: an IoU crop accepted no window in YB_AUG_CROP_ROUNDS rounds   */
+
+typedef struct {
+  int32_t kind;                /* YB_AUG_S_*                                                                  */
+  int32_t jitter;
+  int32_t trials, n_options;
+  uint32_t fill;               /* r | g<<8 | b<<16                                                            */
+  float p;                     /* a transform applies when its uniform is below p                             */
+  float lo[4], span[4];        /* a value drawn from a range is lo + u * span in fp32                         */
+  double min_aspect, max_aspect;
+  double options[YB_AUG_MAX_OPTIONS];
+} yb_aug_sampler;
+
+/* Draws every image's recipe on the device: one warp per image.  transforms: host array (it travels as a kernel
+ * argument).  key_dev: int64 [2], the key's words are their low 32 bits.  descs_dev: src_h, src_w read, n_ops, ops,
+ * out_h and out_w written as the host sampler fills them.  Image i's boxes (fp32 [n, 4] xyxy) and labels (int64) are
+ * rows [box_start[i], box_start[i + 1]) of boxes_dev / labels_dev; its kept boxes go to the same rows of boxes_out_dev
+ * / labels_out_dev in order, their number to counts_dev[i], YB_AUG_ST_* bits to status_dev[i].  The box pointers may
+ * be null when the batch has no boxes.  No host synchronisation, no float atomics: a repeated call writes the same
+ * bits.  Argument errors return YB_ERR_INVALID before the device is touched. */
+int yb_augment_sample(int n_images, const yb_aug_sampler* transforms, int n_transforms, const int64_t* key_dev,
+                      yb_aug_image* descs_dev, const float* boxes_dev, const int64_t* labels_dev,
+                      const int32_t* box_start_dev, float* boxes_out_dev, int64_t* labels_out_dev, int32_t* counts_dev,
+                      int32_t* status_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,6 +5,9 @@ Reports CUDA-event times (median of --iters after warm-up) of
   kernels    the augmentation launches alone, on parameters drawn beforehand
   augment    Compose.apply_batch: host draws + descriptor copy + launches
   step       apply_batch + YOLOTransform(images, targets)
+  sampler    the device sampler's kernel alone (augment_sample_kernel, from a torch.profiler pass of its own)
+  sampled    Compose.apply_batch(..., generator=g): key draw + copies + sampler + read-back + pixel launches
+  sampled step  the same + YOLOTransform(images, targets)
 with the bytes each moves (source read once per pass that reads it, output written once) and the fraction of the
 H100's 3.35 TB/s that is.  For context it times the same torchvision tensor ops the reference runs, on the CPU, image
 by image, on the same recipes.  The card's name and power limit are printed in the same run.
@@ -92,6 +95,20 @@ def events(fn, iters):
     return statistics.median(times)
 
 
+def sampler_kernel_us(fn, iters):
+    """Median device time of augment_sample_kernel over `iters` calls of `fn`, from a profiler pass of its own."""
+    from torch.profiler import ProfilerActivity, profile
+
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for i in range(iters):
+            fn(i)
+        torch.cuda.synchronize()
+    times = [e.time_range.elapsed_us() for e in prof.events() if "augment_sample_kernel" in e.name]
+    if not times:
+        raise SystemExit("the profiler recorded no augment_sample_kernel launch")
+    return statistics.median(times)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=32)
@@ -127,8 +144,20 @@ def main():
         outs, tg = pipe.apply_batch(images, targets)
         lb(outs, tg)
 
+    g = torch.Generator(dev)
+
+    def sampled(i):
+        g.manual_seed(i)
+        pipe.apply_batch(images, targets, generator=g)
+
+    def sampled_step(i):
+        g.manual_seed(i)
+        outs, tg = pipe.apply_batch(images, targets, generator=g)
+        lb(outs, tg)
+
     results = {}
-    for name, fn in (("kernels", kernels), ("augment", augment), ("step", step)):
+    for name, fn in (("kernels", kernels), ("augment", augment), ("step", step), ("sampled", sampled),
+                     ("sampled step", sampled_step)):
         for i in range(args.warmup):
             fn(i)
         torch.cuda.synchronize()
@@ -141,6 +170,9 @@ def main():
           f"{nbytes / (results['kernels'] * 1e-3) / 1e9:.0f} GB/s = {nbytes / (results['kernels'] * 1e-3) / HBM:.1%} of HBM")
     print(f"  augment  {results['augment']:.3f} ms (host draws + copy + launches)")
     print(f"  step     {results['step']:.3f} ms  {lb_bytes / 1e6:.1f} MB with the letterbox")
+    print(f"  sampler  {sampler_kernel_us(sampled, args.iters):.1f} us (augment_sample_kernel alone, median)")
+    print(f"  sampled  {results['sampled']:.3f} ms (device sampler + read-back + launches)")
+    print(f"  sampled step  {results['sampled step']:.3f} ms")
     torch.set_num_threads(os.cpu_count() or 1)
     t0 = time.perf_counter()
     for it in range(args.cpu_iters):

@@ -6,6 +6,7 @@ library is missing, or a wrapper is asked to run without a CUDA device, it raise
 """
 import ctypes
 import itertools
+import math
 import os
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -60,6 +61,7 @@ EXPORTED_SYMBOLS = (
     "yb_yolo_loss_backward",
     "yb_augment_prepare",
     "yb_augment",
+    "yb_augment_sample",
     "yb_conv_wgrad_workspace_bytes",
     "yb_conv_wgrad_config",
     "yb_conv_wgrad",
@@ -227,6 +229,21 @@ class AugImage(ctypes.Structure):
         ("out_block_start", ctypes.c_int32), ("mean_block_start", ctypes.c_int32 * YB_AUG_MAX_CONTRAST),
         ("reserved", ctypes.c_int32), ("ops", AugOp * YB_AUG_MAX_OPS),
     ]
+
+
+YB_AUG_MAX_TRANSFORMS, YB_AUG_MAX_OPTIONS, YB_AUG_CROP_ROUNDS = 16, 16, 1024
+YB_AUG_S_NONE, YB_AUG_S_PHOTOMETRIC, YB_AUG_S_ZOOM_OUT, YB_AUG_S_IOU_CROP, YB_AUG_S_HFLIP = range(5)
+YB_AUG_ST_CROP_ROUNDS = 1
+
+
+class AugSampler(ctypes.Structure):
+    """yb_aug_sampler: one transform of the device parameter sampler (include/yolort_b200.h)."""
+    _fields_ = [
+        ("kind", ctypes.c_int32), ("jitter", ctypes.c_int32), ("trials", ctypes.c_int32), ("n_options", ctypes.c_int32),
+        ("fill", ctypes.c_uint32), ("p", ctypes.c_float), ("lo", ctypes.c_float * 4), ("span", ctypes.c_float * 4),
+        ("min_aspect", ctypes.c_double), ("max_aspect", ctypes.c_double),
+        ("options", ctypes.c_double * YB_AUG_MAX_OPTIONS),
+    ]
 YB_LOSS_MATCH_INT32 = 24
 YB_WGRAD_MAX_PROBLEMS = 8
 
@@ -328,6 +345,7 @@ def lib() -> ctypes.CDLL:
     L.yb_augment_prepare.argtypes = [ctypes.c_int, ctypes.POINTER(AugImage), ctypes.POINTER(ctypes.c_int64)]
     L.yb_augment.argtypes = [ctypes.c_int, ctypes.POINTER(AugImage), ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
                              ctypes.c_void_p, ctypes.c_void_p]
+    L.yb_augment_sample.argtypes = [ctypes.c_int, ctypes.POINTER(AugSampler), ctypes.c_int] + [ctypes.c_void_p] * 10
     L.yb_conv_wgrad_workspace_bytes.restype = ctypes.c_size_t
     L.yb_conv_wgrad_workspace_bytes.argtypes = [ctypes.POINTER(WgradProblem), ctypes.c_int]
     L.yb_conv_wgrad_config.argtypes = [ctypes.POINTER(WgradProblem), ctypes.c_int, ctypes.POINTER(ctypes.c_int32)]
@@ -972,6 +990,64 @@ def augment(descs, out: torch.Tensor, sources: Sequence[torch.Tensor]) -> torch.
                 seen.add(key)
                 im.record_stream(stream)
     return out
+
+
+def augment_sample(samplers, sources: Sequence[torch.Tensor], key: torch.Tensor, boxes: Sequence[torch.Tensor],
+                   labels: Sequence[torch.Tensor], boxes_to_host: bool):
+    """Draws the recipes of the images `sources` on the device (yb_augment_sample) with the transforms `samplers`
+    (AugSampler array) and `key` (int64 [2] on the sources' device).  boxes / labels: fp32 [n, 4] / int64 [n] per image;
+    when all are on the host they cross in the one host-to-device copy that also carries the descriptors.
+
+    Returns (descs, counts, status, boxes, labels): the AugImage array (src pointers, sizes and recipes set), lists of
+    the kept-box counts and YB_AUG_ST_* bits per image, and the batch's boxes [N, 4] / labels [N], image i's kept ones
+    first in its input rows; on the host when `boxes_to_host`, else views into a device buffer.  The read-back of the
+    descriptors, counts and status (and boxes) is the one host synchronisation."""
+    n, dev = len(sources), key.device
+    nb = sum(int(b.shape[0]) for b in boxes)
+    descs = (AugImage * n)()
+    for d, im in zip(descs, sources):
+        d.src = im.data_ptr()
+        d.stride_c, d.stride_y, d.stride_x = (int(v) for v in im.stride())
+        d.src_h, d.src_w = int(im.shape[1]), int(im.shape[2])
+    # one device buffer: the inputs (uploaded in one copy), then the outputs (read back in one copy)
+    layout = {"start": (torch.int32, (n + 1,)), "boxes": (torch.float32, (nb, 4)), "labels": (torch.int64, (nb,)),
+              "descs": (torch.uint8, (ctypes.sizeof(descs),)), "counts": (torch.int32, (n,)),
+              "status": (torch.int32, (n,)), "boxes_out": (torch.float32, (nb, 4)), "labels_out": (torch.int64, (nb,))}
+    off, end = {}, 0
+    for name, (dtype, shape) in layout.items():
+        off[name] = end
+        end += -(-math.prod(shape) * dtype.itemsize // 16) * 16
+
+    def part(t, name, base=0):
+        dtype, shape = layout[name]
+        o = off[name] - base
+        return t[o: o + math.prod(shape) * dtype.itemsize].view(dtype).view(shape)
+
+    stage = torch.empty((off["counts"],), dtype=torch.uint8, pin_memory=True)
+    part(stage, "start").copy_(torch.tensor([0] + list(itertools.accumulate(int(b.shape[0]) for b in boxes)),
+                                            dtype=torch.int32))
+    on_host = all(t.device.type == "cpu" for t in list(boxes) + list(labels))
+    if nb and on_host:
+        torch.cat(list(boxes), out=part(stage, "boxes"))
+        torch.cat(list(labels), out=part(stage, "labels"))
+    ctypes.memmove(stage.data_ptr() + off["descs"], ctypes.addressof(descs), ctypes.sizeof(descs))
+    with device_guard(dev):
+        buf = torch.empty((end,), dtype=torch.uint8, device=dev)
+        buf[: off["counts"]].copy_(stage, non_blocking=True)
+        if nb and not on_host:
+            torch.cat([b.to(dev) for b in boxes], out=part(buf, "boxes"))
+            torch.cat([l.to(dev) for l in labels], out=part(buf, "labels"))
+        p = buf.data_ptr()
+        ptr = {k: p + off[k] if nb or k not in ("boxes", "labels", "boxes_out", "labels_out") else None for k in off}
+        check(lib().yb_augment_sample(n, samplers, len(samplers), key.data_ptr(), ptr["descs"], ptr["boxes"],
+                                      ptr["labels"], ptr["start"], ptr["boxes_out"], ptr["labels_out"], ptr["counts"],
+                                      ptr["status"], current_stream_ptr(dev)), "yb_augment_sample")
+        host = buf[off["descs"]: end if boxes_to_host else off["boxes_out"]].cpu()
+    base = off["descs"]
+    descs = (AugImage * n).from_buffer_copy(host[: ctypes.sizeof(descs)].numpy())
+    src, src_base = (host, base) if boxes_to_host else (buf, 0)
+    return (descs, part(host, "counts", base).tolist(), part(host, "status", base).tolist(),
+            part(src, "boxes_out", src_base), part(src, "labels_out", src_base))
 
 
 # ---------------------------------------------------------------------------------------------------

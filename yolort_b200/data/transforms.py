@@ -21,6 +21,11 @@ How it runs:
 Differences from the reference: a PIL image raises TypeError, a non-uint8 or non-3-D image ValueError, a CPU image
 NativeLibraryError (there is no CPU path); targets with "masks" or "keypoints" raise NotImplementedError.  The
 caller's target tensors are not modified in place (the reference's zoom-out and flip write into them).
+
+`Compose.apply_batch(images, targets, generator=g)` with a CUDA `torch.Generator` draws the parameters on the device
+instead (`csrc/augment_sample.cu`): the reference's transforms, parameter distributions and acceptance rules on a
+Philox4x32-10 stream keyed by one draw from `g`, so `g.manual_seed(s)` reproduces a batch.  It does not reproduce the
+reference's random numbers and does not touch torch's default generator; oracle/sample_augment.py restates its rules.
 """
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -70,6 +75,11 @@ class _Transform(nn.Module):
     def _draw(self, st: _State) -> None:
         raise NotImplementedError
 
+    def _sampler(self, s: "_C.AugSampler") -> Tuple[int, int]:
+        """Describes the transform to the device sampler in `s`; returns the most ops and contrast ops it can add to
+        a recipe."""
+        raise TypeError(f"{type(self).__name__} has no device sampler")
+
     def forward(self, image: Tensor, target: Optional[Dict[str, Tensor]] = None):
         return Compose([self])(image, target)
 
@@ -83,10 +93,7 @@ class Compose:
         return images[0], targets[0]
 
     # -- host side: parameters, boxes and recipes (no device work) -----------------------------------------------
-    def plan(self, sizes: Sequence[Tuple[int, int]], targets: Sequence[Optional[Dict[str, Tensor]]]):
-        """Draws every image's parameters in turn (image 0's transforms, then image 1's, ...: what calling the
-        reference Compose image by image draws) and applies them to host copies of the targets.  Returns the states:
-        output size, recipe and target of each image."""
+    def _check_transforms(self) -> None:
         for i, t in enumerate(self.transforms):
             if not isinstance(t, _Transform):
                 raise TypeError(f"Compose: transform {i} ({type(t).__name__}) is not one of "
@@ -94,6 +101,12 @@ class Compose:
             if isinstance(t, ConvertImageDtype) and t.dtype != torch.uint8 and i != len(self.transforms) - 1:
                 raise NotImplementedError("ConvertImageDtype(float) / ToTensor must be the last transform: the "
                                           "recipes compute on uint8 images")
+
+    def plan(self, sizes: Sequence[Tuple[int, int]], targets: Sequence[Optional[Dict[str, Tensor]]]):
+        """Draws every image's parameters in turn (image 0's transforms, then image 1's, ...: what calling the
+        reference Compose image by image draws) and applies them to host copies of the targets.  Returns the states:
+        output size, recipe and target of each image."""
+        self._check_transforms()
         states = []
         for hw, tg in zip(sizes, targets):
             st = _State(hw, tg)
@@ -103,15 +116,22 @@ class Compose:
         return states
 
     # -- the batch -------------------------------------------------------------------------------------------
-    def apply_batch(self, images: Sequence[Tensor], targets: Optional[Sequence[Optional[Dict[str, Tensor]]]] = None):
+    def apply_batch(self, images: Sequence[Tensor], targets: Optional[Sequence[Optional[Dict[str, Tensor]]]] = None,
+                    generator: Optional[torch.Generator] = None):
         """Augments a batch: the parameters of every image are drawn as `plan` does, then all pixels are computed
-        at once.  Returns (images, targets); the images are views into one device buffer."""
+        at once.  Returns (images, targets); the images are views into one device buffer.
+
+        With `generator` (a CUDA torch.Generator on the images' device) the parameters are drawn on the device from
+        one 64-bit key taken from it (see `sample`); torch's default generator is not used."""
         images = list(images)
         if not images:
             return [], []
         targets = [None] * len(images) if targets is None else list(targets)
         if len(targets) != len(images):
             raise ValueError(f"{len(images)} images and {len(targets)} targets")
+        if generator is not None:
+            descs, out_targets = self.sample(images, targets, generator)
+            return _run_descs(images, descs, self._float_out()), out_targets
         for im in images:
             _check_image(im)
         dev = images[0].device
@@ -122,19 +142,121 @@ class Compose:
         states = self.plan([(int(im.shape[1]), int(im.shape[2])) for im in images], host_targets)
         return run_recipes(images, states), _device_targets(states, targets, target_dev)
 
+    # -- the device sampler ----------------------------------------------------------------------------------
+    def _float_out(self) -> bool:
+        float_out = False
+        for t in self.transforms:
+            if isinstance(t, ConvertImageDtype):
+                float_out = t.dtype == torch.float32
+        return float_out
+
+    def _sampler_table(self) -> "ctypes.Array":
+        """The transforms as yb_aug_sampler entries.  Raises what `plan` raises for a transform list it cannot run,
+        TypeError for a transform without a device sampler and NotImplementedError when some recipe could exceed the
+        descriptor's YB_AUG_MAX_OPS ops or YB_AUG_MAX_CONTRAST contrast ops (a bound from the list, not the draws)."""
+        self._check_transforms()
+        if len(self.transforms) > _C.YB_AUG_MAX_TRANSFORMS:
+            raise NotImplementedError(f"{len(self.transforms)} transforms (the device sampler takes at most "
+                                      f"{_C.YB_AUG_MAX_TRANSFORMS})")
+        table = (_C.AugSampler * len(self.transforms))()
+        ops = contrast = 0
+        for s, t in zip(table, self.transforms):
+            o, c = t._sampler(s)
+            ops, contrast = ops + o, contrast + c
+        if ops > _C.YB_AUG_MAX_OPS or contrast > _C.YB_AUG_MAX_CONTRAST:
+            raise NotImplementedError(f"the transforms can draw a recipe of {ops} ops with {contrast} contrast ops (at "
+                                      f"most {_C.YB_AUG_MAX_OPS} and {_C.YB_AUG_MAX_CONTRAST})")
+        return table
+
+    def sample(self, images: Sequence[Tensor], targets: Sequence[Optional[Dict[str, Tensor]]],
+               generator: torch.Generator):
+        """Draws every image's parameters on the device and carries its boxes through them; no pixel is computed.
+        Returns (descriptors, targets): the yb_aug_image recipes `apply_batch` computes the pixels from, and each
+        target with its kept boxes and labels on the device it came from (other keys pass through).  Every input
+        error is raised before anything is drawn; the read-back of the descriptors is the one host synchronisation."""
+        table = self._sampler_table()
+        need_target = any(isinstance(t, RandomIoUCrop) for t in self.transforms)
+        boxes, labels = _sampled_boxes(targets, need_target)
+        _check_generator(generator)
+        for im in images:
+            _check_image(im)
+        dev = images[0].device
+        if any(im.device != dev for im in images):
+            raise ValueError("apply_batch: every image must be on the same device")
+        _check_generator(generator, dev)
+        to_host = any(t is not None and t["boxes"].device.type == "cpu" for t in targets)
+        descs, counts, status, out_boxes, out_labels = _C.augment_sample(table, images, _draw_key(generator, dev),
+                                                                        boxes, labels, to_host)
+        failed = [i for i, s in enumerate(status) if s & _C.YB_AUG_ST_CROP_ROUNDS]
+        if failed:
+            raise RuntimeError(f"RandomIoUCrop accepted no window in {_C.YB_AUG_CROP_ROUNDS} rounds for image(s) "
+                               f"{failed}: no box centre lies inside any window its options allow")
+        out, row = [], 0
+        for t, b, l, c in zip(targets, boxes, labels, counts):
+            if t is not None:
+                t = dict(t)
+                t["boxes"] = out_boxes[row: row + c].to(b.device)
+                t["labels"] = out_labels[row: row + c].to(l.device)
+            row += int(b.shape[0])
+            out.append(t)
+        return descs, out
+
+
+def _check_generator(generator, dev: Optional[torch.device] = None) -> None:
+    if not isinstance(generator, torch.Generator) or generator.device.type != "cuda":
+        got = generator.device if isinstance(generator, torch.Generator) else type(generator).__name__
+        raise ValueError(f"generator must be a CUDA torch.Generator on the images' device, got {got}")
+    idx = lambda d: torch.cuda.current_device() if d.index is None else d.index  # noqa: E731
+    if dev is not None and idx(generator.device) != idx(dev):
+        raise ValueError(f"generator is on {generator.device}, the images on {dev}")
+
+
+def _draw_key(generator: torch.Generator, dev: torch.device) -> Tensor:
+    """The call's Philox key: two 32-bit words drawn by a device op, so the host never reads the generator's state."""
+    return torch.empty(2, dtype=torch.int64, device=dev).random_(0, 1 << 32, generator=generator)
+
+
+def _sampled_boxes(targets, need_target: bool):
+    """The boxes and labels of each image, checked for the device sampler (none for an image without a target)."""
+    boxes, labels = [], []
+    for i, t in enumerate(targets):
+        if t is None:
+            if need_target:
+                raise ValueError(f"image {i} has no target: RandomIoUCrop needs one")
+            boxes.append(torch.zeros((0, 4), dtype=torch.float32))
+            labels.append(torch.zeros((0,), dtype=torch.int64))
+            continue
+        for key in ("masks", "keypoints"):
+            if key in t:
+                raise NotImplementedError(f"targets with {key!r} are not supported by the GPU augmentations")
+        if "boxes" not in t or "labels" not in t:
+            raise ValueError("a target must hold 'boxes' and 'labels'")
+        b, l = t["boxes"], t["labels"]
+        if not (isinstance(b, Tensor) and b.dtype == torch.float32 and b.dim() == 2 and b.shape[1] == 4):
+            raise ValueError(f"image {i}: boxes must be a float32 [n, 4] tensor")
+        if not (isinstance(l, Tensor) and l.dtype == torch.int64 and l.shape == (b.shape[0],)):
+            raise ValueError(f"image {i}: labels must be an int64 [n] tensor with one label per box")
+        boxes.append(b)
+        labels.append(l)
+    return boxes, labels
+
 
 def run_recipes(images: Sequence[Tensor], states: Sequence["_State"]) -> List[Tensor]:
     """Computes the planned images (one launch, plus one per contrast round); the outputs are views into one buffer."""
     descs = (_C.AugImage * len(images))()
-    total = 0
     for d, im, st in zip(descs, images, states):
         _fill_desc(d, im, st)
+    return _run_descs(images, descs, states[0].float_out)
+
+
+def _run_descs(images: Sequence[Tensor], descs, float_out: bool) -> List[Tensor]:
+    total = 0
+    for d in descs:
         d.out_offset = total
-        total += -(-3 * st.h * st.w // 16) * 16        # every image starts 64-byte aligned
-    dtype = torch.float32 if states[0].float_out else torch.uint8
-    out = torch.empty((total,), dtype=dtype, device=images[0].device)
+        total += -(-3 * d.out_h * d.out_w // 16) * 16     # every image starts 64-byte aligned
+    out = torch.empty((total,), dtype=torch.float32 if float_out else torch.uint8, device=images[0].device)
     _C.augment(descs, out, images)
-    return [out[d.out_offset: d.out_offset + 3 * st.h * st.w].view(3, st.h, st.w) for d, st in zip(descs, states)]
+    return [out[d.out_offset: d.out_offset + 3 * d.out_h * d.out_w].view(3, d.out_h, d.out_w) for d in descs]
 
 
 def _check_image(im) -> None:
@@ -231,12 +353,20 @@ class RandomHorizontalFlip(_Transform):
                 b[:, [0, 2]] = st.w - b[:, [2, 0]]
                 st.target["boxes"] = b
 
+    def _sampler(self, s) -> Tuple[int, int]:
+        s.kind, s.p = _C.YB_AUG_S_HFLIP, self.p
+        return 1, 0
+
 
 class PILToTensor(_Transform):
     """The identity on a uint8 tensor image."""
 
     def _draw(self, st: _State) -> None:
         pass
+
+    def _sampler(self, s) -> Tuple[int, int]:
+        s.kind = _C.YB_AUG_S_NONE
+        return 0, 0
 
 
 class ConvertImageDtype(_Transform):
@@ -248,6 +378,10 @@ class ConvertImageDtype(_Transform):
 
     def _draw(self, st: _State) -> None:
         st.float_out = self.dtype == torch.float32
+
+    def _sampler(self, s) -> Tuple[int, int]:
+        s.kind = _C.YB_AUG_S_NONE
+        return 0, 0
 
 
 class ToTensor(ConvertImageDtype):
@@ -313,6 +447,17 @@ class RandomIoUCrop(_Transform):
                 st.h, st.w = new_h, new_w
                 return
 
+    def _sampler(self, s) -> Tuple[int, int]:
+        if not 0 < len(self.options) <= _C.YB_AUG_MAX_OPTIONS:
+            raise NotImplementedError(f"RandomIoUCrop with {len(self.options)} sampler options (the device sampler "
+                                      f"takes 1 to {_C.YB_AUG_MAX_OPTIONS})")
+        s.kind, s.trials, s.n_options = _C.YB_AUG_S_IOU_CROP, int(self.trials), len(self.options)
+        s.lo[0], s.span[0] = self.min_scale, self.max_scale - self.min_scale
+        s.min_aspect, s.max_aspect = self.min_aspect_ratio, self.max_aspect_ratio
+        for j, o in enumerate(self.options):
+            s.options[j] = o
+        return 1, 0
+
 
 class RandomZoomOut(_Transform):
     def __init__(self, fill: Optional[List[float]] = None, side_range: Tuple[float, float] = (1.0, 4.0), p: float = 0.5):
@@ -334,9 +479,7 @@ class RandomZoomOut(_Transform):
         r = torch.rand(2)
         left = int((canvas_width - orig_w) * r[0])
         top = int((canvas_height - orig_h) * r[1])
-        # the reference overwrites the border with torch.tensor(fill, dtype=uint8)
-        f = torch.tensor(self.fill, dtype=torch.uint8).expand(3).tolist()
-        packed = f[0] | (f[1] << 8) | (f[2] << 16)
+        packed = self._packed_fill()
         st.ops.append((_C.YB_AUG_ZOOM_OUT, (top, left, orig_h, orig_w, canvas_height, canvas_width, packed), None))
         st.h, st.w = canvas_height, canvas_width
         if st.target is not None:
@@ -344,6 +487,16 @@ class RandomZoomOut(_Transform):
             b[:, 0::2] += left
             b[:, 1::2] += top
             st.target["boxes"] = b
+
+    def _packed_fill(self) -> int:
+        # the reference overwrites the border with torch.tensor(fill, dtype=uint8)
+        f = torch.tensor(self.fill, dtype=torch.uint8).expand(3).tolist()
+        return f[0] | (f[1] << 8) | (f[2] << 16)
+
+    def _sampler(self, s) -> Tuple[int, int]:
+        s.kind, s.p, s.fill = _C.YB_AUG_S_ZOOM_OUT, self.p, self._packed_fill()
+        s.lo[0], s.span[0] = self.side_range[0], self.side_range[1] - self.side_range[0]
+        return 1, 0
 
 
 class RandomPhotometricDistort(_Transform):
@@ -381,6 +534,14 @@ class RandomPhotometricDistort(_Transform):
             self._jitter(st, _C.YB_AUG_CONTRAST, self.contrast)
         if r[6] < self.p:
             st.ops.append((_C.YB_AUG_PERMUTE, tuple(torch.randperm(3).tolist()), None))
+
+    def _sampler(self, s) -> Tuple[int, int]:
+        s.kind, s.p = _C.YB_AUG_S_PHOTOMETRIC, self.p
+        for j, rng in enumerate((self.brightness, self.contrast, self.saturation, self.hue)):
+            if rng is not None:
+                s.jitter |= 1 << j
+                s.lo[j], s.span[j] = rng[0], rng[1] - rng[0]
+        return bin(s.jitter).count("1") + 1, int(self.contrast is not None)
 
 
 def _jitter_range(value, center: float):
