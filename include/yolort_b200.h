@@ -192,15 +192,16 @@ typedef struct {
  * Channel counts, channel offsets and cstrides of e4m3 views are multiples of 16 (16 bytes), like every 16-byte view.
  * YB_OP_CONV with dtype YB_F8E4M3 (the FP8 implicit-GEMM kernel) reads the fields as follows:
  *   in, residual:  e4m3 NHWC views (scales s_in, s_res); Cin, in_cstride and res_cstride multiples of 16
- *   out:       an e4m3 NHWC view (scale s_out), Cout and out_cstride multiples of 16; or, with reserved bit 4 (bit 5), an
- *              fp16 (bf16) NHWC view, Cout and out_cstride multiples of 8, that gets the dequantised values (head logits)
+ *   out:       an e4m3 NHWC view (scale s_out), Cout and out_cstride multiples of 16; or, with YB_CONV_E4M3_F16_OUT
+ *              (YB_CONV_E4M3_BF16_OUT), an fp16 (bf16) NHWC view, Cout and out_cstride multiples of 8, that gets the
+ *              dequantised values (head logits)
  *   ksize, stride, pad:  1x1/s1/p0, 3x3/s1/p1 or 3x3/s2/p1
  *   act:       YB_ACT_NONE, SILU, HARDSWISH, LEAKY01 or RELU
  *   weight:    e4m3 [Cout_pad][ksize*ksize][Cin_pad], Cin_pad a multiple of 32 (the K step), zero padded; row c holds
  *              w[c] / s_w[c]
  *   bias:      fp32 [Cout_pad] bias, then fp32 [Cout_pad] multipliers m[c] = s_w[c] * s_in, then {s_res, 1/s_out}
- *   reserved:  bit 4: fp16 output, bit 5: bf16 output, every other bit zero; decode and chain must be NULL; a residual
- *              needs the e4m3 output.
+ *   reserved:  YB_CONV_E4M3_F16_OUT or YB_CONV_E4M3_BF16_OUT, every other bit zero; decode and chain must be NULL;
+ *              a residual needs the e4m3 output.
  *   v = act(acc * m[c] + bias[c]) [+ res * s_res] with the e4m3 dot product acc accumulated in fp32, then
  *   out = RN_satfinite(v * (1/s_out)) (e4m3) or RN(v) (fp16 / bf16).
  * YB_OP_QUANTIZE: dtype is the SOURCE type (YB_F16 or YB_BF16); in is that NHWC view, out an e4m3 NHWC view of the
@@ -226,16 +227,22 @@ typedef struct {
   const float* bias;            /* [Cout_pad] fp32 (folded BN shift, or the head's conv bias)     */
   const void* residual;         /* optional NHWC view added after the activation (Bottleneck)    */
   int32_t res_cstride;
-  int32_t reserved;             /* bit 0: keep a 3x3 conv on the generic im2col kernel; bit 1: `weight` is the banded
-                                   super-pixel stem matrix [Cout_pad][3][128] (engine.stem_band); bit 2: take the
-                                   halo-patch kernel's stride-2 parity-plane variant whatever the channel counts (tests);
-                                   bit 3: do not split N over CTAs with resident weights (A/B timing, tests);
-                                   bit 4: keep one CTA per SM where the shape would take two (tests compare the two
-                                   launches bit for bit); e4m3 convolutions: bits 4 / 5 only (see above), with their
-                                   own meaning; other bits: must be zero */
+  int32_t reserved;             /* option bits of a convolution (YB_CONV_* below); other bits: must be zero */
   const yb_head_decode* decode; /* optional (host pointer, copied at plan creation): fused decode epilogue */
   const yb_conv_chain* chain;   /* optional (host pointer, copied at plan creation): chained pointwise tail  */
 } yb_op_desc;
+
+/* yb_op_desc.reserved option bits of an fp16 / bf16 YB_OP_CONV: */
+#define YB_CONV_FORCE_IM2COL 1   /* keep a 3x3 conv on the generic im2col kernel */
+#define YB_CONV_BAND_STEM 2      /* `weight` is the banded super-pixel stem matrix [Cout_pad][3][128] (engine.stem_band) */
+#define YB_CONV_FORCE_PLANES 4   /* take the halo-patch kernel's stride-2 parity-plane variant whatever the channel
+                                    counts (tests) */
+#define YB_CONV_NO_NSPLIT 8      /* do not split N over CTAs with resident weights (A/B timing, tests) */
+#define YB_CONV_ONE_CTA 16       /* keep one CTA per SM where the shape would take two (tests compare the two launches
+                                    bit for bit) */
+/* ... and of an e4m3 YB_OP_CONV (see above), which takes these two only: */
+#define YB_CONV_E4M3_F16_OUT 16  /* fp16 output */
+#define YB_CONV_E4M3_BF16_OUT 32 /* bf16 output */
 
 /* 1 if `op` (a YB_OP_CONV with op->chain set) can run as one fused launch on this build, else 0 (the caller then
  * emits the two convolutions separately).  Pure host logic: no GPU needed. */

@@ -22,7 +22,6 @@ from yolort_b200.engine import pack_bias, pack_weight
 F16, BF16 = torch.float16, torch.bfloat16
 NONE, SILU, HSWISH, LEAKY, RELU = (_C.YB_ACT_NONE, _C.YB_ACT_SILU, _C.YB_ACT_HARDSWISH, _C.YB_ACT_LEAKY01,
                                    _C.YB_ACT_RELU)
-FORCE_IM2COL, FORCE_PLANES, KEEP_ONE_CTA = 1, 4, 16       # yb_op_desc.reserved bits 0, 2 and 4
 SENTINEL = 7.0
 SMS = torch.cuda.get_device_properties(0).multi_processor_count if torch.cuda.is_available() else 132
 TILE_M = 128                                              # output rows per tile (both kernels)
@@ -239,12 +238,12 @@ def _cases():
             Case(f"{b} 1x1 Cout72 leaky", 2, 16, 20, 80, 72, dtype=dt, act=LEAKY, seed=4, bias_scale=1.0,
                  out_cstride=96, out_off=8),
             Case(f"{b} 1x1 Cout200 none", 1, 20, 24, 64, 200, dtype=dt, act=NONE, seed=5),
-            Case(f"{b} im2col 3x3 s1 128 resid-window", 2, 20, 20, 128, 128, k=3, dtype=dt, reserved=FORCE_IM2COL,
-                 residual=True, res_cstride=256, res_off=64, seed=6),
+            Case(f"{b} im2col 3x3 s1 128 resid-window", 2, 20, 20, 128, 128, k=3, dtype=dt,
+                 reserved=_C.YB_CONV_FORCE_IM2COL, residual=True, res_cstride=256, res_off=64, seed=6),
             Case(f"{b} im2col 3x3 s2 streamed", 1, 24, 16, 256, 128, k=3, s=2, dtype=dt, seed=7, act=HSWISH,
                  bias_scale=2.0),
-            Case(f"{b} im2col 3x3 s1 resident hswish", 2, 18, 22, 32, 64, k=3, dtype=dt, reserved=FORCE_IM2COL,
-                 act=HSWISH, bias_scale=2.0, seed=42),
+            Case(f"{b} im2col 3x3 s1 resident hswish", 2, 18, 22, 32, 64, k=3, dtype=dt,
+                 reserved=_C.YB_CONV_FORCE_IM2COL, act=HSWISH, bias_scale=2.0, seed=42),
             Case(f"{b} im2col 5x5 Cin48", 2, 14, 18, 48, 64, k=5, dtype=dt, seed=8),
             Case(f"{b} 1x1 K1024 streamed 2 N tiles", 1, 16, 16, 1024, 512, dtype=dt, seed=9),
             # ---- 1x1 kernel at 2 x SMs tiles and more: N = 256 without decode, one and two CTAs ----
@@ -255,7 +254,7 @@ def _cases():
                  residual=True, res_cstride=64, res_off=32),
             Case(f"{b} 1cta 1x1 Cout32 at 2xSMs-1", 1, 2 * S - 1, 128, 64, 32, dtype=dt, seed=14),
             Case(f"{b} 2cta im2col 3x3 s2 Cout64 leaky", 4, 2 * 96, 2 * 96, 32, 64, k=3, s=2, dtype=dt,
-                 reserved=FORCE_IM2COL, act=LEAKY, seed=15, bias_scale=2.0),
+                 reserved=_C.YB_CONV_FORCE_IM2COL, act=LEAKY, seed=15, bias_scale=2.0),
             Case(f"{b} 2cta 1x1 Cout64 in-window", 5, 57, S + 1, 64, 64, dtype=dt, in_cstride=128, in_off=64,
                  out_cstride=128, out_off=64, seed=16, bias_scale=6.0),
             # ---- 1x1 kernel with chained tails ----
@@ -267,7 +266,7 @@ def _cases():
             Case(f"{b} chain 1x1 128->[64]->64 resid", 2, 24, 20, 64, 128, dtype=dt, chain=Chain(64, 64),
                  residual=True, seed=21),
             Case(f"{b} chain im2col 3x3 128->[128]->128", 1, 20, 24, 64, 128, k=3, dtype=dt,
-                 reserved=FORCE_IM2COL, chain=Chain(128, 120, store_first=False), seed=22),
+                 reserved=_C.YB_CONV_FORCE_IM2COL, chain=Chain(128, 120, store_first=False), seed=22),
             Case(f"{b} 2cta chain 1x1 64->[32]->32", 2, 128, S, 64, 64, dtype=dt, chain=Chain(32, 32), seed=23,
                  bias_scale=6.0),
             Case(f"{b} 2cta chain 1x1 64->[64]->64 ragged", 3, 97, S - 1, 32, 64, dtype=dt,
@@ -479,7 +478,7 @@ def check_case(case: Case, device=torch.device("cuda:0"), legacy_tol=None) -> di
 
     # ---- two CTAs per SM: the bits of the one-CTA launch ----
     if cfg["ctas_per_sm"] == 2:
-        one = dataclasses.replace(stored, reserved=stored.reserved | KEEP_ONE_CTA)
+        one = dataclasses.replace(stored, reserved=stored.reserved | _C.YB_CONV_ONE_CTA)
         d1, _c1 = build_desc(one, fake_ptr)
         assert _C.conv_config(d1)["ctas_per_sm"] == 1
         o1, o21 = _launch(one, t, device)

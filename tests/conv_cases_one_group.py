@@ -6,7 +6,8 @@ layout takes layers whose one-CTA plan has a 256-column N tile, as two 128-colum
 The cases use the Case / build_desc / check_case machinery of tests/conv_cases.py.  Every case is sized from the
 device's SM count so that it lands on the side of the planner's rule its name states.
 """
-from conv_cases import BF16, F16, FORCE_IM2COL, LEAKY, NONE, RELU, SMS, Case, mma_n
+from conv_cases import BF16, F16, LEAKY, NONE, RELU, SMS, Case, mma_n
+from yolort_b200 import _C
 
 ROWS = 128                                                # rows of the one-CTA tile the threshold counts
 
@@ -53,7 +54,7 @@ def _cases():
             Case(f"{b} 2x1 1x1 96->200 ragged resid-window", 4, 103, S - 7, 96, 200, dtype=dt, seed=104,
                  act=RELU, residual=True, res_cstride=256, res_off=40, out_cstride=232, out_off=24),
             Case(f"{b} 2x1 im2col 3x3 s2 32->256 ragged", 7, 2 * 61, 2 * (S - 3), 32, 256, k=3, s=2, dtype=dt,
-                 reserved=FORCE_IM2COL, seed=105, act=NONE, bias_scale=2.0),
+                 reserved=_C.YB_CONV_FORCE_IM2COL, seed=105, act=NONE, bias_scale=2.0),
             Case(f"{b} 1x2 1x1 512->256 streamed", 3, 128, S, 512, 256, dtype=dt, seed=106),
             Case(f"{b} 1x2 1x1 128->128", 3, 128, S, 128, 128, dtype=dt, seed=107),
         ]

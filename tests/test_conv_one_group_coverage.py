@@ -106,7 +106,7 @@ def test_keep_one_cta_bit_gives_the_two_group_layout():
         if cfg["layout"] != "2x1":
             continue
         d1, _ch = build_desc(c, fake_ptr)
-        d1.reserved |= conv_cases.KEEP_ONE_CTA
+        d1.reserved |= _C.YB_CONV_ONE_CTA
         one = _C.conv_config(d1)
         assert one["layout"] == "1x2" and one["epilogue_groups"] == 2 and one["grid"] <= og.SMS, (c.name, one)
         assert (cfg["block_n"], cfg["n_tiles"], one["block_n"], one["n_tiles"]) == (128, 2, 256, 1), (c.name, one)

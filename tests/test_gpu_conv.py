@@ -20,7 +20,8 @@ def run_conv(N, H, W, Cin, Cout, k, s, p, dtype=torch.float16, act=True, residua
     case = C.Case(f"conv N{N} {H}x{W} {Cin}->{Cout} k{k}s{s}", N, H, W, Cin, Cout, k=k, s=s, dtype=dtype, act=act_code,
                   residual=residual, in_cstride=Cin + in_pad, in_off=in_pad // 2 // 8 * 8, out_cstride=Cout + out_pad,
                   out_off=out_pad // 2 // 8 * 8, seed=seed, bias_scale=bias_scale,
-                  reserved=(C.FORCE_IM2COL if force_im2col else 0) | (C.FORCE_PLANES if force_planes else 0), **kw)
+                  reserved=((_C.YB_CONV_FORCE_IM2COL if force_im2col else 0) |
+                            (_C.YB_CONV_FORCE_PLANES if force_planes else 0)), **kw)
     return C.check_case(case, DEV, legacy_tol=_stagewise_tol(dtype))
 
 

@@ -1,6 +1,6 @@
 """Two CTAs per SM for the shallow convolution launches: which launches of the benchmark models take it (host logic,
-no GPU needed) and, on the H100, bit-identical outputs against the one-CTA launch of the same op (reserved bit 4) on the
-same input -- the per-tile arithmetic and summation order do not depend on how many CTAs share an SM."""
+no GPU needed) and, on the H100, bit-identical outputs against the one-CTA launch of the same op (YB_CONV_ONE_CTA) on
+the same input -- the per-tile arithmetic and summation order do not depend on how many CTAs share an SM."""
 import pytest
 import torch
 
@@ -8,7 +8,6 @@ import yolort_b200.models as M
 from yolort_b200 import _C, engine
 
 DEV = torch.device("cuda:0")
-KEEP_ONE_CTA = 16      # yb_op_desc.reserved bit 4
 
 # (constructor, batch, canvas, dtype, launches expected on two CTAs per SM): the benchmark configurations c2 (yolov5s),
 # c3 (yolov5m, global batch 128 on one GPU), c4 (yolov5l, the smallest and largest canvas of its mix), c5 (yolov5x),
@@ -56,7 +55,7 @@ def test_two_ctas_per_sm_where_the_shape_selects_it(monkeypatch, case):
             static = 1296 if cfg["patch_kernel"] else 2256         # the kernels' static shared memory (ptxas -v)
             assert cfg["grid"] == 2 * 132 and cfg["smem_bytes"] + static <= 228 * 1024 // 2 - 1024
             d1 = _C.OpDesc.from_buffer_copy(d)
-            d1.reserved |= KEEP_ONE_CTA
+            d1.reserved |= _C.YB_CONV_ONE_CTA
             one = _C.conv_config(d1)
             assert one["ctas_per_sm"] == 1 and one["grid"] == 132 and one["chained"] == cfg["chained"]
 
@@ -86,7 +85,7 @@ def test_two_cta_launches_match_one_cta_bit_for_bit(case):
         assert not torch.equal(got, before), plan.op_names[i]
         arena.copy_(before)
         d1 = _C.OpDesc.from_buffer_copy(plan._descs[i])
-        d1.reserved |= KEEP_ONE_CTA
+        d1.reserved |= _C.YB_CONV_ONE_CTA
         assert _ctas(d1) == 1
         one = _C.Plan([d1], DEV)
         one.run()

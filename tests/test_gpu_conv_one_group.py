@@ -61,7 +61,7 @@ def test_one_group_case(case):
     t["out0"] = t["out"].clone()
     stored = case if case.chain is None else dataclasses.replace(case, chain=dataclasses.replace(case.chain, store_first=True))
     out, out2 = conv_cases._launch(stored, t, DEV)
-    one = dataclasses.replace(stored, reserved=stored.reserved | conv_cases.KEEP_ONE_CTA)
+    one = dataclasses.replace(stored, reserved=stored.reserved | _C.YB_CONV_ONE_CTA)
     o1, o21 = conv_cases._launch(one, t, DEV)
     assert torch.equal(o1, out), "one-group launch differs from the one-CTA launch"
     if case.chain is not None:
@@ -95,7 +95,7 @@ def test_one_group_launches_match_one_cta_bit_for_bit(model):
         assert not torch.equal(got, before), plan.op_names[i]
         arena.copy_(before)
         d1 = _C.OpDesc.from_buffer_copy(plan._descs[i])
-        d1.reserved |= conv_cases.KEEP_ONE_CTA
+        d1.reserved |= _C.YB_CONV_ONE_CTA
         assert _layout(d1) == "1x2"
         one = _C.Plan([d1], DEV)
         one.run()

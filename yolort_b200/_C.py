@@ -21,6 +21,9 @@ YB_LAYOUT_NCHW, YB_LAYOUT_S2D16 = 0, 1
 YB_OP_CONV, YB_OP_SPP_POOL, YB_OP_UPSAMPLE2X, YB_OP_ATTENTION, YB_OP_DWCONV, YB_OP_SE, YB_OP_AVGPOOL = 0, 1, 2, 3, 4, 5, 6
 YB_OP_QUANTIZE = 7
 YB_ACT_NONE, YB_ACT_SILU, YB_ACT_HARDSWISH, YB_ACT_LEAKY01, YB_ACT_RELU = 0, 1, 2, 3, 4
+# yb_op_desc.reserved option bits of a convolution (fp16 / bf16; e4m3 convolutions take the last two only)
+YB_CONV_FORCE_IM2COL, YB_CONV_BAND_STEM, YB_CONV_FORCE_PLANES, YB_CONV_NO_NSPLIT, YB_CONV_ONE_CTA = 1, 2, 4, 8, 16
+YB_CONV_E4M3_F16_OUT, YB_CONV_E4M3_BF16_OUT = 16, 32
 YB_MAX_LEVELS, YB_MAX_ANCHORS = 4, 4
 NMS_TV_AUTO, NMS_EXACT_PER_CLASS, NMS_OFFSET_TRICK = 0, 1, 2
 

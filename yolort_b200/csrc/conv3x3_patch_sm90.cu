@@ -574,14 +574,14 @@ TileGeom pick_geom(int H, int W, bool allow_wrap, bool s2) {
 // Eligibility: 3x3 / stride 1 / pad 1 and a feature map that one of the two tilings covers with little waste.
 bool patch_conv_eligible(const yb_op_desc& d) {
   if (d.kind != YB_OP_CONV || d.ksize != 3 || d.pad != 1) return false;
-  if (d.reserved & 1) return false;   // caller asked for the generic im2col kernel
+  if (d.reserved & YB_CONV_FORCE_IM2COL) return false;   // caller asked for the generic im2col kernel
   if (d.stride == 2)   // two column-parity planes: even width, and an output map that 16 x 8 tiles cover well.
     // With two channel chunks (four 38 KB planes per tile) or a split N tile the planes leave little room for the
-    // pipeline, so those stay on the im2col kernel unless the caller forces the variant (bit 2).
-    return (d.reserved & 2) == 0 && d.W % 2 == 0 && d.H % 2 == 0 && classic_eff(d.Ho, d.Wo) >= 0.7 &&
-           ((d.Cin <= 64 && d.Cout <= 128) || (d.reserved & 4));
+    // pipeline, so those stay on the im2col kernel unless the caller forces the variant (YB_CONV_FORCE_PLANES).
+    return (d.reserved & YB_CONV_BAND_STEM) == 0 && d.W % 2 == 0 && d.H % 2 == 0 && classic_eff(d.Ho, d.Wo) >= 0.7 &&
+           ((d.Cin <= 64 && d.Cout <= 128) || (d.reserved & YB_CONV_FORCE_PLANES));
   if (d.stride != 1) return false;
-  const bool band = (d.reserved & 2) != 0;
+  const bool band = (d.reserved & YB_CONV_BAND_STEM) != 0;
   const double eff = band ? classic_eff(d.H, d.W) : (classic_eff(d.H, d.W) > wrap_eff(d.H, d.W) ? classic_eff(d.H, d.W) : wrap_eff(d.H, d.W));
   return eff >= 0.7;
 }
@@ -590,9 +590,9 @@ static int patch_conv_plan(const yb_op_desc& d, int ctas, PatchParams& kp, dim3&
 
 // Pure host logic: tiling, shared-memory layout and launch shape (no driver calls).  Two CTAs per SM when the shape has
 // a two-CTA instance, its plan fits half of the SM's shared memory with resident weights and there are tasks for both
-// (reserved bit 4 keeps one CTA per SM: tests compare the two launches bit for bit).
+// (YB_CONV_ONE_CTA keeps one CTA per SM: tests compare the two launches bit for bit).
 static int patch_conv_configure(const yb_op_desc& d, PatchParams& kp, dim3& grid, size_t& smem_bytes) {
-  if (!(d.reserved & 16) && patch_conv_plan(d, 2, kp, grid, smem_bytes) == YB_OK) return YB_OK;
+  if (!(d.reserved & YB_CONV_ONE_CTA) && patch_conv_plan(d, 2, kp, grid, smem_bytes) == YB_OK) return YB_OK;
   return patch_conv_plan(d, 1, kp, grid, smem_bytes);
 }
 
@@ -607,8 +607,8 @@ static int patch_conv_plan(const yb_op_desc& d, int ctas, PatchParams& kp, dim3&
   kp.s2 = d.stride == 2 ? 1 : 0;
   kp.H = d.Ho;     // the kernel tiles the OUTPUT map (equal to the input extent at stride 1)
   kp.W = d.Wo;
-  // reserved bit 1: the weights are the banded super-pixel stem matrix [Cout_pad][3 rows][2 x 64] (engine.stem_band)
-  kp.band = (d.reserved & 2) ? 1 : 0;
+  // the weights are the banded super-pixel stem matrix [Cout_pad][3 rows][2 x 64] (engine.stem_band)
+  kp.band = (d.reserved & YB_CONV_BAND_STEM) ? 1 : 0;
   kp.tg = pick_geom(kp.H, kp.W, !kp.band, kp.s2 != 0);
   const TileGeom& tg = kp.tg;
   kp.tiles_x = (kp.W + tg.x_step - 1) / tg.x_step;
@@ -653,7 +653,7 @@ static int patch_conv_plan(const yb_op_desc& d, int ctas, PatchParams& kp, dim3&
   // layers (144 KB slice + 3 x 23 KB patches + staging > 222 KB): those keep the pair-of-tiles weight stream.
   int forced_store_cols = 0;
   size_t staging_ns = staging;
-  if (!kp.b_resident && !kp.band && !kp.s2 && d.chain == nullptr && !(d.reserved & 8)) {
+  if (!kp.b_resident && !kp.band && !kp.s2 && d.chain == nullptr && !(d.reserved & YB_CONV_NO_NSPLIT)) {
     for (int ns = 2; ns <= 4 && !kp.b_resident; ns *= 2) {
       if (d.Cout % (16 * ns) || sms % ns) continue;
       const int bn = d.Cout / ns;

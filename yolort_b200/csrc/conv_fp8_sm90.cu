@@ -343,12 +343,15 @@ Fp8KernelFn select_fp8_kernel_t(int block_n) {
   }
 }
 
-int out_kind(const yb_op_desc& d) { return (d.reserved & 16) ? kOutF16 : ((d.reserved & 32) ? kOutBf16 : kOutE4m3); }
+int out_kind(const yb_op_desc& d) {
+  return (d.reserved & YB_CONV_E4M3_F16_OUT) ? kOutF16 : ((d.reserved & YB_CONV_E4M3_BF16_OUT) ? kOutBf16 : kOutE4m3);
+}
 
 // Pure host logic: validation, tiling, pipeline depth and launch shape (no driver calls).
 int fp8_configure(const yb_op_desc& d, Fp8ConvParams& kp, dim3& grid, size_t& smem_bytes) {
   YB_REQUIRE(d.dtype == YB_F8E4M3, "e4m3 conv: dtype must be YB_F8E4M3");
-  YB_REQUIRE((d.reserved & ~48) == 0 && (d.reserved & 48) != 48,
+  constexpr int kOutBits = YB_CONV_E4M3_F16_OUT | YB_CONV_E4M3_BF16_OUT;
+  YB_REQUIRE((d.reserved & ~kOutBits) == 0 && (d.reserved & kOutBits) != kOutBits,
              "e4m3 conv: reserved may only set bit 4 (fp16 output) or bit 5 (bf16 output), got 0x%x", d.reserved);
   YB_REQUIRE(d.decode == nullptr && d.chain == nullptr, "e4m3 conv: no fused decode and no chained tail");
   YB_REQUIRE(d.act >= YB_ACT_NONE && d.act <= YB_ACT_RELU, "e4m3 conv: unknown activation %d", d.act);

@@ -551,7 +551,7 @@ static int conv_configure(const yb_op_desc& d, ConvKernelParams& kp, dim3& grid,
   const long long M_ll = static_cast<long long>(d.N) * Ho * Wo;
   YB_REQUIRE(M_ll > 0 && M_ll < (1ll << 31), "conv: M out of range");
 
-  YB_REQUIRE(!(d.reserved & 2) || patch_conv_eligible(d),
+  YB_REQUIRE(!(d.reserved & YB_CONV_BAND_STEM) || patch_conv_eligible(d),
              "conv: banded stem weights (reserved bit 1) need the halo-patch kernel, which this %dx%d map does not qualify for",
              d.H, d.W);
   if (patch_conv_eligible(d)) return YB_OK;   // configured by patch_conv_configure
@@ -559,9 +559,9 @@ static int conv_configure(const yb_op_desc& d, ConvKernelParams& kp, dim3& grid,
   //   two CTAs of two consumer warpgroups (104 registers) when the shape has such an instance;
   //   otherwise two CTAs of ONE consumer warpgroup (64-row tiles, 232 registers) when the shape has that instance;
   //   one CTA of two consumer warpgroups.
-  // Each two-CTA plan must fit half of the SM's shared memory and have a tile for each of the 2 x SMs CTAs.  Reserved
-  // bit 4 keeps the last layout (tests compare the launches bit for bit).
-  if (!(d.reserved & 16) &&
+  // Each two-CTA plan must fit half of the SM's shared memory and have a tile for each of the 2 x SMs CTAs.
+  // YB_CONV_ONE_CTA keeps the last layout (tests compare the launches bit for bit).
+  if (!(d.reserved & YB_CONV_ONE_CTA) &&
       (conv_plan(d, 2, 2, kp, grid, smem_bytes) == YB_OK || conv_plan(d, 2, 1, kp, grid, smem_bytes) == YB_OK))
     return YB_OK;
   return conv_plan(d, 1, 2, kp, grid, smem_bytes);

@@ -20,7 +20,7 @@ import ctypes
 import math
 import os
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Tuple
+from typing import Callable, Dict, List, Optional, Tuple
 
 import torch
 from torch import nn
@@ -56,7 +56,7 @@ class _View:
     C: int
 
 
-@dataclass
+@dataclass(kw_only=True)
 class _Op:
     kind: int
     src: _View
@@ -236,7 +236,9 @@ class _Lowering:
         wp, bp = self.pack(w, b)
         if ref_flops_per_pixel is None:
             ref_flops_per_pixel = 2 * w.shape[0] * w.shape[1] * k * k
-        self.ops.append(_Op(_C.YB_OP_CONV, src, dst, k, s, p, act, wp, bp, residual, name, ref_flops_per_pixel, pack, force_im2col))
+        self.ops.append(_Op(kind=_C.YB_OP_CONV, src=src, dst=dst, ksize=k, stride=s, pad=p, act=act, weight=wp, bias=bp,
+                            residual=residual, name=name, flops_per_pixel=ref_flops_per_pixel, pack=pack,
+                            force_im2col=force_im2col))
 
     def pack(self, w: torch.Tensor, b: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
         """Packed weight and fp32 bias of a convolution from its fp64 folded weight and bias."""
@@ -251,7 +253,8 @@ class _Lowering:
         assert co4 % 64 == 0 and co4 <= 256, "banded stem needs 64 | 4*Cout <= 256"
         wp = w_band.to(self.dtype).to(self.device).contiguous()
         bp = pack_bias(b, co4, self.device)
-        self.ops.append(_Op(_C.YB_OP_CONV, src, dst, 3, 1, 1, act, wp, bp, None, name, ref_flops_per_pixel, 4, False, True))
+        self.ops.append(_Op(kind=_C.YB_OP_CONV, src=src, dst=dst, ksize=3, stride=1, pad=1, act=act, weight=wp, bias=bp,
+                            name=name, flops_per_pixel=ref_flops_per_pixel, pack=4, band=True))
 
     def conv_module(self, name, m: Conv, src: _View, dst: _View, residual=None):
         w, b = fold_conv_bn(m)
@@ -375,7 +378,7 @@ class _Lowering:
             self.conv(f"{p}.q|k|v+in_proj", w4(w_qkv), ma.in_proj_bias.detach().double(), x, qkv, 1, 1, 0,
                       _C.YB_ACT_NONE, ref_flops_per_pixel=12 * E * E)
             att = _View(self.buf(f"{p}.attn", div, E), 0, E)
-            self.ops.append(_Op(_C.YB_OP_ATTENTION, qkv, att, ksize=heads, name=f"{p}.ma(attention)"))
+            self.ops.append(_Op(kind=_C.YB_OP_ATTENTION, src=qkv, dst=att, ksize=heads, name=f"{p}.ma(attention)"))
             x1 = _View(self.buf(f"{p}.x1", div, E), 0, E)
             self.conv(f"{p}.ma.out_proj", w4(ma.out_proj.weight.detach().double()), ma.out_proj.bias.detach().double(),
                       att, x1, 1, 1, 0, _C.YB_ACT_NONE, residual=x, ref_flops_per_pixel=2 * E * E)
@@ -392,46 +395,55 @@ class _Lowering:
         c_ = m.cv1.conv.out_channels
         cat = self.buf(f"{name}.cat", div, 4 * c_)
         self.conv_module(f"{name}.cv1", m.cv1, src, _View(cat, 0, c_))
-        self.ops.append(_Op(_C.YB_OP_SPP_POOL, _View(cat, 0, c_), _View(cat, c_, 3 * c_), name=f"{name}.pool"))
+        self.ops.append(_Op(kind=_C.YB_OP_SPP_POOL, src=_View(cat, 0, c_), dst=_View(cat, c_, 3 * c_),
+                            name=f"{name}.pool"))
         self.conv_module(f"{name}.cv2", m.cv2, _View(cat, 0, 4 * c_), dst)
 
     def upsample(self, name, src: _View, dst: _View):
-        self.ops.append(_Op(_C.YB_OP_UPSAMPLE2X, src, dst, name=name))
+        self.ops.append(_Op(kind=_C.YB_OP_UPSAMPLE2X, src=src, dst=dst, name=name))
 
     def stem(self, prefix: str, stem: nn.Module, stem_variant: str) -> Tuple[_Buf, _View]:
         """The CSPDarknet stem over the plan's space-to-depth canvas: (canvas buffer, stem output view).  A Focus
         (r3.1 / r4.0) is a channel permutation of the s2d input, the r6.0 6x6/s2/p2 convolution an exact 3x3/s1/p1
         convolution over it."""
-        x0 = self.buf("input.s2d", 2, 16)
         if isinstance(stem, Focus):       # r3.1 / r4.0: Focus = 2x2 space-to-depth + 3x3/s1/p1 conv (darknetv4.py:82)
             stem = stem.conv
             if stem.conv.kernel_size != (3, 3) or stem.conv.stride != (1, 1) or stem.conv.padding != (1, 1):
                 raise NotImplementedError("Focus stem must be the 3x3/s1/p1 convolution")
-            w, b = fold_conv_bn(stem)
-            w_s2d = focus_to_s2d(w)
+            to_s2d = focus_to_s2d
         else:                             # r6.0: 6x6/s2/p2 conv == 3x3/s1/p1 over the same space-to-depth input
             if stem.conv.kernel_size != (6, 6) or stem.conv.stride != (2, 2) or stem.conv.padding != (2, 2):
                 raise NotImplementedError("stem must be the r6.0 6x6/s2/p2 convolution")
-            w, b = fold_conv_bn(stem)
-            w_s2d = stem_to_s2d(w)
+            to_s2d = stem_to_s2d
+        w, b = fold_conv_bn(stem)
+        return self.s2d_stem(f"{prefix}.0", w, b, to_s2d, act_code(stem.act), stem_variant)
+
+    def s2d_stem(self, name: str, w: torch.Tensor, b: torch.Tensor, to_s2d, act: int, variant: str,
+                 what: str = "3x3") -> Tuple[_Buf, _View]:
+        """The first convolution (folded weight `w`, bias `b`), rewritten by `to_s2d` into a 3x3/s1/p1 convolution over
+        the plan's space-to-depth canvas: (canvas buffer, output view).  `variant`: "auto" | "band" | "superpixel" |
+        "im2col"; `what` names the rewrite in the op name.  flops_per_pixel counts the reference convolution's work
+        per super-pixel."""
+        x0 = self.buf("input.s2d", 2, 16)
         co = w.shape[0]
-        t0 = self.buf(f"{prefix}.0", 2, co)
+        t0 = self.buf(name, 2, co)
+        w_s2d = to_s2d(w)
         # The stem runs over "super-pixels" of 4 horizontally adjacent s2d pixels (128-byte TMA rows instead of 32).  Its
         # expanded weight matrix is block-banded, and when the band (6 slabs of 4*Cout x 64) fits in shared memory next
         # to two patches (4*Cout <= 128: yolov5n / s) the banded kernel variant multiplies only the band; wider stems
         # (m / l / x) use the dense super-pixel form.
         spk = 4
         co4 = spk * co
-        if stem_variant == "band" or (stem_variant == "auto" and co4 % 64 == 0 and co4 <= 128
-                                      and act_code(stem.act) in (_C.YB_ACT_SILU, _C.YB_ACT_NONE)):
+        flops = spk * 2 * w.numel()
+        if variant == "band" or (variant == "auto" and co4 % 64 == 0 and co4 <= 128
+                                 and act in (_C.YB_ACT_SILU, _C.YB_ACT_NONE)):
             w_b, b_b = stem_band(w_s2d, b)
-            self.conv_band(f"{prefix}.0(stem: banded 3x3 over s2d super-pixels)", w_b, b_b, _View(x0, 0, 16),
-                           _View(t0, 0, co), act_code(stem.act), ref_flops_per_pixel=spk * 2 * co * 3 * 36)
+            self.conv_band(f"{name}(stem: banded {what} over s2d super-pixels)", w_b, b_b, _View(x0, 0, 16),
+                           _View(t0, 0, co), act, ref_flops_per_pixel=flops)
         else:
             w_sp, b_sp = stem_superpixel(w_s2d, b, spk)
-            self.conv(f"{prefix}.0(stem: 3x3 over s2d super-pixels)", w_sp, b_sp, _View(x0, 0, 16), _View(t0, 0, co),
-                      3, 1, 1, act_code(stem.act), ref_flops_per_pixel=spk * 2 * co * 3 * 36, pack=spk,
-                      force_im2col=(stem_variant == "im2col"))
+            self.conv(f"{name}(stem: {what} over s2d super-pixels)", w_sp, b_sp, _View(x0, 0, 16), _View(t0, 0, co),
+                      3, 1, 1, act, ref_flops_per_pixel=flops, pack=spk, force_im2col=(variant == "im2col"))
         return x0, _View(t0, 0, co)
 
     def stages(self, prefix: str, mods: List[nn.Module], cur: _View, tap_dst: Dict[int, _View]) -> _View:
@@ -462,8 +474,20 @@ class _Lowering:
                 cur = dst
         return cur
 
+    def heads(self, feats: List[_View], convs) -> List[_Buf]:
+        """The detection head: one 1x1 convolution `convs[i]` (an nn.Conv2d with bias, no activation) per level over
+        feats[i], into buffer "head.{i}" with the output channels padded to 16.  Returns those buffers."""
+        head_bufs = []
+        for i, (feat, conv) in enumerate(zip(feats, convs)):
+            co_buf = _round_up(conv.out_channels, 16)
+            hb = self.buf(f"head.{i}", feat.buf.div, co_buf)
+            self.conv(f"head.head.{i}", conv.weight.detach().double(), conv.bias.detach().double(), feat,
+                      _View(hb, 0, co_buf), 1, 1, 0, _C.YB_ACT_NONE)
+            head_bufs.append(hb)
+        return head_bufs
+
     def avgpool(self, name, src: _View, dst: _View):
-        self.ops.append(_Op(_C.YB_OP_AVGPOOL, src, dst, name=name))
+        self.ops.append(_Op(kind=_C.YB_OP_AVGPOOL, src=src, dst=dst, name=name))
 
     def dwconv(self, name, w, b, src: _View, dst: _View, k, s, act):
         """Depthwise k x k / s convolution (YB_OP_DWCONV): w [C,1,k,k] (BN folded, fp64) -> [k*k][C] in the compute
@@ -472,7 +496,8 @@ class _Lowering:
         assert tuple(w.shape) == (C, 1, k, k) and dst.C == C, (name, tuple(w.shape), src.C, dst.C)
         wp = w.reshape(C, k * k).t().contiguous().to(self.dtype).to(self.device)
         bp = b.to(torch.float32).to(self.device).contiguous()
-        self.ops.append(_Op(_C.YB_OP_DWCONV, src, dst, k, s, k // 2, act, wp, bp, None, name, 2 * k * k * C))
+        self.ops.append(_Op(kind=_C.YB_OP_DWCONV, src=src, dst=dst, ksize=k, stride=s, pad=k // 2, act=act, weight=wp,
+                            bias=bp, name=name, flops_per_pixel=2 * k * k * C))
 
     def squeeze_excitation(self, name, m: nn.Module, x: _View):
         """torchvision.ops.SqueezeExcitation (ops/misc.py): x * hardsigmoid(fc2(relu(fc1(mean_hw(x))))) in place
@@ -485,7 +510,7 @@ class _Lowering:
         w2t = m.fc2.weight.detach().reshape(C, S).t().float()
         w = torch.cat([w1t.reshape(-1), w2t.reshape(-1)]).to(self.device).contiguous()
         b = torch.cat([m.fc1.bias.detach().float(), m.fc2.bias.detach().float()]).to(self.device).contiguous()
-        self.ops.append(_Op(_C.YB_OP_SE, x, x, ksize=S, weight=w, bias=b, name=name))
+        self.ops.append(_Op(kind=_C.YB_OP_SE, src=x, dst=x, ksize=S, weight=w, bias=b, name=name))
 
     def conv_norm_act(self, name, m: nn.Sequential, src: _View, dst: _View, residual=None):
         """torchvision Conv2dNormActivation: conv [-> FrozenBatchNorm2d] [-> activation], one group, BN folded in fp64
@@ -550,7 +575,7 @@ class _Fp8Lowering(_Lowering):
     def stem(self, prefix: str, stem: nn.Module, stem_variant: str) -> Tuple[_Buf, _View]:
         x0, out = super().stem(prefix, stem, stem_variant)
         q = _View(self.buf(f"{prefix}.0(e4m3)", out.buf.div, out.C), 0, out.C)
-        self.ops.append(_Op(_C.YB_OP_QUANTIZE, out, q, name=f"{prefix}.0(quantize)"))
+        self.ops.append(_Op(kind=_C.YB_OP_QUANTIZE, src=out, dst=q, name=f"{prefix}.0(quantize)"))
         self.quantized = True
         return x0, q
 
@@ -614,15 +639,7 @@ def lower_yolo(model: nn.Module, dtype: torch.dtype, device: torch.device, stem_
         L.block(f"pan.layer_blocks.{2 * idx + 2}", layer[2 * idx + 2], _View(cat_up[l], 0, 2 * ch[idx]), r)
         results.append(r)
 
-    head_bufs = []
-    for i, (feat, conv) in enumerate(zip(results, model.head.head)):
-        co = conv.out_channels
-        co_buf = _round_up(co, 16)
-        hb = L.buf(f"head.{i}", feat.buf.div, co_buf)
-        L.conv(f"head.head.{i}", conv.weight.detach().double(), conv.bias.detach().double(), feat,
-               _View(hb, 0, co_buf), 1, 1, 0, _C.YB_ACT_NONE)
-        head_bufs.append(hb)
-    return L, x0, head_bufs, {f"p{l + 3}": r for l, r in enumerate(results)}
+    return L, x0, L.heads(results, model.head.head), {f"p{l + 3}": r for l, r in enumerate(results)}
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -734,6 +751,7 @@ def lower_fp8(model: nn.Module, dtype: torch.dtype, device: torch.device, amax: 
             for b in q:
                 scale[id(b)] = s
     head_ids = {id(b) for b in head_bufs}
+    head_out = _C.YB_CONV_E4M3_BF16_OUT if dtype == torch.bfloat16 else _C.YB_CONV_E4M3_F16_OUT     # 16-bit logits
     for i, op in enumerate(L.ops[qi:], start=qi):
         if op.kind == _C.YB_OP_QUANTIZE:
             op.bias = torch.tensor([1.0 / scale[id(op.dst.buf)]], dtype=torch.float32, device=device)
@@ -750,7 +768,7 @@ def lower_fp8(model: nn.Module, dtype: torch.dtype, device: torch.device, amax: 
         tail[2 * co_pad] = scale[id(op.residual.buf)] if op.residual is not None else 0.0
         tail[2 * co_pad + 1] = 1.0 if head else 1.0 / scale[id(op.dst.buf)]
         op.bias = tail.to(torch.float32).to(device).contiguous()
-        op.reserved = (32 if dtype == torch.bfloat16 else 16) if head else 0
+        op.reserved = head_out if head else 0
     return L, x0, head_bufs, feats, scale
 
 
@@ -803,20 +821,13 @@ def lower_lite(model: nn.Module, dtype: torch.dtype, device: torch.device):
     if len(model.head.head) != len(return_layers) + 1 or not isinstance(fpn.extra_blocks, LastLevelMaxPool):
         raise NotImplementedError("lowering covers BackboneWithFPN with LastLevelMaxPool and one head per level")
 
-    x0 = L.buf("input.s2d", 2, 16)
     name0, stem = layers[0]
     conv, bn, act = _split_conv_norm_act(f"body.{name0}", stem)
     if conv.kernel_size != (3, 3) or conv.stride != (2, 2) or conv.padding != (1, 1) or conv.in_channels != 3 \
             or conv.groups != 1:
         raise NotImplementedError("stem must be a 3x3/s2/p1 convolution over RGB")
     w, b = _fold_conv_norm(conv, bn)
-    co = w.shape[0]
-    t0 = L.buf(f"body.{name0}", 2, co)
-    spk = 4
-    w_sp, b_sp = stem_superpixel(stem_s2_to_s2d(w), b, spk)
-    L.conv(f"body.{name0}(stem: 3x3/s2 as 3x3 over s2d super-pixels)", w_sp, b_sp, _View(x0, 0, 16), _View(t0, 0, co),
-           3, 1, 1, act, ref_flops_per_pixel=spk * 2 * co * 3 * 9, pack=spk)
-    cur = _View(t0, 0, co)
+    x0, cur = L.s2d_stem(f"body.{name0}", w, b, stem_s2_to_s2d, act, "superpixel", what="3x3/s2 as 3x3")
     taps: Dict[str, _View] = {}
     if name0 in return_layers:
         taps[return_layers[name0]] = cur
@@ -862,17 +873,7 @@ def lower_lite(model: nn.Module, dtype: torch.dtype, device: torch.device):
              _C.YB_ACT_NONE)
     feats = {str(i): r for i, r in enumerate(results)}
     feats["pool"] = pool
-
-    head_bufs = []
-    for i, (key, hc) in enumerate(zip(list(feats), model.head.head)):
-        feat = feats[key]
-        co = hc.out_channels
-        co_buf = _round_up(co, 16)
-        hb = L.buf(f"head.{i}", feat.buf.div, co_buf)
-        L.conv(f"head.head.{i}", hc.weight.detach().double(), hc.bias.detach().double(), feat, _View(hb, 0, co_buf), 1,
-               1, 0, _C.YB_ACT_NONE)
-        head_bufs.append(hb)
-    return L, x0, head_bufs, feats
+    return L, x0, L.heads(list(feats.values()), model.head.head), feats
 
 
 def lower_darknet(model: nn.Module, dtype: torch.dtype, device: torch.device, stem_variant: str = "auto"):
@@ -949,9 +950,15 @@ class Lowered:
             return None
         return list(head)
 
-    def head_weights(self) -> List[torch.Tensor]:
-        """fp64 [Cout, Cin] weights of the head convolutions (from the parameters)."""
-        return [c.weight.detach().double().view(c.out_channels, c.in_channels) for c in self.head_convs()]
+    def head_dgrad_packs(self) -> List[Tuple[torch.Tensor, torch.Tensor]]:
+        """Per head level, from the parameters: the transposed head weight W^T [Cin, Cout] packed for the conv kernel
+        with the rounding of the forward's packed weights, and a zero bias."""
+        packs = []
+        for c in self.head_convs():
+            w = c.weight.detach().double().view(c.out_channels, c.in_channels)
+            packs.append(self.L.pack(w.t()[:, :, None, None],
+                                     torch.zeros(w.shape[1], dtype=torch.float64, device=w.device)))
+        return packs
 
     def refresh_head(self) -> None:
         """Re-pack and round the head weights and biases from the parameters INTO the tensors every plan points at:
@@ -965,9 +972,8 @@ class Lowered:
             op.bias.copy_(bp)
         packs = self.__dict__.get("_head_dgrad_w")
         if packs is not None:
-            for (wt, _), w in zip(packs, self.head_weights()):
-                wt.copy_(self.L.pack(w.t()[:, :, None, None], torch.zeros(w.shape[1], dtype=torch.float64,
-                                                                            device=w.device))[0])
+            for (wt, _), (new, _) in zip(packs, self.head_dgrad_packs()):
+                wt.copy_(new)
 
 
 def front_op_count(L: _Lowering) -> int:
@@ -1072,6 +1078,104 @@ def assign_offsets(L: _Lowering, x0: _Buf, keep: List[_Buf], N: int, H: int, W: 
     return offsets, top
 
 
+def encode(op: _Op, dtype: torch.dtype, N: int, H: int, W: int, ptr: Callable[[_View], int], *,
+           tail: Optional[_Op] = None, decode: Optional["_C.HeadDecode"] = None,
+           keep_intermediates: bool = False) -> Tuple["_C.OpDesc", Optional["_C.ConvChain"]]:
+    """The yb_op_desc of `op` over N images of an H x W canvas, in compute dtype `dtype` unless the op carries its own
+    element type, with `ptr(view)` the address of a view.  Returns the descriptor and, with `tail` (the 1x1 convolution
+    after `op`, riding on its launch), the yb_conv_chain it points at: the caller keeps that alive as long as the
+    descriptor, and likewise `decode`, the fused decode epilogue of a head convolution.  With `keep_intermediates` a
+    chained op stores its output even when only the tail reads it."""
+    d = _C.OpDesc()
+    hi, wi = op.src.buf.hw(H, W)
+    ho, wo = op.dst.buf.hw(H, W)
+    k = op.pack
+    if wi % k or wo % k:
+        raise ValueError(f"{op.name}: width {wi} not divisible by the pixel packing {k}")
+    d.kind, d.dtype = op.kind, _C.dtype_code(dtype) if op.dtype is None else op.dtype
+    d.N, d.H, d.W = N, hi, wi // k
+    d.Cin, d.in_cstride, d.in_ = op.src.C * k, op.src.buf.C * k, ptr(op.src)
+    d.Ho, d.Wo = ho, wo // k
+    d.Cout, d.out_cstride, d.out = op.dst.C * k, op.dst.buf.C * k, ptr(op.dst)
+    d.ksize, d.stride, d.pad, d.act = op.ksize, op.stride, op.pad, op.act
+    if op.weight is not None:
+        d.weight = op.weight.data_ptr()
+    if op.bias is not None:
+        d.bias = op.bias.data_ptr()
+    if op.kind == _C.YB_OP_CONV:
+        d.Cout_pad, _, d.Cin_pad = op.weight.shape
+        if op.band:
+            d.Cin_pad = 64     # [Cout_pad, 3, 2 x 64] banded stem matrix: one 64-channel chunk of super-pixels
+    if op.dtype == _C.YB_F8E4M3:
+        d.reserved = op.reserved
+    elif op.kind == _C.YB_OP_CONV:
+        if op.force_im2col:
+            d.reserved |= _C.YB_CONV_FORCE_IM2COL
+        if op.band:
+            d.reserved |= _C.YB_CONV_BAND_STEM
+        if os.environ.get("YB_NO_NSPLIT", "0") == "1":      # A/B timing: keep streamed weights + tile pairs
+            d.reserved |= _C.YB_CONV_NO_NSPLIT
+    if op.residual is not None:
+        d.residual, d.res_cstride = ptr(op.residual), op.residual.buf.C
+    if decode is not None:
+        d.decode = ctypes.addressof(decode)
+    chain = None
+    if tail is not None:
+        chain = _C.ConvChain()
+        chain.weight, chain.bias = tail.weight.data_ptr(), tail.bias.data_ptr()
+        chain.Cout_pad, _, chain.K_pad = tail.weight.shape
+        chain.Cout, chain.act = tail.dst.C, tail.act
+        chain.out, chain.out_cstride = ptr(tail.dst), tail.dst.buf.C
+        chain.own_C = op.chain_own
+        if op.chain_extra is not None:
+            extra = op.chain_extra
+            chain.extra, chain.extra_C, chain.extra_cstride = ptr(extra), extra.C, extra.buf.C
+        # stage-wise inspection wants every activation in memory, also the one only the tail reads
+        chain.store_first = 1 if (op.chain_store or keep_intermediates) else 0
+        d.chain = ctypes.addressof(chain)
+    return d, chain
+
+
+def _tensor_ptr(*pairs: Tuple[_Buf, torch.Tensor]) -> Callable[[_View], int]:
+    """`ptr` for encode() over stand-alone buffers, each held by its own tensor: (buffer, tensor) pairs."""
+    addr = {id(b): t.data_ptr() for b, t in pairs}
+    return lambda v: addr[id(v.buf)] + v.ch0 * v.buf.esz
+
+
+def launch_groups(L: _Lowering, N: int, H: int, W: int, fuse_chains: bool, front_ops: int,
+                  keep_intermediates: bool) -> List[Tuple[int, ...]]:
+    """The launch list: groups of op indices that run as one kernel.  An op marked for a chained tail (chain_own) runs
+    together with the next op when the library supports the pair, unless the pair would straddle the end of the
+    chunked front (`front_ops`)."""
+    launches: List[Tuple[int, ...]] = []
+    i = 0
+    while i < len(L.ops):
+        n = 2 if (fuse_chains and i + 1 < len(L.ops) and i + 1 != front_ops and
+                  _chainable(L.ops[i], L.ops[i + 1], L.dtype, N, H, W, keep_intermediates)) else 1
+        launches.append(tuple(range(i, i + n)))
+        i += n
+    return launches
+
+
+def _chainable(op: _Op, tail: _Op, dtype: torch.dtype, N: int, H: int, W: int, keep_intermediates: bool) -> bool:
+    if not (op.chain_own > 0 and op.kind == _C.YB_OP_CONV and op.pack == 1 and tail.kind == _C.YB_OP_CONV
+            and tail.ksize == 1 and tail.stride == 1 and tail.residual is None and tail.pack == 1):
+        return False
+    # support depends on shapes / alignment only, hence the dummy address; `chain` keeps d.chain valid for the query
+    d, chain = encode(op, dtype, N, H, W, lambda v: 4096, tail=tail, keep_intermediates=keep_intermediates)
+    return _C.conv_chain_supported(d)
+
+
+def _op_flops(op: _Op, N: int, H: int, W: int) -> int:
+    """Algorithmic work of one op over N images of an H x W canvas (the reference's, for convolutions)."""
+    ho, wo = op.dst.buf.hw(H, W)
+    if op.kind in (_C.YB_OP_CONV, _C.YB_OP_DWCONV):
+        return N * ho * (wo // op.pack) * op.flops_per_pixel
+    if op.kind == _C.YB_OP_ATTENTION:   # Q K^T and P V: 4 L E per token
+        return N * (ho * wo) * 4 * (ho * wo) * op.dst.C
+    return 0
+
+
 class PlanInstance:
     """Arena + native plan for one (N, H, W); weights come from the Engine's shared `Lowered`."""
 
@@ -1090,117 +1194,24 @@ class PlanInstance:
         # chunked front: 4 chunks when the batch divides (>= 4 images per chunk)
         front_ops = front_op_count(L) if (chunked and N % 4 == 0 and N >= 16 and not keep_intermediates) else 0
         self.front_chunks = 4 if front_ops else 0
-        code = _C.dtype_code(L.dtype)
-        self._chains: List[_C.ConvChain] = []    # yb_conv_chain blocks the descriptors point at (kept alive)
-        no_nsplit = os.environ.get("YB_NO_NSPLIT", "0") == "1"    # A/B timing: keep streamed weights + tile pairs
-
-        def make_desc(op: _Op, ptr) -> "_C.OpDesc":
-            d = _C.OpDesc()
-            hi, wi = op.src.buf.hw(H, W)
-            ho, wo = op.dst.buf.hw(H, W)
-            d.kind, d.dtype = op.kind, code if op.dtype is None else op.dtype
-            k = op.pack
-            if wi % k or wo % k:
-                raise ValueError(f"{op.name}: width {wi} not divisible by the pixel packing {k}")
-            wi, wo = wi // k, wo // k
-            d.N, d.H, d.W = N, hi, wi
-            d.Cin, d.in_cstride, d.in_ = op.src.C * k, op.src.buf.C * k, ptr(op.src)
-            d.Ho, d.Wo = ho, wo
-            d.Cout, d.out_cstride, d.out = op.dst.C * k, op.dst.buf.C * k, ptr(op.dst)
-            d.ksize, d.stride, d.pad, d.act = op.ksize, op.stride, op.pad, op.act
-            if op.kind == _C.YB_OP_CONV:
-                d.weight, d.bias = op.weight.data_ptr(), op.bias.data_ptr()
-                d.Cout_pad, _, d.Cin_pad = op.weight.shape
-                if op.band:
-                    d.Cin_pad = 64     # [Cout_pad, 3, 2 x 64] banded stem matrix: one 64-channel chunk of super-pixels
-            elif op.kind in (_C.YB_OP_DWCONV, _C.YB_OP_SE):
-                d.weight, d.bias = op.weight.data_ptr(), op.bias.data_ptr()
-            elif op.kind == _C.YB_OP_QUANTIZE:
-                d.bias = op.bias.data_ptr()
-            d.reserved = (1 if op.force_im2col else 0) | (2 if op.band else 0) | (8 if no_nsplit else 0)
-            if op.kind in (_C.YB_OP_ATTENTION, _C.YB_OP_DWCONV, _C.YB_OP_SE, _C.YB_OP_AVGPOOL, _C.YB_OP_QUANTIZE):
-                d.reserved = 0        # these ops have no option bits
-            if op.dtype == _C.YB_F8E4M3:
-                d.reserved = op.reserved
-            if op.residual is not None:
-                d.residual, d.res_cstride = ptr(op.residual), op.residual.buf.C
-            return d
-
-        def make_chain(op: _Op, tail: _Op, ptr) -> "_C.ConvChain":
-            """yb_conv_chain for `tail` (the 1x1 convolution after `op`) riding on `op`'s launch."""
-            c = _C.ConvChain()
-            c.weight, c.bias = tail.weight.data_ptr(), tail.bias.data_ptr()
-            c.Cout_pad, _, c.K_pad = tail.weight.shape
-            c.Cout, c.act = tail.dst.C, tail.act
-            c.out, c.out_cstride = ptr(tail.dst), tail.dst.buf.C
-            c.own_C = op.chain_own
-            if op.chain_extra is not None:
-                c.extra, c.extra_C, c.extra_cstride = ptr(op.chain_extra), op.chain_extra.C, op.chain_extra.buf.C
-            # stage-wise inspection wants every activation in memory, also the one only the tail reads
-            c.store_first = 1 if (op.chain_store or keep_intermediates) else 0
-            return c
-
-        def chainable(i: int) -> bool:
-            op = L.ops[i]
-            if not (fuse_chains and op.chain_own > 0 and i + 1 < len(L.ops) and i + 1 != front_ops):
-                return False
-            tail = L.ops[i + 1]
-            if not (tail.kind == _C.YB_OP_CONV and tail.ksize == 1 and tail.stride == 1 and tail.residual is None
-                    and tail.pack == 1 and op.pack == 1 and op.kind == _C.YB_OP_CONV):
-                return False
-            d = make_desc(op, lambda v: 4096)           # support depends on shapes / alignment only
-            c = make_chain(op, tail, lambda v: 4096)
-            d.chain = ctypes.addressof(c)
-            return _C.conv_chain_supported(d)
-
-        # launch list: groups of op indices that run as one kernel
-        launches: List[Tuple[int, ...]] = []
-        i = 0
-        while i < len(L.ops):
-            if chainable(i):
-                launches.append((i, i + 1))
-                i += 2
-            else:
-                launches.append((i,))
-                i += 1
+        launches = launch_groups(L, N, H, W, fuse_chains, front_ops, keep_intermediates)
         self.launch_ops = launches
         step_of = {j: t for t, grp in enumerate(launches) for j in grp}
         self.front_ops = step_of[front_ops - 1] + 1 if front_ops else 0     # in launches (what the run_* methods count)
         self._front_op_count = front_ops                                       # in ops of the lowering
-        offsets, total = assign_offsets(L, x0, keep, N, H, W, reuse=not keep_intermediates, front_ops=front_ops,
-                                        launches=launches)
+        self._offsets, total = assign_offsets(L, x0, keep, N, H, W, reuse=not keep_intermediates, front_ops=front_ops,
+                                              launches=launches)
         self.arena = torch.zeros((max(total, 1024),), dtype=torch.uint8, device=L.device)
         self.arena_bytes = total
         self.unshared_bytes = sum(_round_up(N * b.hw(H, W)[0] * b.hw(H, W)[1] * b.C * b.esz, 1024) for b in L.bufs)
-        base = self.arena.data_ptr()
 
-        def ptr(v: _View) -> int:
-            return base + offsets[id(v.buf)] + v.ch0 * v.buf.esz
-
-        descs = []
-        self.op_names = []
-        self.op_flops = []
-        for grp in launches:
-            op = L.ops[grp[0]]
-            d = make_desc(op, ptr)
-            name = op.name
-            ho, wo = op.dst.buf.hw(H, W)
-            flops = N * ho * (wo // op.pack) * op.flops_per_pixel if op.kind in (_C.YB_OP_CONV, _C.YB_OP_DWCONV) else 0
-            if op.kind == _C.YB_OP_ATTENTION:   # Q K^T and P V: 4 L E per token
-                tokens = (H // op.dst.buf.div) * (W // op.dst.buf.div)
-                flops = N * tokens * 4 * tokens * op.dst.C
-            if len(grp) == 2:
-                tail = L.ops[grp[1]]
-                c = make_chain(op, tail, ptr)
-                self._chains.append(c)
-                d.chain = ctypes.addressof(c)
-                name = f"{op.name} -> {tail.name}"
-                flops += N * tail.dst.buf.hw(H, W)[0] * tail.dst.buf.hw(H, W)[1] * tail.flops_per_pixel
-            descs.append(d)
-            self.op_names.append(name)
-            self.op_flops.append(flops)
         self._low = low                     # keeps the shared weights alive
         self.n_heads = low.n_heads
+        encoded = [self._encode(grp, N, self._ptr) for grp in launches]
+        descs = [d for d, _ in encoded]
+        self._chains = [c for _, c in encoded if c is not None]    # the yb_conv_chain blocks the descriptors point at
+        self.op_names = [" -> ".join(L.ops[j].name for j in grp) for grp in launches]
+        self.op_flops = [sum(_op_flops(L.ops[j], N, H, W) for j in grp) for grp in launches]
         self.plan = _C.Plan(descs, L.device)
         self._descs = descs
         self._front_plans: Optional[List[_C.Plan]] = None
@@ -1208,32 +1219,40 @@ class PlanInstance:
         # fixed NMS arena instead of storing logits (box_head.py:68-82 + :328-360,418 fused).
         self.fused_post = None
         self.plan_fused = None
-        n_heads = len(head_bufs)
         if post is not None and post["n_anchors"] * (post["num_classes"] + 5) <= 256:
             level_hw = [(H // b.div, W // b.div) for b in head_bufs]
             self.fused_post = _C.FusedPost(N, level_hw, post["strides"], post["anchors_px"], post["num_classes"],
                                            post["score_thresh"], post["nms_thresh"], post["detections_per_img"],
                                            post["semantics"], L.device)
-            fused = list(descs[:-n_heads])
-            import ctypes as _ct
-            for d, hd in zip(descs[-n_heads:], self.fused_post.head_decode):
-                d2 = _C.OpDesc.from_buffer_copy(d)
-                d2.decode = _ct.addressof(hd)
-                fused.append(d2)
+            heads = L.ops[len(L.ops) - self.n_heads:]
+            fused = descs[:-self.n_heads] + [encode(op, L.dtype, N, H, W, self._ptr, decode=hd)[0]
+                                             for op, hd in zip(heads, self.fused_post.head_decode)]
             self.plan_fused = _C.Plan(fused, L.device)
 
-        def nhwc(b: _Buf) -> torch.Tensor:
-            h, w = b.hw(H, W)
-            n = N * h * w * b.C
-            o = offsets[id(b)]
-            return self.arena[o: o + n * b.esz].view(L.dtype if b.esz == 2 else torch.float8_e4m3fn).view(N, h, w, b.C)
-
-        self.input = nhwc(x0)                      # [N, H/2, W/2, 16] space-to-depth canvas
-        self.heads = [nhwc(b) for b in head_bufs]  # [N, h, w, round_up(3*(nc+5), 16)]
-        self.features = {k: nhwc(v.buf) for k, v in feats.items()}
+        self.input = self._nhwc(x0)                      # [N, H/2, W/2, 16] space-to-depth canvas
+        self.heads = [self._nhwc(b) for b in head_bufs]  # [N, h, w, round_up(3*(nc+5), 16)]
+        self.features = {k: self._nhwc(v.buf) for k, v in feats.items()}
         # every buffer by name; with arena reuse (the default) only `input`, `heads` and `features` hold their data
         # after a full run -- ask for `keep_intermediates=True` to inspect the others
-        self.buffers = {b.name: nhwc(b) for b in L.bufs}
+        self.buffers = {b.name: self._nhwc(b) for b in L.bufs}
+
+    def _encode(self, grp: Tuple[int, ...], N: int, ptr: Callable[[_View], int]):
+        """encode() of launch `grp`: an op, or an op and its chained tail."""
+        L = self._low.L
+        return encode(L.ops[grp[0]], L.dtype, N, self.H, self.W, ptr, tail=L.ops[grp[1]] if len(grp) == 2 else None,
+                      keep_intermediates=self.keep_intermediates)
+
+    def _ptr(self, v: _View, image: int = 0) -> int:
+        """Address of view `v` from image `image` on (activations are NHWC, image-major)."""
+        h, w = v.buf.hw(self.H, self.W)
+        return self.arena.data_ptr() + self._offsets[id(v.buf)] + (image * h * w * v.buf.C + v.ch0) * v.buf.esz
+
+    def _nhwc(self, b: _Buf) -> torch.Tensor:
+        h, w = b.hw(self.H, self.W)
+        n = self.N * h * w * b.C
+        o = self._offsets[id(b)]
+        dtype = self.dtype if b.esz == 2 else torch.float8_e4m3fn
+        return self.arena[o: o + n * b.esz].view(dtype).view(self.N, h, w, b.C)
 
     @property
     def device_bytes(self) -> int:
@@ -1254,11 +1273,11 @@ class PlanInstance:
         inv = self.__dict__.setdefault("_inv_scales", {})
         if key not in inv:
             inv[key] = torch.tensor([1.0 / self._low.feat_scales[key]], dtype=torch.float32, device=self.device)
-        d = _C.OpDesc()
-        d.kind, d.dtype = _C.YB_OP_QUANTIZE, _C.dtype_code(self.dtype)
-        d.N, d.H, d.W, d.Cin, d.in_cstride, d.in_ = N, h, w, C, C, x.data_ptr()
-        d.Ho, d.Wo, d.Cout, d.out_cstride, d.out = h, w, C, C, dst.data_ptr()
-        d.bias = inv[key].data_ptr()
+        xb, qb = _Buf("x", 1, C), _Buf(key, 1, C, esz=1)
+        # ksize and stride are not read by YB_OP_QUANTIZE
+        op = _Op(kind=_C.YB_OP_QUANTIZE, src=_View(xb, 0, C), dst=_View(qb, 0, C), ksize=0, stride=0, bias=inv[key],
+                 name=f"{key}(quantize)")
+        d, _ = encode(op, self.dtype, N, h, w, _tensor_ptr((xb, x), (qb, dst)))
         _C.Plan([d], self.device).run()
 
     def run(self, first: int = 0, count: Optional[int] = None) -> None:
@@ -1287,36 +1306,13 @@ class PlanInstance:
 
     # -- chunked front ----------------------------------------------------------------------------------------------
     def _build_front_plans(self) -> None:
-        """Launch lists of ops [0, front_ops) restricted to the images of one chunk: same descriptors, N = chunk and
-        every tensor pointer advanced by the chunk's images (activations are NHWC, image-major)."""
-        L = self._low.L
+        """Launch lists of ops [0, front_ops) restricted to the images of one chunk: N = chunk and every view starting
+        at the chunk's first image."""
         c = self.N // self.front_chunks
         plans = []
         for k in range(self.front_chunks):
-            ds = []
-            chains = []
-            for grp, d in zip(self.launch_ops[: self.front_ops], self._descs[: self.front_ops]):
-                op = L.ops[grp[0]]
-                d2 = _C.OpDesc.from_buffer_copy(d)
-                d2.N = c
-
-                def adv(view):
-                    return k * c * (self.H // view.buf.div) * (self.W // view.buf.div) * view.buf.C * view.buf.esz
-
-                d2.in_ = d.in_ + adv(op.src)
-                d2.out = d.out + adv(op.dst)
-                if op.residual is not None:
-                    d2.residual = d.residual + adv(op.residual)
-                if len(grp) == 2:      # chained tail: its own block of pointers
-                    tail = L.ops[grp[1]]
-                    c2 = _C.ConvChain.from_buffer_copy(_C.ConvChain.from_address(d.chain))
-                    c2.out = c2.out + adv(tail.dst)
-                    if op.chain_extra is not None:
-                        c2.extra = c2.extra + adv(op.chain_extra)
-                    chains.append(c2)
-                    d2.chain = ctypes.addressof(c2)
-                ds.append(d2)
-            plans.append(_C.Plan(ds, self.device))      # the native plan copies what it needs at creation
+            encoded = [self._encode(grp, c, lambda v: self._ptr(v, k * c)) for grp in self.launch_ops[: self.front_ops]]
+            plans.append(_C.Plan([d for d, _ in encoded], self.device))   # the native plan copies what it needs here
         self._front_plans = plans
 
     def run_front_chunk(self, k: int) -> None:
@@ -1351,17 +1347,13 @@ class _HeadDgrad:
     def __init__(self, low: "Lowered", lvl: int, N: int, h: int, w: int, cin: int):
         L = low.L
         wt, bias = head_dgrad_weights(low)[lvl]
-        head = L.ops[len(L.ops) - low.n_heads + lvl]
-        cpad = head.dst.buf.C
+        cpad = low.head_bufs[lvl].C
         self.dy = torch.zeros((N, h, w, cpad), dtype=L.dtype, device=L.device)
         self.dx = torch.empty((N, h, w, cin), dtype=L.dtype, device=L.device)
-        d = _C.OpDesc()
-        d.kind, d.dtype = _C.YB_OP_CONV, _C.dtype_code(L.dtype)
-        d.N, d.H, d.W, d.Cin, d.in_cstride, d.in_ = N, h, w, cpad, cpad, self.dy.data_ptr()
-        d.Ho, d.Wo, d.Cout, d.out_cstride, d.out = h, w, cin, cin, self.dx.data_ptr()
-        d.ksize, d.stride, d.pad, d.act = 1, 1, 0, _C.YB_ACT_NONE
-        d.weight, d.bias = wt.data_ptr(), bias.data_ptr()
-        d.Cout_pad, _, d.Cin_pad = wt.shape
+        dy, dx = _Buf("dy", 1, cpad), _Buf("dx", 1, cin)
+        op = _Op(kind=_C.YB_OP_CONV, src=_View(dy, 0, cpad), dst=_View(dx, 0, cin), weight=wt, bias=bias,
+                 name=f"head.head.{lvl}(dgrad)")
+        d, _ = encode(op, L.dtype, N, h, w, _tensor_ptr((dy, self.dy), (dx, self.dx)))
         self.plan = _C.Plan([d], L.device)
         self._keep = (wt, bias)
 
@@ -1376,9 +1368,7 @@ def head_dgrad_weights(low: "Lowered") -> List[Tuple[torch.Tensor, torch.Tensor]
     with them (Engine._refresh_head)."""
     packs = low.__dict__.get("_head_dgrad_w")
     if packs is None:
-        packs = [low.L.pack(w.t()[:, :, None, None], torch.zeros(w.shape[1], dtype=torch.float64, device=w.device))
-                 for w in low.head_weights()]
-        low.__dict__["_head_dgrad_w"] = packs
+        packs = low.__dict__["_head_dgrad_w"] = low.head_dgrad_packs()
     return packs
 
 
@@ -1436,24 +1426,19 @@ class Engine:
             if not self._refresh_head():
                 self.invalidate()
         use_fp8 = self.fp8 is not None if fp8 is None else fp8
-        if use_fp8:
-            if self.fp8 is None:
-                raise ValueError("an FP8 lowering needs a calibration (set_fp8)")
-            if self._low8 is None:
-                with _C.device_guard(self.device):
-                    if self._low is None:
-                        self._tensors = [t for t in list(self.model.parameters()) + list(self.model.buffers())]
-                        self._versions = self._fingerprint()
-                    self._low8 = Lowered(self.model, self.dtype, self.device, self.stem_variant, fp8=self.fp8)
-                self.lowerings += 1
-            return self._low8
-        if self._low is None:
+        if use_fp8 and self.fp8 is None:
+            raise ValueError("an FP8 lowering needs a calibration (set_fp8)")
+        attr = "_low8" if use_fp8 else "_low"
+        low = getattr(self, attr)
+        if low is None:
             with _C.device_guard(self.device):
-                self._tensors = [t for t in list(self.model.parameters()) + list(self.model.buffers())]
-                self._versions = self._fingerprint()
-                self._low = Lowered(self.model, self.dtype, self.device, self.stem_variant)
+                if self._low is None and self._low8 is None:
+                    self._tensors = [t for t in list(self.model.parameters()) + list(self.model.buffers())]
+                    self._versions = self._fingerprint()
+                low = Lowered(self.model, self.dtype, self.device, self.stem_variant, fp8=self.fp8 if use_fp8 else None)
+            setattr(self, attr, low)
             self.lowerings += 1
-        return self._low
+        return low
 
     def _refresh_head(self) -> bool:
         """Head fine-tuning: after in-place edits of the head parameters only (an optimizer step) on a model whose
