@@ -35,6 +35,7 @@ extern "C" {
 #define YB_F8E4M3 4 /* float8 e4m3 ("fn": max 448, no infinities); values are stored divided by a power-of-two scale */
 
 const char* yb_last_error(void);
+/* 2 since yb_conv_config fills a yb_conv_info; it filled twelve ints at 1 */
 int yb_abi_version(void);
 
 /* ------------------------------------------------------------------------------------------------
@@ -209,7 +210,7 @@ typedef struct {
  *   bias: fp32 {1/s}; weight, residual, decode and chain NULL; act and reserved 0.  out = RN_satfinite(in * (1/s)).
  * YB_OP_SPP_POOL and YB_OP_UPSAMPLE2X with dtype YB_F8E4M3: source and destination share one scale, so the pool is a
  *   max over the decoded values and the upsample a copy, both exact; channel counts and cstrides multiples of 16.
- * yb_abi_version() stays 1 with FP8: the descriptor layout is unchanged, and the element type, the op kind and the
+ * FP8 left yb_abi_version() unchanged: the descriptor layout is the same, and the element type, the op kind and the
  * reserved bits are additions that every earlier descriptor leaves at values it already had to use. */
 typedef struct {
   int32_t kind;
@@ -248,22 +249,44 @@ typedef struct {
  * emits the two convolutions separately).  Pure host logic: no GPU needed. */
 int yb_conv_chain_supported(const yb_op_desc* op);
 
-/* Host-only introspection of how a convolution would be launched (tests, tuning): fills 12 ints
- *   [0] 1 = halo-patch kernel, 0 = im2col / 1x1 kernel, 2 = the e4m3 kernel   [1] N-tile width   [2] N tiles   [3] weights resident in
- *   shared memory   [4] M tiles per weight pass   [5] patch slots (pipeline stages)   [6] weight-ring slabs (k-iterations
- *   per stage)   [7] store-box columns   [8] staging buffers per epilogue group (halo-patch kernel) / epilogue groups
- *   (1x1 / im2col kernel)   [9] dynamic shared memory   [10] grid
- *   [11] flags: bit 0 chained tail fused; bit 1 two CTAs resident per SM (else one); bit 2 two CTAs resident per
- *   SM of ONE consumer warpgroup each (1x1 / im2col kernel, 64-row tiles; [8] is then 1).  A convolution takes two
- *   CTAs per SM (bit 1) when its kernel has a two-CTA instance for the N tile (1x1 / im2col: N <= 64 with no tail or
- *   a tail of at most 64 columns; halo patch: N = 32 or 64, or 32 with a 64-column tail, single-tile tasks, resident
- *   weights in one N tile, no banded stem), its plan fits half of
- *   the SM's shared memory and it has at least 2 x SMs tiles; the grid is then up to 2 x SMs.  Otherwise a 1x1 /
- *   im2col convolution takes two one-warpgroup CTAs per SM (bit 2) when its one-CTA plan has a 256-column N tile and
- *   no chained tail and it has at least 3 x SMs 128-row tiles: it then runs as two 128-column N tiles ([1], [2])
- *   whose weights stay resident (at most 80 KB per N tile, one N tile per CTA), in half of the SM's shared memory,
- *   on a grid of 2 x SMs.  Pure host logic. */
-int yb_conv_config(const yb_op_desc* op, int32_t* info12);
+/* How a convolution is launched (yb_conv_config). */
+#define YB_CONV_KERNEL_IM2COL 0   /* the 1x1 / im2col kernel (conv_sm90.cu) */
+#define YB_CONV_KERNEL_PATCH 1    /* the 3x3 halo-patch kernel (conv3x3_patch_sm90.cu) */
+#define YB_CONV_KERNEL_E4M3 2     /* the e4m3 kernel (conv_fp8_sm90.cu) */
+#define YB_CONV_TILING_ROWS 0     /* tiles of consecutive output rows M (1x1 / im2col and e4m3 kernels) */
+#define YB_CONV_TILING_CLASSIC 1  /* halo patch: 16 x 8 pixel tiles */
+#define YB_CONV_TILING_WRAP 2     /* halo patch: 5 x 24 pixel tiles of maps at most 22 pixels wide */
+#define YB_CONV_TILING_STRIDE2 3  /* halo patch: 16 x 8 output pixels over two column-parity planes of the input */
+typedef struct {
+  int32_t kernel;            /* YB_CONV_KERNEL_* */
+  int32_t block_n;           /* N-tile width (the wgmma N) */
+  int32_t n_tiles;           /* N tiles */
+  int32_t weights_resident;  /* the weights of the CTA's N tile stay in shared memory */
+  int32_t tiles_per_pass;    /* M tiles per weight pass (halo patch: 2 when pairs of tiles share each weight slab) */
+  int32_t slots;             /* pipeline stages (halo patch: patch slots) */
+  int32_t ring;              /* k-iterations per stage (halo patch: weight-ring slabs, 0 with resident weights) */
+  int32_t store_cols;        /* store-box columns */
+  int32_t store_bufs;        /* staging buffers per epilogue group */
+  int32_t groups;            /* consumer warpgroups per CTA: 2, or 1 (1x1 / im2col kernel, 64-row tiles) */
+  int32_t resident_ctas;     /* CTAs resident per SM: 1 or 2 */
+  int32_t chained;           /* a chained tail is fused */
+  int32_t smem_bytes;        /* dynamic shared memory per CTA */
+  int32_t grid;              /* CTAs of the persistent grid */
+  int32_t tiling;            /* YB_CONV_TILING_* */
+  int32_t m_tiles;           /* output tiles along M */
+  int32_t work_items;        /* tiles (halo patch: tasks) the grid walks */
+  int32_t tail_n;            /* wgmma N of the chained tail, 0 without one */
+} yb_conv_info;
+
+/* Host-only introspection of how a convolution would be launched (tests, tuning).  A convolution takes two CTAs per SM
+ * of two consumer warpgroups each when its kernel has a two-CTA instance for the N tile (1x1 / im2col: N <= 64 with no
+ * tail or a tail of at most 64 columns; halo patch: N = 32 or 64, or 32 with a 64-column tail, single-tile tasks,
+ * resident weights in one N tile, no banded stem), its plan fits half of the SM's shared memory and it has at least
+ * 2 x SMs tiles; the grid is then up to 2 x SMs.  Otherwise a 1x1 / im2col convolution takes two CTAs per SM of ONE
+ * consumer warpgroup each (64-row tiles) when its one-CTA plan has a 256-column N tile and no chained tail and it has at
+ * least 3 x SMs 128-row tiles: it then runs as two 128-column N tiles whose weights stay resident (at most 80 KB per N
+ * tile, one N tile per CTA), in half of the SM's shared memory, on a grid of 2 x SMs.  Pure host logic. */
+int yb_conv_config(const yb_op_desc* op, yb_conv_info* info);
 
 typedef struct yb_plan yb_plan;
 

@@ -24,7 +24,6 @@ NONE, SILU, HSWISH, LEAKY, RELU = (_C.YB_ACT_NONE, _C.YB_ACT_SILU, _C.YB_ACT_HAR
                                    _C.YB_ACT_RELU)
 SENTINEL = 7.0
 SMS = torch.cuda.get_device_properties(0).multi_processor_count if torch.cuda.is_available() else 132
-TILE_M = 128                                              # output rows per tile (both kernels)
 
 
 @dataclasses.dataclass(frozen=True)
@@ -142,45 +141,12 @@ def fake_ptr(name: str) -> int:
     return _FAKE[name]
 
 
-# ---- what the planner does with a case (host logic, mirrored where yb_conv_config does not report it) -----------------
-def mma_n(n: int) -> int:
-    c = 16
-    while c < n:
-        c <<= 1
-    return c
-
-
-def _classic_eff(H, W):
-    return H * W / (((H + 15) // 16) * ((W + 7) // 8) * 128)
-
-
-def _wrap_eff(H, W):
-    return 0.0 if (W > 22 or W < 9) else H * W / (((H + 4) // 5) * 128)
-
-
-def patch_tiling(case: Case) -> tuple:
-    """(tiling, M tiles) of the halo-patch kernel: pick_geom of conv3x3_patch_sm90.cu."""
-    Ho, Wo = case.Ho, case.Wo
-    if case.s == 2:
-        return "stride2", case.N * ((Ho + 15) // 16) * ((Wo + 7) // 8)
-    if _wrap_eff(Ho, Wo) > _classic_eff(Ho, Wo):
-        return "wrap", case.N * ((Ho + 4) // 5) * ((Wo + 23) // 24)
-    return "classic", case.N * ((Ho + 15) // 16) * ((Wo + 7) // 8)
-
-
+# ---- what the planner does with a case (yb_conv_config) ----------------------------------------------------------------
 def instance_key(case: Case, d, cfg: dict) -> tuple:
     """(kernel, dtype, N tile, fused decode, tail N, CTAs per SM): the template instance the launch runs."""
-    n2 = mma_n(_pads(case.chain.C2, 16, case.dtype)[1]) if case.chain else 0
     kernel = "patch" if cfg["patch_kernel"] else "conv"
-    return (kernel, "bf16" if case.dtype == BF16 else "f16", cfg["block_n"], bool(d.decode), n2, cfg["ctas_per_sm"])
-
-
-def tiles(case: Case, cfg: dict) -> int:
-    """Work items of the persistent grid: tiles (1x1 / im2col kernel) or tasks (patch kernel)."""
-    if cfg["patch_kernel"]:
-        m = patch_tiling(case)[1]
-        return (m + cfg["tiles_per_pass"] - 1) // cfg["tiles_per_pass"] * cfg["n_tiles"]
-    return (case.N * case.Ho * case.Wo + TILE_M - 1) // TILE_M * cfg["n_tiles"]
+    return (kernel, "bf16" if case.dtype == BF16 else "f16", cfg["block_n"], bool(d.decode), cfg["tail_n"],
+            cfg["ctas_per_sm"])
 
 
 def plan_paths(case: Case, cfg: dict) -> set:
@@ -188,13 +154,13 @@ def plan_paths(case: Case, cfg: dict) -> set:
     p = set()
     res = "resident" if cfg["weights_resident"] else "streamed"
     if cfg["patch_kernel"]:
-        tiling, m_tiles = patch_tiling(case)
+        tiling = cfg["patch_tiling"]
         p.add(f"patch {tiling}")
         if cfg["weights_resident"]:
             p.add("patch resident single N tile" if cfg["n_tiles"] == 1 else "patch resident N-split")
         elif cfg["tiles_per_pass"] == 2:
             p.add("patch streamed pairs")
-            if m_tiles % 2:
+            if cfg["m_tiles"] % 2:
                 p.add("patch streamed odd last pair")
         if cfg["ctas_per_sm"] == 2:
             p.add(f"two CTAs patch {tiling}")
@@ -209,7 +175,7 @@ def plan_paths(case: Case, cfg: dict) -> set:
             p.add("conv several N tiles")
         if cfg["ctas_per_sm"] == 2:
             p.add("two CTAs conv")
-    n = tiles(case, cfg)
+    n = cfg["work_items"]
     if cfg["ctas_per_sm"] == 2 and n == 2 * SMS:
         p.add("two CTAs at 2 x SMs tiles")
     if cfg["ctas_per_sm"] == 1 and n == 2 * SMS - 1:

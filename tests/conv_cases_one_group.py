@@ -6,7 +6,7 @@ layout takes layers whose one-CTA plan has a 256-column N tile, as two 128-colum
 The cases use the Case / build_desc / check_case machinery of tests/conv_cases.py.  Every case is sized from the
 device's SM count so that it lands on the side of the planner's rule its name states.
 """
-from conv_cases import BF16, F16, LEAKY, NONE, RELU, SMS, Case, mma_n
+from conv_cases import BF16, F16, LEAKY, NONE, RELU, SMS, Case
 from yolort_b200 import _C
 
 ROWS = 128                                                # rows of the one-CTA tile the threshold counts

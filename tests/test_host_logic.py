@@ -26,7 +26,7 @@ def test_library_exports_every_declared_symbol():
     assert declared == set(_C.EXPORTED_SYMBOLS), declared ^ set(_C.EXPORTED_SYMBOLS)
     for name in declared:
         assert hasattr(lib, name), name
-    assert lib.yb_abi_version() == 1
+    assert lib.yb_abi_version() == 2
 
 
 def test_ctypes_structs_match_header_sizes(tmp_path):

@@ -24,6 +24,8 @@ YB_ACT_NONE, YB_ACT_SILU, YB_ACT_HARDSWISH, YB_ACT_LEAKY01, YB_ACT_RELU = 0, 1, 
 # yb_op_desc.reserved option bits of a convolution (fp16 / bf16; e4m3 convolutions take the last two only)
 YB_CONV_FORCE_IM2COL, YB_CONV_BAND_STEM, YB_CONV_FORCE_PLANES, YB_CONV_NO_NSPLIT, YB_CONV_ONE_CTA = 1, 2, 4, 8, 16
 YB_CONV_E4M3_F16_OUT, YB_CONV_E4M3_BF16_OUT = 16, 32
+YB_CONV_KERNEL_IM2COL, YB_CONV_KERNEL_PATCH, YB_CONV_KERNEL_E4M3 = 0, 1, 2
+PATCH_TILINGS = {1: "classic", 2: "wrap", 3: "stride2"}      # yb_conv_info.tiling of the halo-patch kernel
 YB_MAX_LEVELS, YB_MAX_ANCHORS = 4, 4
 NMS_TV_AUTO, NMS_EXACT_PER_CLASS, NMS_OFFSET_TRICK = 0, 1, 2
 
@@ -112,6 +114,13 @@ class ConvChain(ctypes.Structure):
         ("extra", ctypes.c_void_p), ("extra_C", ctypes.c_int32), ("extra_cstride", ctypes.c_int32),
         ("store_first", ctypes.c_int32),
     ]
+
+
+class ConvInfo(ctypes.Structure):
+    """yb_conv_info: how a convolution is launched (include/yolort_b200.h)."""
+    _fields_ = [(name, ctypes.c_int32) for name in (
+        "kernel", "block_n", "n_tiles", "weights_resident", "tiles_per_pass", "slots", "ring", "store_cols", "store_bufs",
+        "groups", "resident_ctas", "chained", "smem_bytes", "grid", "tiling", "m_tiles", "work_items", "tail_n")]
 
 
 class HeadDecode(ctypes.Structure):
@@ -295,7 +304,7 @@ def lib() -> ctypes.CDLL:
                                          ctypes.POINTER(ctypes.c_float)]
     L.yb_plan_create.argtypes = [ctypes.POINTER(OpDesc), ctypes.c_int, ctypes.POINTER(ctypes.c_void_p)]
     L.yb_conv_chain_supported.argtypes = [ctypes.POINTER(OpDesc)]
-    L.yb_conv_config.argtypes = [ctypes.POINTER(OpDesc), ctypes.POINTER(ctypes.c_int32)]
+    L.yb_conv_config.argtypes = [ctypes.POINTER(OpDesc), ctypes.POINTER(ConvInfo)]
     L.yb_plan_run.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
     L.yb_plan_run_range.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
     L.yb_plan_num_launches.argtypes = [ctypes.c_void_p]
@@ -497,22 +506,22 @@ def conv_chain_supported(op: "OpDesc") -> bool:
 
 def conv_config(op: "OpDesc") -> dict:
     """How the library would launch this convolution (host-only): kernel, tiling, residency, shared memory."""
-    info = (ctypes.c_int32 * 12)()
-    check(lib().yb_conv_config(ctypes.byref(op), info), "yb_conv_config")
-    keys = ("patch_kernel", "block_n", "n_tiles", "weights_resident", "tiles_per_pass", "slots", "ring", "store_cols",
-            "store_bufs", "smem_bytes", "grid", "chained")
-    cfg = dict(zip(keys, [int(v) for v in info]))
-    # slot 11: bit 0 chained tail, bit 1 two CTAs per SM of the 104-register instances, bit 2 two CTAs per SM of one
-    # consumer warpgroup each.  "ctas_per_sm" keeps naming the 104-register layout; "resident_ctas" counts both.
-    flags = cfg["chained"]
-    cfg["ctas_per_sm"] = 2 if flags & 2 else 1
-    cfg["resident_ctas"] = 2 if flags & 6 else 1
-    cfg["layout"] = "2x2" if flags & 2 else ("2x1" if flags & 4 else "1x2")   # CTAs per SM x consumer warpgroups
-    cfg["chained"] &= 1
-    cfg["e4m3_kernel"] = int(cfg["patch_kernel"] == 2)   # slot 0 is 2 for the e4m3 kernel (conv_fp8_sm90.cu)
-    cfg["patch_kernel"] = int(cfg["patch_kernel"] == 1)
-    if not cfg["patch_kernel"]:     # slot 8 of the 1x1 / im2col kernel: consumer warpgroups (sharing two staging buffers)
-        cfg["epilogue_groups"] = cfg.pop("store_bufs")
+    info = ConvInfo()
+    check(lib().yb_conv_config(ctypes.byref(op), ctypes.byref(info)), "yb_conv_config")
+    patch = info.kernel == YB_CONV_KERNEL_PATCH
+    cfg = {k: int(getattr(info, k)) for k in ("block_n", "n_tiles", "weights_resident", "tiles_per_pass", "slots", "ring",
+                                               "store_cols", "smem_bytes", "grid", "chained", "resident_ctas", "m_tiles",
+                                               "work_items", "tail_n")}
+    cfg["patch_kernel"] = int(patch)
+    cfg["e4m3_kernel"] = int(info.kernel == YB_CONV_KERNEL_E4M3)
+    # the halo-patch kernel reports its staging buffers, the others their consumer warpgroups (which share two buffers)
+    cfg["store_bufs" if patch else "epilogue_groups"] = int(info.store_bufs if patch else info.groups)
+    # CTAs per SM x consumer warpgroups: "1x2", "2x2" (the 104-register instances) or "2x1"; "ctas_per_sm" names the
+    # 104-register layout only
+    cfg["layout"] = f"{info.resident_ctas}x{info.groups}"
+    cfg["ctas_per_sm"] = 2 if cfg["layout"] == "2x2" else 1
+    if patch:
+        cfg["patch_tiling"] = PATCH_TILINGS[info.tiling]
     return cfg
 
 

@@ -23,34 +23,53 @@ using namespace yb;
 struct yb_plan {
   struct Step {
     yb_op_desc desc;
-    ConvOp* conv;       // non-null for YB_OP_CONV at f16 / bf16
-    Fp8ConvOp* fp8;     // non-null for YB_OP_CONV at e4m3
+    ConvOp* conv;       // non-null for YB_OP_CONV
     AttentionOp* attn;  // non-null for YB_OP_ATTENTION
   };
   std::vector<Step> steps;
   ~yb_plan() {
     for (auto& s : steps) {
-      if (s.conv) conv_op_destroy(s.conv);
-      if (s.fp8) fp8_conv_op_destroy(s.fp8);
+      delete s.conv;
       if (s.attn) attention_op_destroy(s.attn);
     }
   }
 };
 
-extern "C" const char* yb_last_error(void) { return g_err; }
-extern "C" int yb_abi_version(void) { return 1; }
-
-extern "C" int yb_conv_chain_supported(const yb_op_desc* op) {
-  if (op == nullptr || op->kind != YB_OP_CONV || op->chain == nullptr || op->dtype == YB_F8E4M3) return 0;
-  const int rc = patch_conv_eligible(*op) ? patch_conv_configure_check(*op) : conv_configure_check(*op);
-  return rc == YB_OK ? 1 : 0;
+namespace yb {
+int conv_kernel(const yb_op_desc& d) {
+  if (d.dtype == YB_F8E4M3) return YB_CONV_KERNEL_E4M3;
+  return patch_conv_eligible(d) ? YB_CONV_KERNEL_PATCH : YB_CONV_KERNEL_IM2COL;
 }
 
-extern "C" int yb_conv_config(const yb_op_desc* op, int32_t* info12) {
-  YB_REQUIRE(op != nullptr && info12 != nullptr && op->kind == YB_OP_CONV, "conv_config: needs a convolution op and an output array");
-  for (int i = 0; i < 12; ++i) info12[i] = 0;
-  if (op->dtype == YB_F8E4M3) return fp8_conv_configure_check(*op, info12);
-  return patch_conv_eligible(*op) ? patch_conv_configure_check(*op, info12) : conv_configure_check(*op, info12);
+int conv_config(const yb_op_desc& d, yb_conv_info* info) {
+  switch (conv_kernel(d)) {
+    case YB_CONV_KERNEL_E4M3: return fp8_conv_config(d, info);
+    case YB_CONV_KERNEL_PATCH: return patch_conv_config(d, info);
+    default: return im2col_conv_config(d, info);
+  }
+}
+
+int conv_create(const yb_op_desc& d, ConvOp** out) {
+  switch (conv_kernel(d)) {
+    case YB_CONV_KERNEL_E4M3: return fp8_conv_create(d, out);
+    case YB_CONV_KERNEL_PATCH: return patch_conv_create(d, out);
+    default: return im2col_conv_create(d, out);
+  }
+}
+}  // namespace yb
+
+extern "C" const char* yb_last_error(void) { return g_err; }
+extern "C" int yb_abi_version(void) { return 2; }
+
+extern "C" int yb_conv_chain_supported(const yb_op_desc* op) {
+  if (op == nullptr || op->kind != YB_OP_CONV || op->chain == nullptr) return 0;
+  return conv_config(*op, nullptr) == YB_OK ? 1 : 0;
+}
+
+extern "C" int yb_conv_config(const yb_op_desc* op, yb_conv_info* info) {
+  YB_REQUIRE(op != nullptr && info != nullptr && op->kind == YB_OP_CONV, "conv_config: needs a convolution op and an output struct");
+  *info = yb_conv_info();
+  return conv_config(*op, info);
 }
 
 extern "C" int yb_plan_create(const yb_op_desc* ops, int n_ops, yb_plan** plan_out) {
@@ -60,7 +79,6 @@ extern "C" int yb_plan_create(const yb_op_desc* ops, int n_ops, yb_plan** plan_o
     yb_plan::Step st;
     st.desc = ops[i];
     st.conv = nullptr;
-    st.fp8 = nullptr;
     st.attn = nullptr;
     int rc = YB_OK;
     if (ops[i].in == nullptr || ops[i].out == nullptr) {
@@ -70,10 +88,8 @@ extern "C" int yb_plan_create(const yb_op_desc* ops, int n_ops, yb_plan** plan_o
       if (ops[i].weight == nullptr || ops[i].bias == nullptr) {
         set_error("plan_create: conv op %d without weight/bias", i);
         rc = YB_ERR_INVALID;
-      } else if (ops[i].dtype == YB_F8E4M3) {
-        rc = fp8_conv_op_create(ops[i], &st.fp8);   // validates before any driver call
       } else {
-        rc = conv_op_create(ops[i], &st.conv);
+        rc = conv_create(ops[i], &st.conv);   // validates before any driver call
       }
     } else if (ops[i].kind == YB_OP_ATTENTION) {
       rc = attention_op_create(ops[i], &st.attn);   // validates before any driver call
@@ -115,7 +131,7 @@ extern "C" int yb_plan_run_range(yb_plan* plan, int first, int count, void* stre
     int rc;
     switch (st.desc.kind) {
       case YB_OP_CONV:
-        rc = st.fp8 ? fp8_conv_op_launch(st.fp8, stream) : conv_op_launch(st.conv, stream);
+        rc = st.conv->launch(stream);
         break;
       case YB_OP_ATTENTION:
         rc = attention_op_launch(st.attn, stream);

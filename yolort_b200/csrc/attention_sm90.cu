@@ -288,9 +288,6 @@ int attention_configure_check(const yb_op_desc& d) {
 int attention_op_create(const yb_op_desc& d, AttentionOp** out) {
   int rc = attention_configure_check(d);
   if (rc != YB_OK) return rc;
-  EncodeTiledFn encode = nullptr;
-  rc = encode_tiled_entry(&encode);
-  if (rc != YB_OK) return rc;
   AttentionOp* op = new AttentionOp();
   const long long L = static_cast<long long>(d.H) * d.W;
   op->bf16 = d.dtype == YB_BF16;
@@ -299,23 +296,16 @@ int attention_op_create(const yb_op_desc& d, AttentionOp** out) {
   op->p.scale_log2 = 1.4426950408889634f / 8.f;   // log2(e) / sqrt(64)
   op->grid = dim3(static_cast<unsigned>((L + kBlockQ - 1) / kBlockQ), static_cast<unsigned>(d.ksize), static_cast<unsigned>(d.N));
   const CUtensorMapDataType dt = op->bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  cuuint32_t box[3] = {kHeadDim, kBlockKV, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  cuuint64_t dims[3] = {static_cast<cuuint64_t>(d.Cin), static_cast<cuuint64_t>(L), static_cast<cuuint64_t>(d.N)};
-  cuuint64_t strides[2] = {static_cast<cuuint64_t>(d.in_cstride) * 2, static_cast<cuuint64_t>(d.in_cstride) * 2 * L};
-  CUresult cr = encode(&op->tmap_qkv, dt, 3, const_cast<void*>(d.in), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr == CUDA_SUCCESS) {
-    cuuint64_t odims[3] = {static_cast<cuuint64_t>(d.Cout), static_cast<cuuint64_t>(L), static_cast<cuuint64_t>(d.N)};
-    cuuint64_t ostrides[2] = {static_cast<cuuint64_t>(d.out_cstride) * 2, static_cast<cuuint64_t>(d.out_cstride) * 2 * L};
-    cr = encode(&op->tmap_out, dt, 3, d.out, odims, ostrides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const cuuint32_t box[3] = {kHeadDim, kBlockKV, 1};
+  const cuuint64_t dims[3] = {static_cast<cuuint64_t>(d.Cin), static_cast<cuuint64_t>(L), static_cast<cuuint64_t>(d.N)};
+  rc = tmap_tiled(&op->tmap_qkv, "attention q | k | v", dt, d.in, 3, dims, d.in_cstride, box, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+  if (rc == YB_OK) {
+    const cuuint64_t odims[3] = {static_cast<cuuint64_t>(d.Cout), static_cast<cuuint64_t>(L), static_cast<cuuint64_t>(d.N)};
+    rc = tmap_tiled(&op->tmap_out, "attention output", dt, d.out, 3, odims, d.out_cstride, box, CU_TENSOR_MAP_L2_PROMOTION_NONE);
   }
-  if (cr != CUDA_SUCCESS) {
-    set_error("attention: cuTensorMapEncodeTiled failed with CUresult %d (Cin=%d cs=%d L=%lld N=%d)", static_cast<int>(cr),
-              d.Cin, d.in_cstride, L, d.N);
+  if (rc != YB_OK) {
     delete op;
-    return YB_ERR_CUDA;
+    return rc;
   }
   cudaError_t e = op->bf16 ? cudaFuncSetAttribute(attention_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                   static_cast<int>(kSmemBytes))
@@ -331,20 +321,8 @@ int attention_op_create(const yb_op_desc& d, AttentionOp** out) {
 }
 
 int attention_op_launch(const AttentionOp* op, cudaStream_t stream) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = op->grid;
-  cfg.blockDim = dim3(kThreads, 1, 1);
-  cfg.dynamicSmemBytes = kSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  if (op->bf16)
-    YB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, attention_wgmma_kernel<true>, op->tmap_qkv, op->tmap_out, op->p));
-  else
-    YB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, attention_wgmma_kernel<false>, op->tmap_qkv, op->tmap_out, op->p));
+  YB_CHECK_CUDA(launch_pdl(op->bf16 ? attention_wgmma_kernel<true> : attention_wgmma_kernel<false>, op->grid, dim3(kThreads),
+                           kSmemBytes, stream, op->tmap_qkv, op->tmap_out, op->p));
   return YB_OK;
 }
 

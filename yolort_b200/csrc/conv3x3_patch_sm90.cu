@@ -530,22 +530,7 @@ PatchKernelFn select_patch_kernel(const PatchParams& kp) {
   return kp.ep.is_bf16 ? select_patch_kernel_t<true>(kp) : select_patch_kernel_t<false>(kp);
 }
 
-struct PatchConvOp {
-  CUtensorMap tmap_a, tmap_b, tmap_out, tmap_w2, tmap_x, tmap_out2;
-  PatchParams kp;
-  PatchKernelFn fn = nullptr;
-  dim3 grid;
-  size_t smem_bytes;
-};
-
 namespace {
-// wgmma N of an output tile: the next power of two >= 16 (weight rows past Cout_pad are zero-filled by the TMA unit, the
-// store clips columns past Cout)
-int mma_n(int n) {
-  int c = 16;
-  while (c < n) c <<= 1;
-  return c;
-}
 // Fraction of the accumulator rows that are real output pixels, per tiling.
 double classic_eff(int H, int W) {
   const int ty = (H + 15) / 16, tx = (W + 7) / 8;
@@ -767,144 +752,105 @@ static int patch_conv_plan(const yb_op_desc& d, int ctas, PatchParams& kp, dim3&
   return YB_OK;
 }
 
-int patch_conv_configure_check(const yb_op_desc& d, int* info) {
+int patch_conv_config(const yb_op_desc& d, yb_conv_info* info) {
   PatchParams kp;
   dim3 grid;
   size_t smem = 0;
-  const int rc = patch_conv_configure(d, kp, grid, smem);
+  int rc = conv_validate(d);
+  if (rc == YB_OK) rc = patch_conv_configure(d, kp, grid, smem);
   if (rc == YB_OK && info) {   // yb_conv_config: see include/yolort_b200.h
-    info[0] = 1;
-    info[1] = kp.block_n;
-    info[2] = kp.n_tiles;
-    info[3] = kp.b_resident;
-    info[4] = kp.pair;
-    info[5] = kp.a_slots;
-    info[6] = kp.b_resident ? 0 : kp.b_stages;
-    info[7] = kp.store_cols;
-    info[8] = kp.store_bufs;
-    info[9] = static_cast<int>(smem);
-    info[10] = static_cast<int>(grid.x);
-    info[11] = kp.ch.on | (kp.ctas == 2 ? 2 : 0);
+    info->kernel = YB_CONV_KERNEL_PATCH;
+    info->block_n = kp.block_n;
+    info->n_tiles = kp.n_tiles;
+    info->weights_resident = kp.b_resident;
+    info->tiles_per_pass = kp.pair;
+    info->slots = kp.a_slots;
+    info->ring = kp.b_resident ? 0 : kp.b_stages;
+    info->store_cols = kp.store_cols;
+    info->store_bufs = kp.store_bufs;
+    info->groups = kConsumers;
+    info->resident_ctas = kp.ctas;
+    info->chained = kp.ch.on;
+    info->smem_bytes = static_cast<int>(smem);
+    info->grid = static_cast<int>(grid.x);
+    info->tiling = kp.s2 ? YB_CONV_TILING_STRIDE2 : (kp.tg.x_step == 24 ? YB_CONV_TILING_WRAP : YB_CONV_TILING_CLASSIC);
+    info->m_tiles = kp.m_tiles;
+    info->work_items = kp.num_tasks;
+    info->tail_n = kp.ch.n2;
   }
   return rc;
 }
 
-int patch_conv_create(const yb_op_desc& d, EncodeTiledFn encode_tiled, PatchConvOp** out) {
+struct PatchConvOp final : ConvOp {
+  CUtensorMap tmap_a, tmap_b, tmap_out, tmap_w2, tmap_x, tmap_out2;
+  PatchParams kp;
+  PatchKernelFn fn = nullptr;
+  dim3 grid;
+  size_t smem_bytes;
+  int launch(cudaStream_t stream) const override {
+    YB_CHECK_CUDA(launch_pdl(fn, grid, dim3(kThreads), smem_bytes, stream, tmap_a, tmap_b, tmap_out, tmap_w2, tmap_x,
+                             tmap_out2, kp));
+    return YB_OK;
+  }
+};
+
+int patch_conv_create(const yb_op_desc& d, ConvOp** out) {
   PatchConvOp* op = new PatchConvOp();
   PatchParams& kp = op->kp;
-  int rc = patch_conv_configure(d, kp, op->grid, op->smem_bytes);
-  if (rc != YB_OK) {
-    delete op;
-    return rc;
-  }
+  int rc = conv_validate(d);
+  if (rc == YB_OK) rc = patch_conv_configure(d, kp, op->grid, op->smem_bytes);
   const TileGeom& tg = kp.tg;
-  const int block_n = kp.block_n;
-
   const CUtensorMapDataType dt = kp.ep.is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  const int rb = kp.block_k * 2;
-  const CUtensorMapSwizzle sw = rb == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (rb == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-  CUresult cr;
-  if (kp.s2) {
+  const uint32_t bk = kp.block_k;
+  if (rc == YB_OK && kp.s2) {
     // [C, column parity, W/2, H, N] over the NHWC input: a box with parity extent 1 is one plane's patch
-    const cuuint64_t cs = static_cast<cuuint64_t>(d.in_cstride) * 2;
-    cuuint64_t dims[5] = {static_cast<cuuint64_t>(d.Cin), 2, static_cast<cuuint64_t>(d.W / 2), static_cast<cuuint64_t>(d.H),
-                          static_cast<cuuint64_t>(d.N)};
-    cuuint64_t strides[4] = {cs, 2 * cs, cs * d.W, cs * d.W * d.H};
-    cuuint32_t box[5] = {static_cast<cuuint32_t>(kp.block_k), 1, static_cast<cuuint32_t>(tg.pitch), static_cast<cuuint32_t>(tg.patch_h), 1};
-    cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-    cr = encode_tiled(&op->tmap_a, dt, 5, const_cast<void*>(d.in), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                      sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) {
-      set_error("patch conv: cuTensorMapEncodeTiled (stride-2 input planes) failed with CUresult %d", static_cast<int>(cr));
-      delete op;
-      return YB_ERR_CUDA;
-    }
-  } else {
-    cuuint64_t dims[4] = {static_cast<cuuint64_t>(d.Cin), static_cast<cuuint64_t>(d.W), static_cast<cuuint64_t>(d.H),
-                          static_cast<cuuint64_t>(d.N)};
-    cuuint64_t strides[3] = {static_cast<cuuint64_t>(d.in_cstride) * 2, static_cast<cuuint64_t>(d.in_cstride) * 2 * d.W,
-                             static_cast<cuuint64_t>(d.in_cstride) * 2 * d.W * d.H};
-    cuuint32_t box[4] = {static_cast<cuuint32_t>(kp.block_k), static_cast<cuuint32_t>(tg.pitch), static_cast<cuuint32_t>(tg.patch_h), 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    cr = encode_tiled(&op->tmap_a, dt, 4, const_cast<void*>(d.in), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                      sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) {
-      set_error("patch conv: cuTensorMapEncodeTiled (input patch) failed with CUresult %d", static_cast<int>(cr));
-      delete op;
-      return YB_ERR_CUDA;
-    }
+    const cuuint64_t dims[5] = {static_cast<cuuint64_t>(d.Cin), 2, static_cast<cuuint64_t>(d.W / 2),
+                                static_cast<cuuint64_t>(d.H), static_cast<cuuint64_t>(d.N)};
+    const cuuint32_t box[5] = {bk, 1, static_cast<cuuint32_t>(tg.pitch), static_cast<cuuint32_t>(tg.patch_h), 1};
+    rc = tmap_tiled(&op->tmap_a, "patch conv stride-2 input planes", dt, d.in, 5, dims, d.in_cstride, box,
+                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+  } else if (rc == YB_OK) {
+    const cuuint64_t dims[4] = {static_cast<cuuint64_t>(d.Cin), static_cast<cuuint64_t>(d.W), static_cast<cuuint64_t>(d.H),
+                                static_cast<cuuint64_t>(d.N)};
+    const cuuint32_t box[4] = {bk, static_cast<cuuint32_t>(tg.pitch), static_cast<cuuint32_t>(tg.patch_h), 1};
+    rc = tmap_tiled(&op->tmap_a, "patch conv input patch", dt, d.in, 4, dims, d.in_cstride, box,
+                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
   }
-  {
-    const int ktot = kp.band ? 6 * 64 : 9 * d.Cin_pad;
-    cuuint64_t dims[2] = {static_cast<cuuint64_t>(ktot), static_cast<cuuint64_t>(d.Cout_pad)};
-    cuuint64_t strides[1] = {static_cast<cuuint64_t>(ktot) * 2};
-    cuuint32_t box[2] = {static_cast<cuuint32_t>(kp.block_k), static_cast<cuuint32_t>(block_n)};
-    cuuint32_t estr[2] = {1, 1};
-    cr = encode_tiled(&op->tmap_b, dt, 2, const_cast<void*>(d.weight), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                      sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) {
-      set_error("patch conv: cuTensorMapEncodeTiled (weights) failed with CUresult %d", static_cast<int>(cr));
-      delete op;
-      return YB_ERR_CUDA;
-    }
-  }
-  {
-    cuuint64_t dims[4] = {static_cast<cuuint64_t>(d.Cout), static_cast<cuuint64_t>(d.Wo), static_cast<cuuint64_t>(d.Ho),
-                          static_cast<cuuint64_t>(d.N)};
-    cuuint64_t strides[3] = {static_cast<cuuint64_t>(d.out_cstride) * 2, static_cast<cuuint64_t>(d.out_cstride) * 2 * d.Wo,
-                             static_cast<cuuint64_t>(d.out_cstride) * 2 * d.Wo * d.Ho};
-    cuuint32_t box[4] = {static_cast<cuuint32_t>(kp.store_cols), static_cast<cuuint32_t>(tg.tile_w), static_cast<cuuint32_t>(tg.tile_h), 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    const int srb = kp.store_cols * 2;
-    cr = encode_tiled(&op->tmap_out, dt, 4, d.out, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                      srb == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (srb == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B),
-                      CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) {
-      set_error("patch conv: cuTensorMapEncodeTiled (output) failed with CUresult %d", static_cast<int>(cr));
-      delete op;
-      return YB_ERR_CUDA;
-    }
-  }
+  const int ktot = kp.band ? 6 * 64 : 9 * d.Cin_pad;
+  if (rc == YB_OK)
+    rc = tmap_matrix(&op->tmap_b, "patch conv weights", dt, d.weight, ktot, d.Cout_pad, ktot, bk, kp.block_n,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  // NHWC views of the output extent, in boxes of the output tile's tile_w x tile_h pixels
+  const cuuint64_t out_px[3] = {static_cast<cuuint64_t>(d.Wo), static_cast<cuuint64_t>(d.Ho), static_cast<cuuint64_t>(d.N)};
+  auto out_view = [&](CUtensorMap* map, const char* what, const void* base, int C, int cstride, uint32_t box_c,
+                      CUtensorMapL2promotion l2) {
+    const cuuint64_t dims[4] = {static_cast<cuuint64_t>(C), out_px[0], out_px[1], out_px[2]};
+    const cuuint32_t box[4] = {box_c, static_cast<cuuint32_t>(tg.tile_w), static_cast<cuuint32_t>(tg.tile_h), 1};
+    return tmap_tiled(map, what, dt, base, 4, dims, cstride, box, l2);
+  };
+  if (rc == YB_OK)
+    rc = out_view(&op->tmap_out, "patch conv output", d.out, d.Cout, d.out_cstride, kp.store_cols,
+                  CU_TENSOR_MAP_L2_PROMOTION_NONE);
   op->tmap_w2 = op->tmap_b;      // placeholders when nothing is chained (never dereferenced)
   op->tmap_x = op->tmap_a;
   op->tmap_out2 = op->tmap_out;
-  if (kp.ch.on) {
+  if (rc == YB_OK && kp.ch.on) {
     const yb_conv_chain& c = *d.chain;
-    const int kc = kp.ch.w2_row_bytes / 2;
-    const CUtensorMapSwizzle swk = kc == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (kc == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-    cuuint64_t wdims[2] = {static_cast<cuuint64_t>(c.K_pad), static_cast<cuuint64_t>(c.Cout_pad)};
-    cuuint64_t wstrides[1] = {static_cast<cuuint64_t>(c.K_pad) * 2};
-    cuuint32_t wbox[2] = {static_cast<cuuint32_t>(kc), static_cast<cuuint32_t>(kp.ch.n2)};
-    cuuint32_t estr2[2] = {1, 1};
-    cr = encode_tiled(&op->tmap_w2, dt, 2, const_cast<void*>(c.weight), wdims, wstrides, wbox, estr2, CU_TENSOR_MAP_INTERLEAVE_NONE, swk,
-                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    cuuint32_t estr4[4] = {1, 1, 1, 1};
-    if (cr == CUDA_SUCCESS && kp.ch.extra_on) {   // the tile's pixels of the extra operand: the output tile's box
-      cuuint64_t dims[4] = {static_cast<cuuint64_t>(c.extra_C), static_cast<cuuint64_t>(d.Wo), static_cast<cuuint64_t>(d.Ho),
-                            static_cast<cuuint64_t>(d.N)};
-      cuuint64_t strides[3] = {static_cast<cuuint64_t>(c.extra_cstride) * 2, static_cast<cuuint64_t>(c.extra_cstride) * 2 * d.Wo,
-                               static_cast<cuuint64_t>(c.extra_cstride) * 2 * d.Wo * d.Ho};
-      cuuint32_t box[4] = {static_cast<cuuint32_t>(kc), static_cast<cuuint32_t>(tg.tile_w), static_cast<cuuint32_t>(tg.tile_h), 1};
-      cr = encode_tiled(&op->tmap_x, dt, 4, const_cast<void*>(c.extra), dims, strides, box, estr4, CU_TENSOR_MAP_INTERLEAVE_NONE, swk,
-                        CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    }
-    if (cr == CUDA_SUCCESS) {
-      cuuint64_t dims[4] = {static_cast<cuuint64_t>(c.Cout), static_cast<cuuint64_t>(d.Wo), static_cast<cuuint64_t>(d.Ho),
-                            static_cast<cuuint64_t>(d.N)};
-      cuuint64_t strides[3] = {static_cast<cuuint64_t>(c.out_cstride) * 2, static_cast<cuuint64_t>(c.out_cstride) * 2 * d.Wo,
-                               static_cast<cuuint64_t>(c.out_cstride) * 2 * d.Wo * d.Ho};
-      cuuint32_t box[4] = {64, static_cast<cuuint32_t>(tg.tile_w), static_cast<cuuint32_t>(tg.tile_h), 1};
-      cr = encode_tiled(&op->tmap_out2, dt, 4, c.out, dims, strides, box, estr4, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    }
-    if (cr != CUDA_SUCCESS) {
-      set_error("patch conv: cuTensorMapEncodeTiled (chained tail) failed with CUresult %d", static_cast<int>(cr));
-      delete op;
-      return YB_ERR_CUDA;
-    }
+    const uint32_t kc = kp.ch.w2_row_bytes / 2;
+    rc = tmap_matrix(&op->tmap_w2, "patch conv chained tail weights", dt, c.weight, c.K_pad, c.Cout_pad, c.K_pad, kc,
+                     kp.ch.n2, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+    if (rc == YB_OK && kp.ch.extra_on)   // the tile's pixels of the extra operand: the output tile's box
+      rc = out_view(&op->tmap_x, "patch conv chained tail extra operand", c.extra, c.extra_C, c.extra_cstride, kc,
+                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+    if (rc == YB_OK)
+      rc = out_view(&op->tmap_out2, "patch conv chained tail output", c.out, c.Cout, c.out_cstride, 64,
+                    CU_TENSOR_MAP_L2_PROMOTION_NONE);
   }
-  op->fn = select_patch_kernel(kp);
-  rc = set_smem_attributes(reinterpret_cast<const void*>(op->fn), kSmemBudget, kp.ctas, op->smem_bytes, kThreads, "patch conv");
+  if (rc == YB_OK) {
+    op->fn = select_patch_kernel(kp);
+    rc = set_smem_attributes(reinterpret_cast<const void*>(op->fn), kSmemBudget, kp.ctas, op->smem_bytes, kThreads,
+                             "patch conv");
+  }
   if (rc != YB_OK) {
     delete op;
     return rc;
@@ -912,22 +858,5 @@ int patch_conv_create(const yb_op_desc& d, EncodeTiledFn encode_tiled, PatchConv
   *out = op;
   return YB_OK;
 }
-
-int patch_conv_launch(const PatchConvOp* op, cudaStream_t stream) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = op->grid;
-  cfg.blockDim = dim3(kThreads, 1, 1);
-  cfg.dynamicSmemBytes = op->smem_bytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  YB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, op->fn, op->tmap_a, op->tmap_b, op->tmap_out, op->tmap_w2, op->tmap_x, op->tmap_out2, op->kp));
-  return YB_OK;
-}
-
-void patch_conv_destroy(PatchConvOp* op) { delete op; }
 
 }  // namespace yb

@@ -7,6 +7,7 @@
 // :149-173 (C3: cv1||cv2 -> m.0.cv1, m.last.cv2 -> cv3 over the concat).
 #pragma once
 #include "conv_epilogue.cuh"
+#include "host_sm90.h"
 
 namespace yb {
 
@@ -62,8 +63,7 @@ inline const char* chain_setup(const yb_op_desc& d, int block_n, int n_tiles, in
   if (c.Cout_pad % 16 || c.Cout_pad < c.Cout || c.Cout_pad > 256 || c.Cout % 8) return "tail Cout/Cout_pad";
   if (c.out_cstride % 8 || c.out_cstride < c.Cout) return "tail out_cstride";
   if ((reinterpret_cast<uintptr_t>(c.out) & 15) || (reinterpret_cast<uintptr_t>(c.weight) & 15)) return "tail tensors must be 16-byte aligned";
-  int n2 = 16;   // a wgmma N; the weight rows past Cout_pad are zero-filled by the TMA unit
-  while (n2 < c.Cout_pad) n2 <<= 1;
+  const int n2 = mma_n(c.Cout_pad);
   cp->on = 1;
   cp->n2 = n2;
   cp->own_chunks = own_chunks;

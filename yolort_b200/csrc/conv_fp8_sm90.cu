@@ -316,18 +316,6 @@ __global__ void quantize_e4m3_kernel(const uint16_t* __restrict__ in, int in_cs,
   *reinterpret_cast<uint4*>(out + pix * out_cs + c16 * 16) = make_uint4(w[0], w[1], w[2], w[3]);
 }
 
-CUtensorMapSwizzle swizzle_for_bytes(int row_bytes) {
-  return row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                          : (row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                             : (row_bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_NONE));
-}
-
-int mma_n(int n) {
-  int c = 16;
-  while (c < n) c <<= 1;
-  return c;
-}
-
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 using Fp8KernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const Fp8ConvParams);
@@ -370,20 +358,12 @@ int fp8_configure(const yb_op_desc& d, Fp8ConvParams& kp, dim3& grid, size_t& sm
   YB_REQUIRE(d.residual == nullptr || (out == kOutE4m3 && aligned16(d.residual) && d.res_cstride % 16 == 0 &&
                                        d.res_cstride >= d.Cout),
              "e4m3 conv: a residual needs the e4m3 output, 16-byte alignment and res_cstride a multiple of 16");
-  const int Ho = (d.H + 2 * d.pad - d.ksize) / d.stride + 1;
-  const int Wo = (d.W + 2 * d.pad - d.ksize) / d.stride + 1;
-  YB_REQUIRE(Ho == d.Ho && Wo == d.Wo, "e4m3 conv: output extent mismatch (%d,%d) vs (%d,%d)", Ho, Wo, d.Ho, d.Wo);
-  const long long M_ll = static_cast<long long>(d.N) * Ho * Wo;
-  YB_REQUIRE(M_ll > 0 && M_ll < (1ll << 31), "e4m3 conv: M out of range");
-
   kp = Fp8ConvParams();
-  kp.M = static_cast<int>(M_ll);
+  const int rc = conv_rows(d, "e4m3 conv", &kp.M);
+  if (rc != YB_OK) return rc;
   const int m_tiles = (kp.M + kBlockM - 1) / kBlockM;
-  const int sms = num_sms();
-  int n_tiles = (d.Cout + kMaxBlockN - 1) / kMaxBlockN;
-  int block_n = mma_n((d.Cout + n_tiles - 1) / n_tiles);
-  if (m_tiles * n_tiles < 2 * sms && block_n > 128) block_n /= 2;
-  n_tiles = (d.Cout + block_n - 1) / block_n;
+  const int block_n = conv_block_n(d.Cout, m_tiles, false);
+  const int n_tiles = (d.Cout + block_n - 1) / block_n;
   kp.block_n = block_n;
   kp.n_tiles = n_tiles;
   kp.num_tiles = m_tiles * n_tiles;
@@ -392,8 +372,8 @@ int fp8_configure(const yb_op_desc& d, Fp8ConvParams& kp, dim3& grid, size_t& sm
   kp.chunks = d.Cin_pad / kp.block_k;
   kp.num_k_iters = d.ksize * d.ksize * kp.chunks;
   kp.mode = d.ksize == 1 ? 0 : 1;
-  kp.HoWo = Ho * Wo;
-  kp.Wo = Wo;
+  kp.HoWo = d.Ho * d.Wo;
+  kp.Wo = d.Wo;
   kp.stride = d.stride;
   kp.pad = d.pad;
   // store boxes of 128-byte rows where the tile allows (e4m3: up to 128 columns, 16-bit outputs: up to 64)
@@ -412,157 +392,95 @@ int fp8_configure(const yb_op_desc& d, Fp8ConvParams& kp, dim3& grid, size_t& sm
   kp.ep.residual = d.residual;
   kp.ep.res_cstride = d.res_cstride;
 
-  const size_t fixed = static_cast<size_t>(kStageBufs) * kStageBufBytes + 1024;
-  const size_t b_total = static_cast<size_t>(kp.num_k_iters) * kp.b_stage_bytes;
-  kp.b_resident = (n_tiles == 1 && b_total <= 80 * 1024) ? 1 : 0;
-  kp.b_res_bytes = kp.b_resident ? static_cast<uint32_t>(b_total) : 0u;
-  const uint32_t per_iter = kp.a_stage_bytes + (kp.b_resident ? 0u : kp.b_stage_bytes);
-  YB_REQUIRE(kSmemBudget > fixed + kp.b_res_bytes + 2 * per_iter, "e4m3 conv: shared memory budget exceeded (block_n=%d)",
-             kp.block_n);
-  const size_t avail = kSmemBudget - fixed - kp.b_res_bytes;
-  const size_t target = avail / 3 < 32 * 1024 ? avail / 3 : 32 * 1024;
-  int kpg_max = static_cast<int>(target / per_iter);
-  if (kpg_max < 1) kpg_max = 1;
-  if (kpg_max > kp.num_k_iters) kpg_max = kp.num_k_iters;
-  const int groups = (kp.num_k_iters + kpg_max - 1) / kpg_max;
-  kp.kpg = (kp.num_k_iters + groups - 1) / groups;
-  const uint32_t stage_bytes = kp.kpg * per_iter;
-  int stages = static_cast<int>(avail / stage_bytes);
-  if (stages > kMaxStages) stages = kMaxStages;
-  if (stages < 2) stages = 2;
-  kp.stages = stages;
-  grid = dim3(kp.num_tiles < sms ? kp.num_tiles : sms, 1, 1);
-  const size_t smem = static_cast<size_t>(stages) * stage_bytes + kp.b_res_bytes + fixed;
-  YB_REQUIRE(smem <= kSmemBudget, "e4m3 conv: %zu bytes of shared memory needed, %zu available", smem, kSmemBudget);
-  smem_bytes = smem;
+  KPipeline pipe;
+  const int prc = size_k_pipeline(kSmemBudget, static_cast<size_t>(kStageBufs) * kStageBufBytes + 1024, kp.a_stage_bytes,
+                                  kp.b_stage_bytes, kp.num_k_iters, n_tiles == 1, kMaxStages, "e4m3 conv", kp.block_n, &pipe);
+  if (prc != YB_OK) return prc;
+  kp.b_resident = pipe.b_resident;
+  kp.b_res_bytes = pipe.b_res_bytes;
+  kp.kpg = pipe.kpg;
+  kp.stages = pipe.stages;
+  grid = dim3(kp.num_tiles < num_sms() ? kp.num_tiles : num_sms(), 1, 1);
+  smem_bytes = pipe.smem;
   return YB_OK;
 }
 
 }  // namespace
 
-struct Fp8ConvOp {
-  CUtensorMap tmap_a, tmap_b, tmap_out;
-  Fp8ConvParams kp;
-  Fp8KernelFn fn = nullptr;
-  dim3 grid;
-  size_t smem_bytes;
-};
-
-int fp8_conv_configure_check(const yb_op_desc& d, int* info) {
+int fp8_conv_config(const yb_op_desc& d, yb_conv_info* info) {
   Fp8ConvParams kp;
   dim3 grid;
   size_t smem = 0;
   const int rc = fp8_configure(d, kp, grid, smem);
   if (rc == YB_OK && info) {   // yb_conv_config: see include/yolort_b200.h
-    info[0] = 2;               // the e4m3 kernel
-    info[1] = kp.block_n;
-    info[2] = kp.n_tiles;
-    info[3] = kp.b_resident;
-    info[4] = 1;
-    info[5] = kp.stages;
-    info[6] = kp.kpg;
-    info[7] = kp.store_cols;
-    info[8] = kConsumers;
-    info[9] = static_cast<int>(smem);
-    info[10] = static_cast<int>(grid.x);
-    info[11] = 0;
+    info->kernel = YB_CONV_KERNEL_E4M3;
+    info->block_n = kp.block_n;
+    info->n_tiles = kp.n_tiles;
+    info->weights_resident = kp.b_resident;
+    info->tiles_per_pass = 1;
+    info->slots = kp.stages;
+    info->ring = kp.kpg;
+    info->store_cols = kp.store_cols;
+    info->store_bufs = kStageBufs;
+    info->groups = kConsumers;
+    info->resident_ctas = 1;
+    info->smem_bytes = static_cast<int>(smem);
+    info->grid = static_cast<int>(grid.x);
+    info->tiling = YB_CONV_TILING_ROWS;
+    info->m_tiles = kp.num_tiles / kp.n_tiles;
+    info->work_items = kp.num_tiles;
   }
   return rc;
 }
 
-int fp8_conv_op_create(const yb_op_desc& d, Fp8ConvOp** out) {
+struct Fp8ConvOp final : ConvOp {
+  CUtensorMap tmap_a, tmap_b, tmap_out;
+  Fp8ConvParams kp;
+  Fp8KernelFn fn = nullptr;
+  dim3 grid;
+  size_t smem_bytes;
+  int launch(cudaStream_t stream) const override {
+    YB_CHECK_CUDA(launch_pdl(fn, grid, dim3(kThreads), smem_bytes, stream, tmap_a, tmap_b, tmap_out, kp));
+    return YB_OK;
+  }
+};
+
+int fp8_conv_create(const yb_op_desc& d, ConvOp** out) {
   Fp8ConvOp* op = new Fp8ConvOp();
+  const Fp8ConvParams& kp = op->kp;
   int rc = fp8_configure(d, op->kp, op->grid, op->smem_bytes);   // validates before any driver call
-  EncodeTiledFn enc_tiled = nullptr;
-  EncodeIm2colFn enc_im2col = nullptr;
-  if (rc == YB_OK) rc = encode_tiled_entry(&enc_tiled);
-  if (rc == YB_OK) rc = encode_im2col_entry(&enc_im2col);
+  const CUtensorMapDataType u8 = CU_TENSOR_MAP_DATA_TYPE_UINT8;
+  if (rc == YB_OK)
+    rc = kp.mode == 0 ? tmap_matrix(&op->tmap_a, "e4m3 conv input", u8, d.in, d.Cin, kp.M, d.in_cstride, kp.block_k, kBlockM,
+                                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B)
+                      : tmap_im2col(&op->tmap_a, "e4m3 conv input", u8, d, kp.block_k, kBlockM);
+  const int ktot = d.ksize * d.ksize * d.Cin_pad;
+  if (rc == YB_OK)
+    rc = tmap_matrix(&op->tmap_b, "e4m3 conv weights", u8, d.weight, ktot, d.Cout_pad, ktot, kp.block_k, kp.block_n,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  const int ok = out_kind(d);
+  const CUtensorMapDataType dt = ok == kOutE4m3 ? u8 : (ok == kOutBf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                                       : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+  if (rc == YB_OK)
+    rc = tmap_matrix(&op->tmap_out, "e4m3 conv output", dt, d.out, d.Cout, kp.M, d.out_cstride, kp.store_cols, kBlockM,
+                     CU_TENSOR_MAP_L2_PROMOTION_NONE);
+  if (rc == YB_OK) {
+    op->fn = ok == kOutE4m3 ? select_fp8_kernel_t<kOutE4m3>(kp.block_n)
+                            : (ok == kOutF16 ? select_fp8_kernel_t<kOutF16>(kp.block_n)
+                                               : select_fp8_kernel_t<kOutBf16>(kp.block_n));
+    const cudaError_t e = cudaFuncSetAttribute(op->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kSmemBudget));
+    if (e != cudaSuccess) {
+      set_error("e4m3 conv: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
+      rc = YB_ERR_CUDA;
+    }
+  }
   if (rc != YB_OK) {
     delete op;
     return rc;
   }
-  const Fp8ConvParams& kp = op->kp;
-  const CUtensorMapDataType u8 = CU_TENSOR_MAP_DATA_TYPE_UINT8;
-  const CUtensorMapSwizzle sw = swizzle_for_bytes(kp.block_k);
-  const cuuint32_t estr1[2] = {1, 1};
-  CUresult cr;
-  if (kp.mode == 0) {
-    cuuint64_t dims[2] = {static_cast<cuuint64_t>(d.Cin), static_cast<cuuint64_t>(kp.M)};
-    cuuint64_t strides[1] = {static_cast<cuuint64_t>(d.in_cstride)};
-    cuuint32_t box[2] = {static_cast<cuuint32_t>(kp.block_k), kBlockM};
-    cr = enc_tiled(&op->tmap_a, u8, 2, const_cast<void*>(d.in), dims, strides, box, estr1, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  } else {
-    cuuint64_t dims[4] = {static_cast<cuuint64_t>(d.Cin), static_cast<cuuint64_t>(d.W), static_cast<cuuint64_t>(d.H),
-                          static_cast<cuuint64_t>(d.N)};
-    cuuint64_t strides[3] = {static_cast<cuuint64_t>(d.in_cstride), static_cast<cuuint64_t>(d.in_cstride) * d.W,
-                             static_cast<cuuint64_t>(d.in_cstride) * d.W * d.H};
-    int lower[2] = {-d.pad, -d.pad};
-    int upper[2] = {d.pad - (d.ksize - 1), d.pad - (d.ksize - 1)};
-    cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(d.stride), static_cast<cuuint32_t>(d.stride), 1};
-    cr = enc_im2col(&op->tmap_a, u8, 4, const_cast<void*>(d.in), dims, strides, lower, upper,
-                    static_cast<cuuint32_t>(kp.block_k), kBlockM, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
-                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    // the small-tensor im2col descriptor workaround of conv_op_create (conv_sm90.cu)
-    int drv = 0;
-    cudaDriverGetVersion(&drv);
-    const size_t span = static_cast<size_t>(d.in_cstride) * d.W * d.H * d.N;
-    if (cr == CUDA_SUCCESS && drv <= 13010 && span < 131072) reinterpret_cast<uint64_t*>(&op->tmap_a)[1] &= ~(1ull << 21);
-  }
-  if (cr == CUDA_SUCCESS) {
-    const int ktot = d.ksize * d.ksize * d.Cin_pad;
-    cuuint64_t dims[2] = {static_cast<cuuint64_t>(ktot), static_cast<cuuint64_t>(d.Cout_pad)};
-    cuuint64_t strides[1] = {static_cast<cuuint64_t>(ktot)};
-    cuuint32_t box[2] = {static_cast<cuuint32_t>(kp.block_k), static_cast<cuuint32_t>(kp.block_n)};
-    cr = enc_tiled(&op->tmap_b, u8, 2, const_cast<void*>(d.weight), dims, strides, box, estr1,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  }
-  const int ok = out_kind(d);
-  if (cr == CUDA_SUCCESS) {
-    const int esz = ok == kOutE4m3 ? 1 : 2;
-    const CUtensorMapDataType dt = ok == kOutE4m3 ? u8 : (ok == kOutBf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
-                                                                           : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
-    cuuint64_t dims[2] = {static_cast<cuuint64_t>(d.Cout), static_cast<cuuint64_t>(kp.M)};
-    cuuint64_t strides[1] = {static_cast<cuuint64_t>(d.out_cstride) * esz};
-    cuuint32_t box[2] = {static_cast<cuuint32_t>(kp.store_cols), kBlockM};
-    cr = enc_tiled(&op->tmap_out, dt, 2, d.out, dims, strides, box, estr1, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   swizzle_for_bytes(kp.store_cols * esz), CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  }
-  if (cr != CUDA_SUCCESS) {
-    set_error("e4m3 conv: cuTensorMapEncode failed with CUresult %d (Cin=%d cs=%d H=%d W=%d N=%d k=%d s=%d)",
-              static_cast<int>(cr), d.Cin, d.in_cstride, d.H, d.W, d.N, d.ksize, d.stride);
-    delete op;
-    return YB_ERR_CUDA;
-  }
-  op->fn = ok == kOutE4m3 ? select_fp8_kernel_t<kOutE4m3>(kp.block_n)
-                          : (ok == kOutF16 ? select_fp8_kernel_t<kOutF16>(kp.block_n)
-                                             : select_fp8_kernel_t<kOutBf16>(kp.block_n));
-  cudaError_t e = cudaFuncSetAttribute(op->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kSmemBudget));
-  if (e != cudaSuccess) {
-    set_error("e4m3 conv: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
-    delete op;
-    return YB_ERR_CUDA;
-  }
   *out = op;
   return YB_OK;
 }
-
-int fp8_conv_op_launch(const Fp8ConvOp* op, cudaStream_t stream) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = op->grid;
-  cfg.blockDim = dim3(kThreads, 1, 1);
-  cfg.dynamicSmemBytes = op->smem_bytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  YB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, op->fn, op->tmap_a, op->tmap_b, op->tmap_out, op->kp));
-  return YB_OK;
-}
-
-void fp8_conv_op_destroy(Fp8ConvOp* op) { delete op; }
 
 int quantize_configure_check(const yb_op_desc& d) {
   YB_REQUIRE(d.dtype == YB_F16 || d.dtype == YB_BF16, "quantize: dtype (the source type) must be f16 or bf16");
@@ -582,21 +500,11 @@ int quantize_configure_check(const yb_op_desc& d) {
 int quantize_launch(const yb_op_desc& d, cudaStream_t stream) {
   const long long pixels = static_cast<long long>(d.N) * d.H * d.W;
   const long long total = pixels * (d.Cin >> 4);
-  cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(256, 1, 1);
-  cfg.gridDim = dim3(static_cast<unsigned>((total + 255) / 256), 1, 1);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
+  const dim3 grid(static_cast<unsigned>((total + 255) / 256));
   const uint16_t* in = static_cast<const uint16_t*>(d.in);
   uint8_t* out = static_cast<uint8_t*>(d.out);
-  if (d.dtype == YB_BF16)
-    YB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, quantize_e4m3_kernel<true>, in, d.in_cstride, out, d.out_cstride, pixels, d.Cin, d.bias));
-  else
-    YB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, quantize_e4m3_kernel<false>, in, d.in_cstride, out, d.out_cstride, pixels, d.Cin, d.bias));
+  YB_CHECK_CUDA(launch_pdl(d.dtype == YB_BF16 ? quantize_e4m3_kernel<true> : quantize_e4m3_kernel<false>, grid, dim3(256), 0,
+                           stream, in, d.in_cstride, out, d.out_cstride, pixels, d.Cin, d.bias));
   return YB_OK;
 }
 

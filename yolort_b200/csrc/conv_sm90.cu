@@ -415,53 +415,6 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   if (issuer) tma_store_wait_all<0>();
 }
 
-// ---- host side -----------------------------------------------------------------------------------
-EncodeTiledFn g_encode_tiled = nullptr;
-EncodeIm2colFn g_encode_im2col = nullptr;
-
-int load_driver_entry_points() {
-  if (g_encode_tiled && g_encode_im2col) return YB_OK;
-  void* fn = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  YB_CHECK_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-  YB_REQUIRE(fn != nullptr && qres == cudaDriverEntryPointSuccess,
-             "cuTensorMapEncodeTiled not available from the driver");
-  g_encode_tiled = reinterpret_cast<EncodeTiledFn>(fn);
-  fn = nullptr;
-  YB_CHECK_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &fn, cudaEnableDefault, &qres));
-  YB_REQUIRE(fn != nullptr && qres == cudaDriverEntryPointSuccess,
-             "cuTensorMapEncodeIm2col not available from the driver");
-  g_encode_im2col = reinterpret_cast<EncodeIm2colFn>(fn);
-  return YB_OK;
-}
-
-CUtensorMapSwizzle swizzle_for_row_bytes(int row_bytes) {
-  return row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                          : (row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-}
-
-// wgmma N of an output tile: the next power of two >= 16 (weight rows past Cout_pad are zero-filled by the TMA unit, the
-// store clips columns past Cout)
-int mma_n(int n) {
-  int c = 16;
-  while (c < n) c <<= 1;
-  return c;
-}
-
-}  // namespace
-
-int encode_tiled_entry(EncodeTiledFn* out) {
-  const int rc = load_driver_entry_points();
-  if (rc == YB_OK) *out = g_encode_tiled;
-  return rc;
-}
-
-int encode_im2col_entry(EncodeIm2colFn* out) {
-  const int rc = load_driver_entry_points();
-  if (rc == YB_OK) *out = g_encode_im2col;
-  return rc;
-}
-
 using ConvKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
                               const ConvKernelParams);
 
@@ -513,20 +466,12 @@ ConvKernelFn select_conv_kernel(const ConvKernelParams& kp) {
   return kp.ep.is_bf16 ? select_conv_kernel_t<true>(kp) : select_conv_kernel_t<false>(kp);
 }
 
-struct ConvOp {
-  PatchConvOp* patch = nullptr;  // non-null: this conv runs on the halo-patch kernel
-  CUtensorMap tmap_a, tmap_b, tmap_out, tmap_w2, tmap_out2;
-  ConvKernelParams kp;
-  ConvKernelFn fn = nullptr;
-  dim3 grid;
-  size_t smem_bytes;
-};
+}  // namespace
 
 static int conv_plan(const yb_op_desc& d, int ctas, int groups, ConvKernelParams& kp, dim3& grid, size_t& smem_bytes);
 
-// Pure host logic: validates the op and derives tiling, pipeline depth, shared-memory layout and launch shape
-// (no driver calls: yb_conv_chain_supported runs this without a GPU).
-static int conv_configure(const yb_op_desc& d, ConvKernelParams& kp, dim3& grid, size_t& smem_bytes) {
+// Validation of an fp16 / bf16 convolution descriptor, shared with the halo-patch kernel (pure host logic).
+int conv_validate(const yb_op_desc& d) {
   YB_REQUIRE(d.dtype == YB_F16 || d.dtype == YB_BF16, "conv: dtype must be f16 or bf16");
   YB_REQUIRE((d.reserved & ~31) == 0, "conv: reserved bits 5 and up must be zero, got 0x%x", d.reserved);
   YB_REQUIRE(d.ksize >= 1 && d.ksize <= 7 && d.stride >= 1 && d.stride <= 2, "conv: ksize/stride");
@@ -544,17 +489,18 @@ static int conv_configure(const yb_op_desc& d, ConvKernelParams& kp, dim3& grid,
   YB_REQUIRE(d.residual == nullptr ||
                  ((reinterpret_cast<uintptr_t>(d.residual) & 15) == 0 && d.res_cstride % 8 == 0),
              "conv: residual alignment");
-  const int Ho = (d.H + 2 * d.pad - d.ksize) / d.stride + 1;
-  const int Wo = (d.W + 2 * d.pad - d.ksize) / d.stride + 1;
-  YB_REQUIRE(Ho == d.Ho && Wo == d.Wo, "conv: output extent mismatch (%d,%d) vs (%d,%d)", Ho, Wo, d.Ho,
-             d.Wo);
-  const long long M_ll = static_cast<long long>(d.N) * Ho * Wo;
-  YB_REQUIRE(M_ll > 0 && M_ll < (1ll << 31), "conv: M out of range");
+  int M;
+  return conv_rows(d, "conv", &M);
+}
 
-  YB_REQUIRE(!(d.reserved & YB_CONV_BAND_STEM) || patch_conv_eligible(d),
+// Pure host logic: validates the op and derives tiling, pipeline depth, shared-memory layout and launch shape
+// (no driver calls: yb_conv_chain_supported runs this without a GPU).
+static int conv_configure(const yb_op_desc& d, ConvKernelParams& kp, dim3& grid, size_t& smem_bytes) {
+  const int rc = conv_validate(d);
+  if (rc != YB_OK) return rc;
+  YB_REQUIRE(!(d.reserved & YB_CONV_BAND_STEM),
              "conv: banded stem weights (reserved bit 1) need the halo-patch kernel, which this %dx%d map does not qualify for",
              d.H, d.W);
-  if (patch_conv_eligible(d)) return YB_OK;   // configured by patch_conv_configure
   // Three layouts, tried in this order:
   //   two CTAs of two consumer warpgroups (104 registers) when the shape has such an instance;
   //   otherwise two CTAs of ONE consumer warpgroup (64-row tiles, 232 registers) when the shape has that instance;
@@ -574,29 +520,24 @@ static int conv_configure(const yb_op_desc& d, ConvKernelParams& kp, dim3& grid,
 // shapes without a 104-register two-CTA instance.
 static int conv_plan(const yb_op_desc& d, int ctas, int groups, ConvKernelParams& kp, dim3& grid, size_t& smem_bytes) {
   const int Ho = d.Ho, Wo = d.Wo;
-  const long long M_ll = static_cast<long long>(d.N) * Ho * Wo;
   const size_t budget = ctas == 2 ? smem_per_sm() / 2 - kSmemReservedPerCta - kStaticSmem : kSmemBudget;
   const int block_m = tile_rows(groups);
   kp = ConvKernelParams();
   kp.ctas = ctas;
   kp.groups = groups;
-  kp.M = static_cast<int>(M_ll);
+  kp.M = static_cast<int>(static_cast<long long>(d.N) * Ho * Wo);
   kp.ep.Cout = d.Cout;
   const int m_tiles = (kp.M + block_m - 1) / block_m;
   const int sms = num_sms();
-  // N tile: the whole Cout up to 256 columns (fewest A re-reads); halve it when that leaves fewer
-  // than two 128-row tiles per SM so the persistent grid balances better (the same N tile in every layout).
-  int n_tiles = (d.Cout + kMaxBlockN - 1) / kMaxBlockN;
-  int block_n = mma_n((d.Cout + n_tiles - 1) / n_tiles);
   const int m_tiles128 = (kp.M + tile_rows(2) - 1) / tile_rows(2);
-  if (m_tiles128 * n_tiles < 2 * sms && block_n > 128 && d.chain == nullptr) block_n /= 2;
+  int block_n = conv_block_n(d.Cout, m_tiles128, d.chain != nullptr);   // the same N tile in every layout
   if (groups == 1) {
     // one consumer warpgroup: only layers whose one-CTA plan has a 256-column N tile, split into two 128-column ones,
     // with at least 3 x SMs 128-row tiles (DESIGN.md section 3: measured gains at 400 and 1600 such tiles, none at 100)
     if (block_n != 256 || d.chain != nullptr || m_tiles128 < 3 * sms) return YB_ERR_INVALID;
     block_n = 128;
   }
-  n_tiles = (d.Cout + block_n - 1) / block_n;
+  int n_tiles = (d.Cout + block_n - 1) / block_n;
   YB_REQUIRE(mma_n(block_n) == block_n && block_n <= kMaxBlockN, "conv: N tile %d is not a wgmma N", block_n);
   kp.block_n = block_n;
   kp.n_tiles = n_tiles;
@@ -651,31 +592,18 @@ static int conv_plan(const yb_op_desc& d, int ctas, int groups, ConvKernelParams
                kp.block_n, kp.ch.n2);
     chain_bytes = static_cast<size_t>(kp.ch.w2_chunks) * kp.ch.w2_sub_bytes;
   }
-  // Weights stay resident in shared memory when the layer has a single N tile and they are small:
-  // the persistent CTA then streams only activations (halves the L2->SM traffic of the shallow layers).  A one-group
-  // plan (grid 2 x SMs) also keeps them resident over several N tiles when the grid is a multiple of the N tiles: every
-  // CTA then has one N tile and holds its weights.
+  // A one-group plan (grid 2 x SMs) also keeps the weights resident over several N tiles when the grid is a multiple of
+  // the N tiles: every CTA then has one N tile and holds its weights.
   const size_t fixed = static_cast<size_t>(kStageBufs) * stage_buf_bytes(groups) + 1024 + chain_bytes;
-  const size_t b_total = static_cast<size_t>(kp.num_k_iters) * kp.b_stage_bytes;
   const bool fixed_n = n_tiles == 1 || (groups == 1 && (2 * sms) % n_tiles == 0);
-  kp.b_resident = (fixed_n && b_total <= 80 * 1024) ? 1 : 0;
-  kp.b_res_bytes = kp.b_resident ? static_cast<uint32_t>(b_total) : 0u;
-  // k-iterations per pipeline stage: aim at ~32 KB per stage so that one mbarrier round trip moves
-  // enough bytes (a 16-channel tap is only 4 KB), in near-equal groups.
-  const uint32_t per_iter = kp.a_stage_bytes + (kp.b_resident ? 0u : kp.b_stage_bytes);
-  YB_REQUIRE(budget > fixed + kp.b_res_bytes + 2 * per_iter, "conv: shared memory budget exceeded (block_n=%d)", kp.block_n);
-  const size_t avail = budget - fixed - kp.b_res_bytes;
-  const size_t target = avail / 3 < 32 * 1024 ? avail / 3 : 32 * 1024;   // keep at least three stages in flight
-  int kpg_max = static_cast<int>(target / per_iter);
-  if (kpg_max < 1) kpg_max = 1;
-  if (kpg_max > kp.num_k_iters) kpg_max = kp.num_k_iters;
-  const int kgroups = (kp.num_k_iters + kpg_max - 1) / kpg_max;
-  kp.kpg = (kp.num_k_iters + kgroups - 1) / kgroups;
-  const uint32_t stage_bytes = kp.kpg * per_iter;
-  int stages = static_cast<int>(avail / stage_bytes);
-  if (stages > kMaxStages) stages = kMaxStages;
-  if (stages < 2) stages = 2;
-  kp.stages = stages;
+  KPipeline pipe;
+  const int rc = size_k_pipeline(budget, fixed, kp.a_stage_bytes, kp.b_stage_bytes, kp.num_k_iters, fixed_n, kMaxStages,
+                                 "conv", kp.block_n, &pipe);
+  if (rc != YB_OK) return rc;
+  kp.b_resident = pipe.b_resident;
+  kp.b_res_bytes = pipe.b_res_bytes;
+  kp.kpg = pipe.kpg;
+  kp.stages = pipe.stages;
   kp.ep.is_bf16 = d.dtype == YB_BF16;
   kp.ep.act = d.act;
   kp.bias = d.bias;
@@ -690,184 +618,90 @@ static int conv_plan(const yb_op_desc& d, int ctas, int groups, ConvKernelParams
   }
   const int max_grid = ctas * sms;   // a grid that is not a multiple of the N tiles loads the bias per tile
   grid = dim3(kp.num_tiles < max_grid ? kp.num_tiles : max_grid, 1, 1);
-  const size_t smem = static_cast<size_t>(stages) * stage_bytes + kp.b_res_bytes + fixed;
-  YB_REQUIRE(smem <= budget, "conv: %zu bytes of shared memory needed, %zu available", smem, budget);
-  smem_bytes = smem;
+  smem_bytes = pipe.smem;
   return YB_OK;
 }
 
-int conv_configure_check(const yb_op_desc& d, int* info) {
+int im2col_conv_config(const yb_op_desc& d, yb_conv_info* info) {
   ConvKernelParams kp;
   dim3 grid;
   size_t smem = 0;
   const int rc = conv_configure(d, kp, grid, smem);
-  if (rc == YB_OK && info && !patch_conv_eligible(d)) {   // yb_conv_config: see include/yolort_b200.h
-    info[0] = 0;
-    info[1] = kp.block_n;
-    info[2] = kp.n_tiles;
-    info[3] = kp.b_resident;
-    info[4] = 1;
-    info[5] = kp.stages;
-    info[6] = kp.kpg;
-    info[7] = kp.store_cols;
-    info[8] = kp.groups;          // (im2col / 1x1 kernel: consumer warpgroups; they share two staging buffers)
-    info[9] = static_cast<int>(smem);
-    info[10] = static_cast<int>(grid.x);
-    // bit 1: two CTAs of the 104-register instances; bit 2: two CTAs of one consumer warpgroup
-    info[11] = kp.ch.on | (kp.ctas == 2 ? (kp.groups == 2 ? 2 : 4) : 0);
+  if (rc == YB_OK && info) {   // yb_conv_config: see include/yolort_b200.h
+    info->kernel = YB_CONV_KERNEL_IM2COL;
+    info->block_n = kp.block_n;
+    info->n_tiles = kp.n_tiles;
+    info->weights_resident = kp.b_resident;
+    info->tiles_per_pass = 1;
+    info->slots = kp.stages;
+    info->ring = kp.kpg;
+    info->store_cols = kp.store_cols;
+    info->store_bufs = kStageBufs;   // shared by the consumer warpgroups
+    info->groups = kp.groups;
+    info->resident_ctas = kp.ctas;
+    info->chained = kp.ch.on;
+    info->smem_bytes = static_cast<int>(smem);
+    info->grid = static_cast<int>(grid.x);
+    info->tiling = YB_CONV_TILING_ROWS;
+    info->m_tiles = kp.num_tiles / kp.n_tiles;
+    info->work_items = kp.num_tiles;
+    info->tail_n = kp.ch.n2;
   }
   return rc;
 }
 
-int conv_op_create(const yb_op_desc& d, ConvOp** out) {
-  int rc = load_driver_entry_points();
-  if (rc != YB_OK) return rc;
-  ConvOp* op = new ConvOp();
-  rc = conv_configure(d, op->kp, op->grid, op->smem_bytes);
-  if (rc != YB_OK) {
-    delete op;
-    return rc;
-  }
-  if (patch_conv_eligible(d)) {
-    rc = patch_conv_create(d, g_encode_tiled, &op->patch);
-    if (rc != YB_OK) {
-      delete op;
-      return rc;
-    }
-    *out = op;
+struct Im2colConvOp final : ConvOp {
+  CUtensorMap tmap_a, tmap_b, tmap_out, tmap_w2, tmap_out2;
+  ConvKernelParams kp;
+  ConvKernelFn fn = nullptr;
+  dim3 grid;
+  size_t smem_bytes;
+  int launch(cudaStream_t stream) const override {
+    YB_CHECK_CUDA(launch_pdl(fn, grid, dim3(cta_threads(kp.groups)), smem_bytes, stream, tmap_a, tmap_b, tmap_out, tmap_w2,
+                             tmap_out2, kp));
     return YB_OK;
   }
-  ConvKernelParams& kp = op->kp;
-  const int Ho = d.Ho, Wo = d.Wo;
-  (void)Ho; (void)Wo;
-  const cuuint32_t block_m = tile_rows(kp.groups);   // rows of the A, output and tail-output boxes
+};
 
-  const CUtensorMapDataType dt =
-      kp.ep.is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  const CUtensorMapSwizzle sw = swizzle_for_row_bytes(kp.block_k * 2);
-  CUresult cr;
-  if (kp.mode == 0) {
-    cuuint64_t dims[2] = {static_cast<cuuint64_t>(d.Cin), static_cast<cuuint64_t>(kp.M)};
-    cuuint64_t strides[1] = {static_cast<cuuint64_t>(d.in_cstride) * 2};
-    cuuint32_t box[2] = {static_cast<cuuint32_t>(kp.block_k), block_m};
-    cuuint32_t estr[2] = {1, 1};
-    cr = g_encode_tiled(&op->tmap_a, dt, 2, const_cast<void*>(d.in), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  } else {
-    cuuint64_t dims[4] = {static_cast<cuuint64_t>(d.Cin), static_cast<cuuint64_t>(d.W),
-                          static_cast<cuuint64_t>(d.H), static_cast<cuuint64_t>(d.N)};
-    cuuint64_t strides[3] = {static_cast<cuuint64_t>(d.in_cstride) * 2,
-                             static_cast<cuuint64_t>(d.in_cstride) * 2 * d.W,
-                             static_cast<cuuint64_t>(d.in_cstride) * 2 * d.W * d.H};
-    int lower[2] = {-d.pad, -d.pad};
-    int upper[2] = {d.pad - (d.ksize - 1), d.pad - (d.ksize - 1)};
-    cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(d.stride), static_cast<cuuint32_t>(d.stride), 1};
-    cr = g_encode_im2col(&op->tmap_a, dt, 4, const_cast<void*>(d.in), dims, strides, lower, upper,
-                         static_cast<cuuint32_t>(kp.block_k), block_m, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    // Driver workaround also applied by CUTLASS (copy_traits_sm90_im2col.hpp): for tensors smaller
-    // than 128 KiB, drivers <= 13.1 set a descriptor bit that makes im2col loads fault.
-    int drv = 0;
-    cudaDriverGetVersion(&drv);
-    const size_t span = static_cast<size_t>(d.in_cstride) * 2 * d.W * d.H * d.N;
-    if (cr == CUDA_SUCCESS && drv <= 13010 && span < 131072) {
-      reinterpret_cast<uint64_t*>(&op->tmap_a)[1] &= ~(1ull << 21);
-    }
-  }
-  if (cr != CUDA_SUCCESS) {
-    set_error("conv: cuTensorMapEncode (A, mode %d) failed with CUresult %d (Cin=%d cs=%d H=%d W=%d N=%d k=%d s=%d bk=%d)",
-              kp.mode, static_cast<int>(cr), d.Cin, d.in_cstride, d.H, d.W, d.N, d.ksize, d.stride,
-              kp.block_k);
-    delete op;
-    return YB_ERR_CUDA;
-  }
-  {
-    const int ktot = d.ksize * d.ksize * d.Cin_pad;
-    cuuint64_t dims[2] = {static_cast<cuuint64_t>(ktot), static_cast<cuuint64_t>(d.Cout_pad)};
-    cuuint64_t strides[1] = {static_cast<cuuint64_t>(ktot) * 2};
-    cuuint32_t box[2] = {static_cast<cuuint32_t>(kp.block_k), static_cast<cuuint32_t>(kp.block_n)};
-    cuuint32_t estr[2] = {1, 1};
-    cr = g_encode_tiled(&op->tmap_b, dt, 2, const_cast<void*>(d.weight), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) {
-      set_error("conv: cuTensorMapEncodeTiled (weights) failed with CUresult %d", static_cast<int>(cr));
-      delete op;
-      return YB_ERR_CUDA;
-    }
-  }
-  {
-    // destination view [M rows, Cout channels], row pitch = out_cstride; boxes of block_m rows x store_cols
-    cuuint64_t dims[2] = {static_cast<cuuint64_t>(d.Cout), static_cast<cuuint64_t>(kp.M)};
-    cuuint64_t strides[1] = {static_cast<cuuint64_t>(d.out_cstride) * 2};
-    cuuint32_t box[2] = {static_cast<cuuint32_t>(kp.store_cols), block_m};
-    cuuint32_t estr[2] = {1, 1};
-    cr = g_encode_tiled(&op->tmap_out, dt, 2, d.out, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        swizzle_for_row_bytes(kp.store_cols * 2), CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) {
-      set_error("conv: cuTensorMapEncodeTiled (output) failed with CUresult %d", static_cast<int>(cr));
-      delete op;
-      return YB_ERR_CUDA;
-    }
-  }
+int im2col_conv_create(const yb_op_desc& d, ConvOp** out) {
+  Im2colConvOp* op = new Im2colConvOp();
+  ConvKernelParams& kp = op->kp;
+  int rc = conv_configure(d, kp, op->grid, op->smem_bytes);
+  const uint32_t block_m = tile_rows(kp.groups);   // rows of the A, output and tail-output boxes
+  const CUtensorMapDataType dt = kp.ep.is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  if (rc == YB_OK)
+    rc = kp.mode == 0 ? tmap_matrix(&op->tmap_a, "conv input", dt, d.in, d.Cin, kp.M, d.in_cstride, kp.block_k, block_m,
+                                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B)
+                      : tmap_im2col(&op->tmap_a, "conv input", dt, d, kp.block_k, block_m);
+  const int ktot = d.ksize * d.ksize * d.Cin_pad;
+  if (rc == YB_OK)
+    rc = tmap_matrix(&op->tmap_b, "conv weights", dt, d.weight, ktot, d.Cout_pad, ktot, kp.block_k, kp.block_n,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  // destination view [M rows, Cout channels], row pitch = out_cstride; boxes of block_m rows x store_cols
+  if (rc == YB_OK)
+    rc = tmap_matrix(&op->tmap_out, "conv output", dt, d.out, d.Cout, kp.M, d.out_cstride, kp.store_cols, block_m,
+                     CU_TENSOR_MAP_L2_PROMOTION_NONE);
   op->tmap_w2 = op->tmap_b;      // placeholders when nothing is chained (never dereferenced)
   op->tmap_out2 = op->tmap_out;
-  if (kp.ch.on) {
+  if (rc == YB_OK && kp.ch.on) {
     const yb_conv_chain& c = *d.chain;
-    const int kc = kp.ch.w2_row_bytes / 2;
-    cuuint64_t wdims[2] = {static_cast<cuuint64_t>(c.K_pad), static_cast<cuuint64_t>(c.Cout_pad)};
-    cuuint64_t wstrides[1] = {static_cast<cuuint64_t>(c.K_pad) * 2};
-    cuuint32_t wbox[2] = {static_cast<cuuint32_t>(kc), static_cast<cuuint32_t>(kp.ch.n2)};
-    cuuint32_t estr[2] = {1, 1};
-    cr = g_encode_tiled(&op->tmap_w2, dt, 2, const_cast<void*>(c.weight), wdims, wstrides, wbox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        swizzle_for_row_bytes(kc * 2), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr == CUDA_SUCCESS) {
-      const int s2 = chain_store2_cols(kp.ch.n2);
-      cuuint64_t odims[2] = {static_cast<cuuint64_t>(c.Cout), static_cast<cuuint64_t>(kp.M)};
-      cuuint64_t ostrides[1] = {static_cast<cuuint64_t>(c.out_cstride) * 2};
-      cuuint32_t obox[2] = {static_cast<cuuint32_t>(s2), block_m};
-      cr = g_encode_tiled(&op->tmap_out2, dt, 2, c.out, odims, ostrides, obox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                          swizzle_for_row_bytes(s2 * 2), CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    }
-    if (cr != CUDA_SUCCESS) {
-      set_error("conv: cuTensorMapEncodeTiled (chained tail) failed with CUresult %d", static_cast<int>(cr));
-      delete op;
-      return YB_ERR_CUDA;
-    }
+    rc = tmap_matrix(&op->tmap_w2, "conv chained tail weights", dt, c.weight, c.K_pad, c.Cout_pad, c.K_pad,
+                     kp.ch.w2_row_bytes / 2, kp.ch.n2, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+    if (rc == YB_OK)
+      rc = tmap_matrix(&op->tmap_out2, "conv chained tail output", dt, c.out, c.Cout, kp.M, c.out_cstride,
+                       chain_store2_cols(kp.ch.n2), block_m, CU_TENSOR_MAP_L2_PROMOTION_NONE);
   }
-  op->fn = select_conv_kernel(kp);
-  rc = set_smem_attributes(reinterpret_cast<const void*>(op->fn), kSmemBudget, kp.ctas, op->smem_bytes, cta_threads(kp.groups),
-                           "conv");
+  if (rc == YB_OK) {
+    op->fn = select_conv_kernel(kp);
+    rc = set_smem_attributes(reinterpret_cast<const void*>(op->fn), kSmemBudget, kp.ctas, op->smem_bytes,
+                             cta_threads(kp.groups), "conv");
+  }
   if (rc != YB_OK) {
     delete op;
     return rc;
   }
   *out = op;
   return YB_OK;
-}
-
-int conv_op_launch(const ConvOp* op, cudaStream_t stream) {
-  if (op->patch) return patch_conv_launch(op->patch, stream);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = op->grid;
-  cfg.blockDim = dim3(cta_threads(op->kp.groups), 1, 1);
-  cfg.dynamicSmemBytes = op->smem_bytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  YB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, op->fn, op->tmap_a, op->tmap_b, op->tmap_out, op->tmap_w2, op->tmap_out2, op->kp));
-  return YB_OK;
-}
-
-void conv_op_destroy(ConvOp* op) {
-  if (op && op->patch) patch_conv_destroy(op->patch);
-  delete op;
 }
 
 }  // namespace yb

@@ -1,45 +1,34 @@
-// Host-side handle of one prepared convolution launch (tensor maps + kernel parameters).
+// Host-side handles of the prepared launches (tensor maps + kernel parameters) and the plan ops' entry points.
 #pragma once
-#include <cuda_runtime.h>
-
-#include "../../include/yolort_b200.h"
-
-#include <cuda.h>
+#include "host_sm90.h"
 
 namespace yb {
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+// One prepared convolution launch, on whichever kernel conv_kernel picks.
+struct ConvOp {
+  virtual ~ConvOp() = default;
+  virtual int launch(cudaStream_t stream) const = 0;
+};
+
+// The one choice of a convolution kernel (YB_CONV_KERNEL_*): e4m3 for YB_F8E4M3, else the halo-patch kernel for the
+// shapes patch_conv_eligible admits, else 1x1 / im2col.
+int conv_kernel(const yb_op_desc& d);
+int conv_config(const yb_op_desc& d, yb_conv_info* info);   // host-only validation + tiling (no driver calls)
+int conv_create(const yb_op_desc& d, ConvOp** out);
+
+// fp16 / bf16 validation shared by the 1x1 / im2col and halo-patch kernels; 1x1 / im2col kernel (conv_sm90.cu)
+int conv_validate(const yb_op_desc& d);
+int im2col_conv_config(const yb_op_desc& d, yb_conv_info* info);
+int im2col_conv_create(const yb_op_desc& d, ConvOp** out);
 
 // 3x3/s1 halo-patch variant (conv3x3_patch_sm90.cu)
-struct PatchConvOp;
 bool patch_conv_eligible(const yb_op_desc& d);
-int patch_conv_create(const yb_op_desc& d, EncodeTiledFn encode_tiled, PatchConvOp** out);
-int patch_conv_configure_check(const yb_op_desc& d, int* info = nullptr);   // host-only validation + tiling (no driver calls)
-int patch_conv_launch(const PatchConvOp* op, cudaStream_t stream);
-void patch_conv_destroy(PatchConvOp* op);
-
-struct ConvOp;
-int conv_op_create(const yb_op_desc& d, ConvOp** out);
-int conv_configure_check(const yb_op_desc& d, int* info = nullptr);         // host-only validation + tiling (no driver calls)
-int conv_op_launch(const ConvOp* op, cudaStream_t stream);
-void conv_op_destroy(ConvOp* op);
-
-typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                   const cuuint64_t*, const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*,
-                                   CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
-                                   CUtensorMapFloatOOBfill);
-
-// cuTensorMapEncodeTiled / cuTensorMapEncodeIm2col from the driver (looked up once)
-int encode_tiled_entry(EncodeTiledFn* out);
-int encode_im2col_entry(EncodeIm2colFn* out);
+int patch_conv_config(const yb_op_desc& d, yb_conv_info* info);
+int patch_conv_create(const yb_op_desc& d, ConvOp** out);
 
 // e4m3 convolution and the fp16/bf16 -> e4m3 quantisation op (conv_fp8_sm90.cu)
-struct Fp8ConvOp;
-int fp8_conv_configure_check(const yb_op_desc& d, int* info = nullptr);   // host-only validation + tiling (no driver calls)
-int fp8_conv_op_create(const yb_op_desc& d, Fp8ConvOp** out);
-int fp8_conv_op_launch(const Fp8ConvOp* op, cudaStream_t stream);
-void fp8_conv_op_destroy(Fp8ConvOp* op);
+int fp8_conv_config(const yb_op_desc& d, yb_conv_info* info);
+int fp8_conv_create(const yb_op_desc& d, ConvOp** out);
 int quantize_configure_check(const yb_op_desc& d);                         // host-only validation (no driver calls)
 int quantize_launch(const yb_op_desc& d, cudaStream_t stream);
 

@@ -416,29 +416,14 @@ extern "C" int yb_conv_wgrad(const yb_wgrad_problem* problems, int n, void* work
     set_error("conv_wgrad: workspace of %zu bytes (16-byte aligned) needed, got %zu", need, workspace_bytes);
     return YB_ERR_WORKSPACE;
   }
-  EncodeTiledFn encode = nullptr;
-  rc = encode_tiled_entry(&encode);
-  if (rc != YB_OK) return rc;
   const CUtensorMapDataType dt = problems[0].dtype == YB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  for (int q = 0; q < n; ++q) {
+  for (int q = 0; q < n && rc == YB_OK; ++q) {
     const yb_wgrad_problem& a = problems[q];
-    cuuint32_t box[2] = {64, static_cast<cuuint32_t>(kPx)};
-    cuuint32_t estr[2] = {1, 1};
-    cuuint64_t dims[2] = {static_cast<cuuint64_t>(a.Cout), static_cast<cuuint64_t>(a.P)};
-    cuuint64_t strides[1] = {static_cast<cuuint64_t>(a.dy_stride) * 2};
-    CUresult cr = encode(&kp.dy[q], dt, 2, const_cast<void*>(a.dy), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr == CUDA_SUCCESS) {
-      cuuint64_t xdims[2] = {static_cast<cuuint64_t>(a.Cin), static_cast<cuuint64_t>(a.P)};
-      cuuint64_t xstrides[1] = {static_cast<cuuint64_t>(a.x_stride) * 2};
-      cr = encode(&kp.x[q], dt, 2, const_cast<void*>(a.x), xdims, xstrides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    }
-    if (cr != CUDA_SUCCESS) {
-      set_error("conv_wgrad: problem %d: cuTensorMapEncodeTiled failed with CUresult %d", q, static_cast<int>(cr));
-      return YB_ERR_CUDA;
-    }
+    rc = tmap_matrix(&kp.dy[q], "conv_wgrad: dy", dt, a.dy, a.Cout, a.P, a.dy_stride, 64, kPx, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+    if (rc == YB_OK)
+      rc = tmap_matrix(&kp.x[q], "conv_wgrad: x", dt, a.x, a.Cin, a.P, a.x_stride, 64, kPx, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
   }
+  if (rc != YB_OK) return rc;
   kp.ws = static_cast<float*>(workspace_dev);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const bool bf16 = problems[0].dtype == YB_BF16;

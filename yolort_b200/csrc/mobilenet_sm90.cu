@@ -275,15 +275,6 @@ int dwconv_launch(const yb_op_desc& d, cudaStream_t stream) {
   p.in_cs = d.in_cstride, p.out_cs = d.out_cstride, p.act = d.act;
   p.xgroups = (d.Wo + kDwPix - 1) / kDwPix;
   const long long total = static_cast<long long>(d.N) * d.Ho * p.xgroups * (d.Cin >> 3);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(static_cast<unsigned>((total + kDwThreads - 1) / kDwThreads));
-  cfg.blockDim = dim3(kDwThreads);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
   using Fn = void (*)(const DwParams);
   static const Fn table[2][3][2] = {
       {{dwconv_kernel<false, 1, 1>, dwconv_kernel<false, 1, 2>}, {dwconv_kernel<false, 3, 1>, dwconv_kernel<false, 3, 2>},
@@ -291,7 +282,7 @@ int dwconv_launch(const yb_op_desc& d, cudaStream_t stream) {
       {{dwconv_kernel<true, 1, 1>, dwconv_kernel<true, 1, 2>}, {dwconv_kernel<true, 3, 1>, dwconv_kernel<true, 3, 2>},
        {dwconv_kernel<true, 5, 1>, dwconv_kernel<true, 5, 2>}}};
   const Fn fn = table[d.dtype == YB_BF16 ? 1 : 0][d.ksize / 2][d.stride - 1];
-  YB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, fn, p));
+  YB_CHECK_CUDA(launch_pdl(fn, dim3(static_cast<unsigned>((total + kDwThreads - 1) / kDwThreads)), dim3(kDwThreads), 0, stream, p));
   return YB_OK;
 }
 
@@ -303,20 +294,8 @@ int se_launch(const yb_op_desc& d, cudaStream_t stream) {
   p.w2t = p.w1t + static_cast<long long>(p.C) * p.S;
   p.b1 = d.bias;
   p.b2 = d.bias + p.S;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(kSeCtas, static_cast<unsigned>(d.N));
-  cfg.blockDim = dim3(kSeThreads);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = kSeCtas;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 2;
-  YB_CHECK_CUDA(d.dtype == YB_BF16 ? cudaLaunchKernelEx(&cfg, se_kernel<true>, p) : cudaLaunchKernelEx(&cfg, se_kernel<false>, p));
+  YB_CHECK_CUDA(launch_pdl_cluster(kSeCtas, d.dtype == YB_BF16 ? se_kernel<true> : se_kernel<false>,
+                                   dim3(kSeCtas, static_cast<unsigned>(d.N)), dim3(kSeThreads), 0, stream, p));
   return YB_OK;
 }
 

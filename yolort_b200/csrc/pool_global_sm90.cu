@@ -101,17 +101,9 @@ int avgpool_launch(const yb_op_desc& d, cudaStream_t stream) {
   p.in_cs = d.in_cstride, p.out_cs = d.out_cstride;
   p.octs = p.C8 < kOcts ? p.C8 : kOcts;
   p.lanes = kPoolThreads / p.octs;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(static_cast<unsigned>((p.C8 + p.octs - 1) / p.octs), static_cast<unsigned>(d.N));
-  cfg.blockDim = dim3(kPoolThreads);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  YB_CHECK_CUDA(d.dtype == YB_BF16 ? cudaLaunchKernelEx(&cfg, avgpool_kernel<true>, p)
-                                   : cudaLaunchKernelEx(&cfg, avgpool_kernel<false>, p));
+  YB_CHECK_CUDA(launch_pdl(d.dtype == YB_BF16 ? avgpool_kernel<true> : avgpool_kernel<false>,
+                           dim3(static_cast<unsigned>((p.C8 + p.octs - 1) / p.octs), static_cast<unsigned>(d.N)),
+                           dim3(kPoolThreads), 0, stream, p));
   return YB_OK;
 }
 
