@@ -78,6 +78,13 @@ int yb_letterbox_strided(int n, const void* const* src_dev, int src_dtype, int s
                          const yb_letterbox_geom* geom, int Hb, int Wb, float fill, const float* u8_lut_dev,
                          void* dst_dev, int dst_dtype, int dst_layout, void* stream);
 
+/* One test-time-augmentation canvas (scale_img, yolort/v5/utils/torch_utils.py:288-300, of the canvas or of its
+ * left-right mirror): n space-to-depth canvases [n, Hb/2, Wb/2, 16] (fp16 or bf16) -> [n, Hp/2, Wp/2, 16] of the same
+ * dtype.  Pixels [0, nh) x [0, nw) are the bilinear resize (align_corners=False, ratios float(Hb)/nh, float(Wb)/nw,
+ * fp32 arithmetic, one rounding) of the canvas, mirrored when flip_lr; the rest is `fill`; channel 3 is zero. */
+int yb_canvas_rescale(int n, const void* src_dev, int dtype, int Hb, int Wb, int nh, int nw, int flip_lr, float fill,
+                      void* dst_dev, int Hp, int Wp, void* stream);
+
 /* Host-only: scale_coords parameters of transform.py:354-367 for one image:
  * out[0]=gain, out[1]=pad_x, out[2]=pad_y (all fp32, fractional pads). */
 int yb_scale_coords_params(int Hb, int Wb, int src_h, int src_w, float* out3);
@@ -367,6 +374,27 @@ int yb_nms_finish(const yb_nms_params* p, const yb_head_level* levels, const flo
  * split exists so that a caller can time (or overlap) the three steps separately. */
 int yb_decode_candidates(const yb_nms_params* p, const yb_head_level* levels, void* workspace_dev,
                          size_t workspace_bytes, void* stream);
+
+/* Test-time augmentation (YOLOv5's `augment=True`, yolort/v5/models/yolo.py:152-208): the head logits of up to
+ * YB_TTA_MAX_PASSES plan runs over rescaled / mirrored canvases decoded into ONE candidate arena per image and
+ * suppressed together.  A pass lists the level slices that take part, in order (the reference's _clip_augmented drops
+ * the last level of pass 0 and the first level of pass 2: leave those out).  Every box is decoded, then
+ * (cx, cy, w, h) /= scale (fp32 division) and, for a mirrored pass, cx = canvas_w - cx, then converted to corners.
+ * Candidate index = (kept anchor over all passes in the order given) * n_classes + class; it must fit 32 bits.
+ * The levels must be the plan's NHWC head buffers (16-bit logits, rows of <= 512 bytes).  `p->n_levels` is not read.
+ * Outputs, status words and the overflow rule are those of yb_decode_nms. */
+#define YB_TTA_MAX_PASSES 3
+typedef struct {
+  int32_t n_levels;        /* level slices of this pass that take part (<= YB_MAX_LEVELS)            */
+  int32_t flip_lr;         /* 1: the pass ran on the left-right mirrored canvas                      */
+  float scale;             /* the pass's canvas scale s                                              */
+  float canvas_w;          /* Wb, width of the unscaled canvas (un-mirroring: cx = Wb - cx)          */
+  yb_head_level levels[YB_MAX_LEVELS];
+} yb_tta_pass;
+size_t yb_decode_nms_tta_workspace_bytes(const yb_nms_params* p, int n_passes, const yb_tta_pass* passes);
+int yb_decode_nms_tta(const yb_nms_params* p, int n_passes, const yb_tta_pass* passes, const float* rescale_dev,
+                      float* boxes_dev, float* scores_dev, int64_t* labels_dev, int32_t* counts_dev, int64_t* status_dev,
+                      void* workspace_dev, size_t workspace_bytes, void* stream);
 
 /* Dense decode, no threshold / NMS (replaces LogitsDecoder.forward: yolort/relay/logits_decoder.py:26-61, the
  * output the reference hands to TensorRT's EfficientNMS plugin): boxes_dev [n_images, anchors_per_image, 4] fp32

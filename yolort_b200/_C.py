@@ -36,6 +36,7 @@ EXPORTED_SYMBOLS = (
     "yb_letterbox_geometry",
     "yb_letterbox",
     "yb_letterbox_strided",
+    "yb_canvas_rescale",
     "yb_scale_coords_params",
     "yb_conv_chain_supported",
     "yb_conv_config",
@@ -48,6 +49,8 @@ EXPORTED_SYMBOLS = (
     "yb_decode_nms_debug_offset",
     "yb_decode_nms",
     "yb_decode_dense",
+    "yb_decode_nms_tta_workspace_bytes",
+    "yb_decode_nms_tta",
     "yb_nms_layout",
     "yb_nms_begin",
     "yb_nms_finish",
@@ -152,6 +155,17 @@ class HeadLevel(ctypes.Structure):
         ("stride_y", ctypes.c_int64), ("stride_x", ctypes.c_int64),
         ("stride_px", ctypes.c_float),
         ("anchors_px", ctypes.c_float * (2 * YB_MAX_ANCHORS)),
+    ]
+
+
+YB_TTA_MAX_PASSES = 3
+
+
+class TtaPass(ctypes.Structure):
+    _fields_ = [
+        ("n_levels", ctypes.c_int32), ("flip_lr", ctypes.c_int32),
+        ("scale", ctypes.c_float), ("canvas_w", ctypes.c_float),
+        ("levels", HeadLevel * YB_MAX_LEVELS),
     ]
 
 
@@ -317,6 +331,12 @@ def lib() -> ctypes.CDLL:
         ctypes.POINTER(NmsParams), ctypes.POINTER(HeadLevel), ctypes.c_void_p, ctypes.c_void_p,
         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
         ctypes.c_size_t, ctypes.c_void_p]
+    L.yb_canvas_rescale.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_int] * 5 + [
+        ctypes.c_float, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
+    L.yb_decode_nms_tta_workspace_bytes.restype = ctypes.c_size_t
+    L.yb_decode_nms_tta_workspace_bytes.argtypes = [ctypes.POINTER(NmsParams), ctypes.c_int, ctypes.POINTER(TtaPass)]
+    L.yb_decode_nms_tta.argtypes = [ctypes.POINTER(NmsParams), ctypes.c_int, ctypes.POINTER(TtaPass)] + \
+        [ctypes.c_void_p] * 7 + [ctypes.c_size_t, ctypes.c_void_p]
     L.yb_decode_dense.argtypes = [ctypes.POINTER(NmsParams), ctypes.POINTER(HeadLevel), ctypes.c_void_p,
                                   ctypes.c_void_p, ctypes.c_void_p]
     L.yb_nms_layout.argtypes = [ctypes.POINTER(NmsParams), ctypes.POINTER(HeadLevel), ctypes.c_void_p, ctypes.c_size_t,
@@ -753,6 +773,113 @@ class FusedPost:
                                       scores.data_ptr(), labels.data_ptr(), counts.data_ptr(), self.status.data_ptr(),
                                       self.ws.data_ptr(), self.ws.numel(), current_stream_ptr(dev)), "yb_nms_finish")
         return boxes, scores, labels, counts, self.status
+
+
+# ---------------------------------------------------------------------------------------------------
+# test-time augmentation (yolort/v5/models/yolo.py:152-208)
+# ---------------------------------------------------------------------------------------------------
+TTA_SCALES = (1.0, 0.83, 0.67)      # _forward_augment's fixed lists (yolo.py:154-155): scale, left-right mirror
+TTA_FLIPS = (False, True, False)
+TTA_FILL = 0.447                    # scale_img's pad value (torch_utils.py:300)
+
+
+def tta_pass_geometry(Hb: int, Wb: int, gs: int) -> List[Tuple[int, int, int, int]]:
+    """(nh, nw, Hp, Wp) per pass: scale_img (torch_utils.py:288-300) of an Hb x Wb canvas, resized to
+    int(H * s) x int(W * s) and padded to ceil(H * s / gs) * gs x ceil(W * s / gs) * gs (Python doubles, as the
+    reference); scale 1 is the canvas itself."""
+    out = []
+    for s in TTA_SCALES:
+        if s == 1.0:
+            out.append((Hb, Wb, Hb, Wb))
+            continue
+        out.append((int(Hb * s), int(Wb * s), math.ceil(Hb * s / gs) * gs, math.ceil(Wb * s / gs) * gs))
+    return out
+
+
+def canvas_rescale(src: torch.Tensor, dst: torch.Tensor, nh: int, nw: int, flip_lr: bool, fill: float = TTA_FILL) -> torch.Tensor:
+    """One pass canvas: src [N, Hb/2, Wb/2, 16] space-to-depth (fp16 / bf16) -> dst [N, Hp/2, Wp/2, 16], the bilinear
+    resize of the (mirrored) canvas to nh x nw at the top left, `fill` elsewhere (yb_canvas_rescale)."""
+    require_cuda(src, "canvas_rescale")
+    if src.dtype != dst.dtype or src.dim() != 4 or dst.dim() != 4 or src.shape[3] != 16 or dst.shape[3] != 16 \
+            or src.shape[0] != dst.shape[0] or not src.is_contiguous() or not dst.is_contiguous():
+        raise NativeLibraryError(f"canvas_rescale: expected two contiguous [N,H/2,W/2,16] canvases of one dtype, got "
+                                 f"{tuple(src.shape)} {src.dtype} -> {tuple(dst.shape)} {dst.dtype}")
+    n, h2, w2, _ = src.shape
+    _, hp2, wp2, _ = dst.shape
+    dev = src.device
+    with device_guard(dev):
+        check(lib().yb_canvas_rescale(int(n), src.data_ptr(), dtype_code(src.dtype), 2 * int(h2), 2 * int(w2), int(nh),
+                                      int(nw), int(bool(flip_lr)), float(fill), dst.data_ptr(), 2 * int(hp2),
+                                      2 * int(wp2), current_stream_ptr(dev)), "yb_canvas_rescale")
+    return dst
+
+
+_tta_arenas: Dict[torch.device, _NmsArena] = {}
+
+
+def decode_nms_tta_padded(passes, canvas_w: int, strides: Sequence[float], anchors_px: Sequence[Sequence[float]],
+                          num_classes: int, score_thresh: float, nms_thresh: float, detections_per_img: int,
+                          semantics: int = NMS_TV_AUTO, rescale: Optional[torch.Tensor] = None):
+    """Multi-pass decode + one NMS per image.  `passes`: per pass (heads, level_ids, scale, flip_lr) with `heads` the
+    pass's NHWC head buffers and `level_ids` the levels that take part, in order.  Padded device outputs as
+    decode_nms_padded, without synchronising."""
+    t0 = passes[0][0][0]
+    require_cuda(t0, "decode_nms_tta")
+    dev = t0.device
+    n_images = int(t0.shape[0])
+    n_anchors = len(anchors_px[0]) // 2
+    if len(passes) > YB_TTA_MAX_PASSES or n_anchors > YB_MAX_ANCHORS:
+        raise NativeLibraryError("decode_nms_tta: too many passes/anchors")
+    arr = (TtaPass * len(passes))()
+    for q, (heads, level_ids, scale, flip) in enumerate(passes):
+        if len(level_ids) > YB_MAX_LEVELS:
+            raise NativeLibraryError("decode_nms_tta: too many levels")
+        arr[q].n_levels, arr[q].flip_lr = len(level_ids), int(bool(flip))
+        arr[q].scale, arr[q].canvas_w = float(scale), float(canvas_w)
+        for j, l in enumerate(level_ids):
+            require_cuda(heads[l], "decode_nms_tta")
+            arr[q].levels[j] = _level_struct(heads[l], "nhwc", n_anchors, num_classes + 5, strides[l], anchors_px[l])
+    arena = _tta_arenas.setdefault(dev, _NmsArena())
+    D = int(detections_per_img)
+    boxes = torch.empty((n_images, D, 4), dtype=torch.float32, device=dev)
+    scores = torch.empty((n_images, D), dtype=torch.float32, device=dev)
+    labels = torch.empty((n_images, D), dtype=torch.int64, device=dev)
+    counts = torch.empty((n_images,), dtype=torch.int32, device=dev)
+    status = torch.empty((4,), dtype=torch.int64, device=dev)
+    p = NmsParams(n_images, 0, n_anchors, int(num_classes), float(score_thresh), float(nms_thresh), D, int(semantics),
+                  int(arena.cap_per_image) * n_images)
+    need = lib().yb_decode_nms_tta_workspace_bytes(ctypes.byref(p), len(passes), arr)
+    if need == 0:
+        raise NativeLibraryError(f"yb_decode_nms_tta_workspace_bytes: {lib().yb_last_error().decode()}")
+    if arena.ws is None or arena.ws.numel() < need or arena.ws.device != dev:
+        arena.ws = None
+        arena.ws = torch.empty((need,), dtype=torch.uint8, device=dev)
+    with device_guard(dev):
+        check(lib().yb_decode_nms_tta(ctypes.byref(p), len(passes), arr, rescale.data_ptr() if rescale is not None else None,
+                                      boxes.data_ptr(), scores.data_ptr(), labels.data_ptr(), counts.data_ptr(),
+                                      status.data_ptr(), arena.ws.data_ptr(), arena.ws.numel(), current_stream_ptr(dev)),
+              "yb_decode_nms_tta")
+    return boxes, scores, labels, counts, status
+
+
+def decode_nms_tta(passes, canvas_w: int, strides, anchors_px, num_classes: int, score_thresh: float, nms_thresh: float,
+                   detections_per_img: int, semantics: int = NMS_TV_AUTO,
+                   rescale: Optional[torch.Tensor] = None) -> List[Dict[str, torch.Tensor]]:
+    """decode_nms_tta_padded + the reference's List[Dict]: one device->host read of counts + status; an image that
+    overflowed its share of the candidate arena grows it and re-runs (never truncates)."""
+    dev = passes[0][0][0].device
+    while True:
+        boxes, scores, labels, counts, status = decode_nms_tta_padded(
+            passes, canvas_w, strides, anchors_px, num_classes, score_thresh, nms_thresh, detections_per_img, semantics,
+            rescale)
+        host = torch.cat([counts.to(torch.int64), status]).tolist()
+        n = counts.numel()
+        if host[n + 1] == 0:
+            break
+        arena = _tta_arenas[dev]
+        arena.cap_per_image = max(2 * arena.cap_per_image, int(host[n + 2]))
+        arena.ws = None
+    return [{"scores": scores[i, :host[i]], "labels": labels[i, :host[i]], "boxes": boxes[i, :host[i]]} for i in range(n)]
 
 
 def batched_nms(boxes: torch.Tensor, scores: torch.Tensor, labels: torch.Tensor, iou_threshold: float,

@@ -47,4 +47,22 @@ __device__ __forceinline__ float4 decode_box(float sx, float sy, float sw, float
   return make_float4(__fsub_rn(cx, hw), __fsub_rn(cy, hh), __fadd_rn(cx, hw), __fadd_rn(cy, hh));
 }
 
+// The same box of a test-time-augmentation pass: (cx, cy, w, h) divided by the pass scale (IEEE fp32 division, as
+// `p[..., :4] /= scale`, v5/models/yolo.py:181), cx = Wb - cx for the mirrored pass (:185), then the corner conversion.
+__device__ __forceinline__ float4 decode_box_descaled(float sx, float sy, float sw, float sh, int x, int y, float stride_px,
+                                                      float aw, float ah, float scale, bool flip, float flip_w) {
+  float cx = __fmul_rn(__fadd_rn(__fsub_rn(__fmul_rn(sx, 2.0f), 0.5f), static_cast<float>(x)), stride_px);
+  float cy = __fmul_rn(__fadd_rn(__fsub_rn(__fmul_rn(sy, 2.0f), 0.5f), static_cast<float>(y)), stride_px);
+  const float tw = __fmul_rn(sw, 2.0f), th = __fmul_rn(sh, 2.0f);
+  float w = __fmul_rn(__fmul_rn(tw, tw), aw);
+  float h = __fmul_rn(__fmul_rn(th, th), ah);
+  cx = __fdiv_rn(cx, scale);
+  cy = __fdiv_rn(cy, scale);
+  w = __fdiv_rn(w, scale);
+  h = __fdiv_rn(h, scale);
+  if (flip) cx = __fsub_rn(flip_w, cx);
+  const float hw = __fmul_rn(0.5f, w), hh = __fmul_rn(0.5f, h);
+  return make_float4(__fsub_rn(cx, hw), __fsub_rn(cy, hh), __fadd_rn(cx, hw), __fadd_rn(cy, hh));
+}
+
 }  // namespace yb

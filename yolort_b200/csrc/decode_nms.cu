@@ -56,6 +56,7 @@ __device__ __forceinline__ float ld_logit<__nv_bfloat16>(const void* base, long 
 }
 
 struct DecodeParams {
+  static constexpr int kLevels = YB_MAX_LEVELS;
   yb_head_level lvl[YB_MAX_LEVELS];
   int lvl_start[YB_MAX_LEVELS + 1];  // first flat anchor index of each level
   int pix_start[YB_MAX_LEVELS + 1];  // first flat PIXEL index of each level (row kernel)
@@ -63,6 +64,23 @@ struct DecodeParams {
   int anchors_per_image;
   float score_thresh;
   long long cap_per_image;
+};
+
+// Multi-pass (test-time augmentation) decode: the kept level slices of up to YB_TTA_MAX_PASSES passes, in the order the
+// reference concatenates them (v5/models/yolo.py:161-162), each with its pass's descale (:180-185).
+constexpr int kTtaLevels = YB_TTA_MAX_PASSES * YB_MAX_LEVELS;
+struct TtaDecodeParams {
+  static constexpr int kLevels = kTtaLevels;
+  yb_head_level lvl[kTtaLevels];
+  int lvl_start[kTtaLevels + 1];
+  int pix_start[kTtaLevels + 1];
+  int n_images, n_levels, n_anchors, n_classes;
+  int anchors_per_image;
+  float score_thresh;
+  long long cap_per_image;
+  float scale[kTtaLevels];     // the level's pass scale s: (cx, cy, w, h) /= s
+  float flip_w[kTtaLevels];    // mirrored pass: cx = Wb - cx after the descale; 0: not mirrored
+  int flip[kTtaLevels];
 };
 
 // workspace carve-up (device)
@@ -181,6 +199,33 @@ constexpr int kRowPitch = kRowMaxBytes + 16;   // shared-memory row pitch: 132 w
 constexpr int kRowList = 512;        // block-local candidate list (entries beyond it fall back to global atomics)
 constexpr int kRowPairs = kRowPixels * YB_MAX_ANCHORS;   // per-warp list of (pixel, anchor) pairs that passed objectness
 
+// bit positions in the row kernel's (pixel, anchor) pair word: px | py << 10 | level << kLv | anchor << kAnchor | lane << kLane
+template <typename Params>
+struct PairBits {
+  static constexpr int kLv = 20, kLvMask = 3, kAnchor = 22, kLane = 24;
+};
+template <>
+struct PairBits<TtaDecodeParams> {   // 12 level slices: 4 bits of level
+  static constexpr int kLv = 27, kLvMask = 15, kAnchor = 20, kLane = 22;
+};
+
+// candidate index (key low word) and box of one anchor: the single-pass kernel's, and the multi-pass kernel's (unsigned
+// index: anchors x classes may exceed 2^31; box descaled / un-mirrored before the corner conversion)
+__device__ __forceinline__ uint32_t candidate_index(const DecodeParams& p, int anchor, int k) {
+  return static_cast<uint32_t>(anchor * p.n_classes + k);
+}
+__device__ __forceinline__ uint32_t candidate_index(const TtaDecodeParams& p, int anchor, int k) {
+  return static_cast<uint32_t>(anchor) * static_cast<uint32_t>(p.n_classes) + static_cast<uint32_t>(k);
+}
+__device__ __forceinline__ float4 pass_box(const DecodeParams&, int, float sx, float sy, float sw, float sh, int x, int y,
+                                           float stride_px, float aw, float ah) {
+  return decode_box(sx, sy, sw, sh, x, y, stride_px, aw, ah);
+}
+__device__ __forceinline__ float4 pass_box(const TtaDecodeParams& p, int l, float sx, float sy, float sw, float sh, int x,
+                                           int y, float stride_px, float aw, float ah) {
+  return decode_box_descaled(sx, sy, sw, sh, x, y, stride_px, aw, ah, p.scale[l], p.flip[l] != 0, p.flip_w[l]);
+}
+
 template <typename T>
 __device__ __forceinline__ float row_elem(const uint8_t* row, int e) {
   if constexpr (std::is_same<T, __half>::value)
@@ -189,9 +234,13 @@ __device__ __forceinline__ float row_elem(const uint8_t* row, int e) {
     return __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(row)[e]);
 }
 
-template <typename T>
+// Params = TtaDecodeParams: the multi-pass variant.  Up to 12 level slices (4 bits of level in the pair word instead of 2:
+// PairBits), each box descaled (and un-mirrored) before the corner conversion (pass_box), candidate index anchor * nc +
+// class in 32 unsigned bits (candidate_index).  With Params = DecodeParams those helpers are the single-pass kernel's
+// own expressions and the instance compiles to the same SASS as before the variant existed.
+template <typename T, typename Params>
 __global__ void __launch_bounds__(kRowWarps * 32)
-decode_rows_kernel(const __grid_constant__ DecodeParams p, Workspace ws, int blocks_per_image) {
+decode_rows_kernel(const __grid_constant__ Params p, Workspace ws, int blocks_per_image) {
   extern __shared__ __align__(16) uint8_t s_rows_raw[];     // [kRowWarps][kRowPixels][kRowPitch] | list[kRowList] u64 | pairs[kRowWarps][kRowPairs] uint2
   __shared__ int s_count, s_base, s_maxc;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -214,7 +263,7 @@ decode_rows_kernel(const __grid_constant__ DecodeParams p, Workspace ws, int blo
   int row_chunks = 0;                                          // 16-byte chunks of this pixel's row
   if (valid) {
 #pragma unroll
-    for (int i = 1; i < YB_MAX_LEVELS; ++i)
+    for (int i = 1; i < Params::kLevels; ++i)
       if (i < p.n_levels && r >= p.pix_start[i]) lv = i;
     const yb_head_level& L = p.lvl[lv];
     const int rr = r - p.pix_start[lv];
@@ -278,18 +327,19 @@ decode_rows_kernel(const __grid_constant__ DecodeParams p, Workspace ws, int blo
     if (a >= p.n_anchors) break;
     const bool pass = (pass_bits >> a) & 1u;
     const uint32_t bal = __ballot_sync(0xffffffffu, pass);
-    if (pass)   // px, py: 10 bits each (maps up to 1023 wide), level 2, anchor 2, source lane 5
+    if (pass)   // px, py: 10 bits each (maps up to 1023 wide), level, anchor 2, source lane 5
       s_pairs[n_pairs + __popc(bal & lt_lanes)] =
-          make_uint2(static_cast<uint32_t>(px) | static_cast<uint32_t>(py) << 10 | static_cast<uint32_t>(lv) << 20 |
-                         static_cast<uint32_t>(a) << 22 | static_cast<uint32_t>(lane) << 24,
+          make_uint2(static_cast<uint32_t>(px) | static_cast<uint32_t>(py) << 10 | static_cast<uint32_t>(lv) << PairBits<Params>::kLv |
+                         static_cast<uint32_t>(a) << PairBits<Params>::kAnchor | static_cast<uint32_t>(lane) << PairBits<Params>::kLane,
                      __float_as_uint(obj[a]));
     n_pairs += __popc(bal);
   }
   __syncwarp();
   for (int q = lane; q < n_pairs; q += 32) {
     const uint2 ent = s_pairs[q];
-    const int qx = ent.x & 1023, qy = (ent.x >> 10) & 1023, ql = (ent.x >> 20) & 3, a = (ent.x >> 22) & 3;
-    const uint8_t* q_row = s_rows + ((ent.x >> 24) & 31) * kRowPitch;
+    const int qx = ent.x & 1023, qy = (ent.x >> 10) & 1023, ql = (ent.x >> PairBits<Params>::kLv) & PairBits<Params>::kLvMask,
+              a = (ent.x >> PairBits<Params>::kAnchor) & 3;
+    const uint8_t* q_row = s_rows + ((ent.x >> PairBits<Params>::kLane) & 31) * kRowPitch;
     const float q_obj = __uint_as_float(ent.y);
     const yb_head_level& L = p.lvl[ql];
     float lt = -INFINITY;
@@ -332,8 +382,7 @@ decode_rows_kernel(const __grid_constant__ DecodeParams p, Workspace ws, int blo
         const float score = __fmul_rn(sigmoidf_ref(x), q_obj);
         if (score > p.score_thresh) {
           any = true;
-          const uint64_t key = (static_cast<uint64_t>(orderable_desc(score)) << 32) |
-                               static_cast<uint32_t>(anchor * p.n_classes + k);
+          const uint64_t key = (static_cast<uint64_t>(orderable_desc(score)) << 32) | candidate_index(p, anchor, k);
           const int slot = atomicAdd(&s_count, 1);             // shared-memory atomic: block-local slot
           if (slot < kRowList) {
             s_list[slot] = key;
@@ -345,9 +394,9 @@ decode_rows_kernel(const __grid_constant__ DecodeParams p, Workspace ws, int blo
       }
     }
     if (any) {
-      const float4 b = decode_box(sigmoidf_ref(row_elem<T>(q_row, a * K + 0)), sigmoidf_ref(row_elem<T>(q_row, a * K + 1)),
-                                  sigmoidf_ref(row_elem<T>(q_row, a * K + 2)), sigmoidf_ref(row_elem<T>(q_row, a * K + 3)),
-                                  qx, qy, L.stride_px, L.anchors_px[2 * a], L.anchors_px[2 * a + 1]);
+      const float4 b = pass_box(p, ql, sigmoidf_ref(row_elem<T>(q_row, a * K + 0)), sigmoidf_ref(row_elem<T>(q_row, a * K + 1)),
+                                sigmoidf_ref(row_elem<T>(q_row, a * K + 2)), sigmoidf_ref(row_elem<T>(q_row, a * K + 3)),
+                                qx, qy, L.stride_px, L.anchors_px[2 * a], L.anchors_px[2 * a + 1]);
       ws.boxes[static_cast<long long>(img) * p.anchors_per_image + anchor] = b;
       lane_maxc = fmaxf(lane_maxc, fmaxf(fmaxf(b.x, b.y), fmaxf(b.z, b.w)));
     }
@@ -1031,15 +1080,11 @@ extern "C" int yb_nms_begin(const yb_nms_params* p, const yb_head_level* levels,
   return YB_OK;
 }
 
-extern "C" int yb_nms_finish(const yb_nms_params* p, const yb_head_level* levels, const float* rescale_dev,
-                             float* boxes_dev, float* scores_dev, int64_t* labels_dev, int32_t* counts_dev,
-                             int64_t* status_dev, void* workspace_dev, size_t workspace_bytes, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  YB_REQUIRE(boxes_dev && scores_dev && labels_dev && counts_dev && status_dev, "nms_finish: null output");
-  Workspace ws;
-  long long apm, cap;
-  int rc = prepare(p, levels, workspace_dev, workspace_bytes, ws, apm, cap);
-  if (rc != YB_OK) return rc;
+namespace {
+// sort + sweep + rescale of the decoded candidates in `ws` (anchors_per_image `apm`, arena share `cap` per image)
+int launch_nms(const yb_nms_params* p, long long apm, long long cap, const Workspace& ws, const float* rescale_dev,
+               float* boxes_dev, float* scores_dev, int64_t* labels_dev, int32_t* counts_dev, int64_t* status_dev,
+               cudaStream_t stream) {
   NmsParams np;
   np.n_classes = p->n_classes;
   np.anchors_per_image = static_cast<int>(apm);
@@ -1058,11 +1103,24 @@ extern "C" int yb_nms_finish(const yb_nms_params* p, const yb_head_level* levels
   np.out_counts = counts_dev;
   np.status = reinterpret_cast<long long*>(status_dev);
   const size_t smem = nms_smem_bytes(p->max_det);
-  rc = ensure_nms_smem(smem);
+  const int rc = ensure_nms_smem(smem);
   if (rc != YB_OK) return rc;
   nms_image_kernel<<<p->n_images, kNmsThreads, smem, stream>>>(np, ws);
   YB_CHECK_CUDA(cudaGetLastError());
   return YB_OK;
+}
+}  // namespace
+
+extern "C" int yb_nms_finish(const yb_nms_params* p, const yb_head_level* levels, const float* rescale_dev,
+                             float* boxes_dev, float* scores_dev, int64_t* labels_dev, int32_t* counts_dev,
+                             int64_t* status_dev, void* workspace_dev, size_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  YB_REQUIRE(boxes_dev && scores_dev && labels_dev && counts_dev && status_dev, "nms_finish: null output");
+  Workspace ws;
+  long long apm, cap;
+  int rc = prepare(p, levels, workspace_dev, workspace_bytes, ws, apm, cap);
+  if (rc != YB_OK) return rc;
+  return launch_nms(p, apm, cap, ws, rescale_dev, boxes_dev, scores_dev, labels_dev, counts_dev, status_dev, stream);
 }
 
 namespace yb {
@@ -1178,14 +1236,14 @@ extern "C" int yb_decode_candidates(const yb_nms_params* p, const yb_head_level*
     constexpr int kRowSmem = kRowWarps * kRowPixels * kRowPitch + kRowList * 8 + kRowWarps * kRowPairs * 8;   // 66 KB rows + 4 KB candidate list + 4 KB pair lists
     static bool configured = false;
     if (!configured) {
-      YB_CHECK_CUDA(cudaFuncSetAttribute(decode_rows_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRowSmem));
-      YB_CHECK_CUDA(cudaFuncSetAttribute(decode_rows_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRowSmem));
+      YB_CHECK_CUDA(cudaFuncSetAttribute(decode_rows_kernel<__half, DecodeParams>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRowSmem));
+      YB_CHECK_CUDA(cudaFuncSetAttribute(decode_rows_kernel<__nv_bfloat16, DecodeParams>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRowSmem));
       configured = true;
     }
     if (dtype == YB_F16)
-      decode_rows_kernel<__half><<<rblocks, kRowWarps * 32, kRowSmem, stream>>>(dp, ws, bpi);
+      decode_rows_kernel<__half, DecodeParams><<<rblocks, kRowWarps * 32, kRowSmem, stream>>>(dp, ws, bpi);
     else
-      decode_rows_kernel<__nv_bfloat16><<<rblocks, kRowWarps * 32, kRowSmem, stream>>>(dp, ws, bpi);
+      decode_rows_kernel<__nv_bfloat16, DecodeParams><<<rblocks, kRowWarps * 32, kRowSmem, stream>>>(dp, ws, bpi);
     YB_CHECK_CUDA(cudaGetLastError());
     return YB_OK;
   }
@@ -1271,4 +1329,123 @@ extern "C" int yb_batched_nms(const float* boxes_dev, const float* scores_dev, c
   nms_image_kernel<<<1, kNmsThreads, smem, stream>>>(np, ws);
   YB_CHECK_CUDA(cudaGetLastError());
   return YB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Test-time augmentation: one per-image candidate arena over every pass (v5/models/yolo.py:152-163)
+// ---------------------------------------------------------------------------------------------
+namespace {
+// validates the passes and fills the multi-pass decode parameters; `apm` = kept anchors per image over all passes
+int fill_tta_params(const yb_nms_params* p, int n_passes, const yb_tta_pass* passes, TtaDecodeParams& dp, int& dtype,
+                    long long& apm) {
+  YB_REQUIRE(p && passes, "decode_nms_tta: null argument");
+  YB_REQUIRE(p->n_images > 0, "decode_nms_tta: n_images");
+  YB_REQUIRE(n_passes > 0 && n_passes <= YB_TTA_MAX_PASSES, "decode_nms_tta: 1..%d passes", YB_TTA_MAX_PASSES);
+  YB_REQUIRE(p->n_anchors > 0 && p->n_anchors <= YB_MAX_ANCHORS && p->n_classes > 0, "decode_nms_tta: anchors/classes");
+  YB_REQUIRE(p->max_det > 0 && p->max_det <= 4096, "decode_nms_tta: max_det must be in [1, 4096]");
+  YB_REQUIRE(p->semantics >= 0 && p->semantics <= 2, "decode_nms_tta: bad semantics");
+  int nl = 0;
+  dtype = -1;
+  dp.lvl_start[0] = 0;
+  dp.pix_start[0] = 0;
+  for (int q = 0; q < n_passes; ++q) {
+    const yb_tta_pass& P = passes[q];
+    YB_REQUIRE(P.n_levels >= 0 && P.n_levels <= YB_MAX_LEVELS, "decode_nms_tta: pass %d has %d levels", q, P.n_levels);
+    YB_REQUIRE(P.scale > 0.f, "decode_nms_tta: pass %d scale must be positive", q);
+    for (int l = 0; l < P.n_levels; ++l) {
+      const yb_head_level& L = P.levels[l];
+      if (dtype < 0) dtype = L.dtype;
+      YB_REQUIRE(L.dtype == dtype && (dtype == YB_F16 || dtype == YB_BF16),
+                 "decode_nms_tta: every level must hold fp16 (or every level bf16) logits");
+      YB_REQUIRE(L.logits != nullptr && L.H > 0 && L.W > 0 && L.H <= 1023 && L.W <= 1023,
+                 "decode_nms_tta: pass %d level %d empty or wider than 1023", q, l);
+      // the row kernel's layout: NHWC rows of A*(nc+5) 16-bit logits, 16-byte aligned, at most 512 bytes
+      YB_REQUIRE(L.stride_a == p->n_classes + 5 && L.stride_x % 8 == 0 && L.stride_x * 2 <= kRowMaxBytes &&
+                     L.stride_x >= static_cast<long long>(p->n_anchors) * (p->n_classes + 5) && L.stride_y % 8 == 0 &&
+                     L.stride_n % 8 == 0 && (reinterpret_cast<uintptr_t>(L.logits) & 15) == 0,
+                 "decode_nms_tta: pass %d level %d is not an NHWC head buffer of <= 512-byte rows", q, l);
+      dp.lvl[nl] = L;
+      dp.scale[nl] = P.scale;
+      dp.flip[nl] = P.flip_lr ? 1 : 0;
+      dp.flip_w[nl] = P.canvas_w;
+      dp.lvl_start[nl + 1] = dp.lvl_start[nl] + p->n_anchors * L.H * L.W;
+      dp.pix_start[nl + 1] = dp.pix_start[nl] + L.H * L.W;
+      ++nl;
+    }
+  }
+  YB_REQUIRE(nl > 0, "decode_nms_tta: no levels");
+  for (int l = nl; l < kTtaLevels; ++l) {
+    dp.lvl[l] = dp.lvl[0];
+    dp.scale[l] = 1.f;
+    dp.flip[l] = 0;
+    dp.flip_w[l] = 0.f;
+    dp.lvl_start[l + 1] = dp.lvl_start[l];
+    dp.pix_start[l + 1] = dp.pix_start[l];
+  }
+  apm = dp.lvl_start[nl];
+  // the key's low word holds anchor * nc + class (unsigned); the NMS kernel indexes anchors with an int
+  YB_REQUIRE(apm < (1ll << 31) && apm * p->n_classes < (1ll << 32),
+             "decode_nms_tta: %lld anchors x %d classes overflow the 32-bit candidate index", apm, p->n_classes);
+  dp.n_images = p->n_images;
+  dp.n_levels = nl;
+  dp.n_anchors = p->n_anchors;
+  dp.n_classes = p->n_classes;
+  dp.anchors_per_image = static_cast<int>(apm);
+  dp.score_thresh = p->score_thresh;
+  dp.cap_per_image = 0;
+  return YB_OK;
+}
+}  // namespace
+
+extern "C" size_t yb_decode_nms_tta_workspace_bytes(const yb_nms_params* p, int n_passes, const yb_tta_pass* passes) {
+  TtaDecodeParams dp;
+  int dtype;
+  long long apm;
+  if (fill_tta_params(p, n_passes, passes, dp, dtype, apm) != YB_OK) return 0;
+  Workspace ws;
+  const long long cap = (p->max_candidates + p->n_images - 1) / p->n_images;
+  return carve(ws, nullptr, p->n_images, cap > 0 ? cap : 1, apm);
+}
+
+extern "C" int yb_decode_nms_tta(const yb_nms_params* p, int n_passes, const yb_tta_pass* passes,
+                                 const float* rescale_dev, float* boxes_dev, float* scores_dev, int64_t* labels_dev,
+                                 int32_t* counts_dev, int64_t* status_dev, void* workspace_dev, size_t workspace_bytes,
+                                 void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  YB_REQUIRE(boxes_dev && scores_dev && labels_dev && counts_dev && status_dev && workspace_dev,
+             "decode_nms_tta: null output");
+  TtaDecodeParams dp;
+  int dtype;
+  long long apm;
+  int rc = fill_tta_params(p, n_passes, passes, dp, dtype, apm);
+  if (rc != YB_OK) return rc;
+  const long long cap = (p->max_candidates + p->n_images - 1) / p->n_images;
+  YB_REQUIRE(cap >= 1, "decode_nms_tta: max_candidates too small");
+  Workspace ws;
+  const size_t need = carve(ws, static_cast<uint8_t*>(workspace_dev), p->n_images, cap, apm);
+  if (need > workspace_bytes) {
+    set_error("decode_nms_tta: workspace of %zu bytes needed, %zu given", need, workspace_bytes);
+    return YB_ERR_WORKSPACE;
+  }
+  dp.cap_per_image = cap;
+  init_counters_kernel<<<(p->n_images + 127) / 128 + 1, 128, 0, stream>>>(ws, p->n_images,
+                                                                          reinterpret_cast<long long*>(status_dev), 0);
+  YB_CHECK_CUDA(cudaGetLastError());
+  const int bpi = (dp.pix_start[dp.n_levels] + kRowWarps * kRowPixels - 1) / (kRowWarps * kRowPixels);
+  const unsigned rblocks = static_cast<unsigned>(p->n_images) * static_cast<unsigned>(bpi);
+  constexpr int kRowSmem = kRowWarps * kRowPixels * kRowPitch + kRowList * 8 + kRowWarps * kRowPairs * 8;
+  static bool configured = false;
+  if (!configured) {
+    YB_CHECK_CUDA(cudaFuncSetAttribute(decode_rows_kernel<__half, TtaDecodeParams>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, kRowSmem));
+    YB_CHECK_CUDA(cudaFuncSetAttribute(decode_rows_kernel<__nv_bfloat16, TtaDecodeParams>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, kRowSmem));
+    configured = true;
+  }
+  if (dtype == YB_F16)
+    decode_rows_kernel<__half, TtaDecodeParams><<<rblocks, kRowWarps * 32, kRowSmem, stream>>>(dp, ws, bpi);
+  else
+    decode_rows_kernel<__nv_bfloat16, TtaDecodeParams><<<rblocks, kRowWarps * 32, kRowSmem, stream>>>(dp, ws, bpi);
+  YB_CHECK_CUDA(cudaGetLastError());
+  return launch_nms(p, apm, cap, ws, rescale_dev, boxes_dev, scores_dev, labels_dev, counts_dev, status_dev, stream);
 }

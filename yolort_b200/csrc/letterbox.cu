@@ -486,8 +486,106 @@ int launch_src(const BatchGeom& bg, int img0, int count, int Hb, int Wb, float f
   return YB_ERR_INVALID;
 }
 
+// ---- test-time augmentation: rescaled (and mirrored) copies of a space-to-depth canvas --------------------------------
+// scale_img (yolort/v5/utils/torch_utils.py:288-300) of `x.flip(3) if flip else x` (v5/models/yolo.py:157):
+// F.interpolate(size=(nh, nw), bilinear, align_corners=False) then F.pad(right/bottom, 0.447).  The sample indices are
+// src_coord's, computed in the mirrored frame; a mirrored tap at column i reads column Wb-1-i of the canvas.  Work item
+// = half a space-to-depth pixel (canvas row 2Y+dy, columns 2X and 2X+1): 16 contiguous output bytes, consecutive
+// threads -> consecutive items, so a warp stores one contiguous 512-byte run.  Each tap is one 8-byte load (the four
+// channels of a pixel sit together in the source layout).  HBM-bound: the source canvas is read about once (neighbouring
+// items share taps through L1/L2) and the pass canvas written once.
+template <typename DstT>
+__device__ __forceinline__ void load_px4(const DstT* img, int W2, int y, int x, float (&v)[3]) {
+  const uint2 raw = __ldg(reinterpret_cast<const uint2*>(img + ((static_cast<size_t>(y >> 1) * W2 + (x >> 1)) * 16 +
+                                                                ((y & 1) * 2 + (x & 1)) * 4)));
+  const DstT* e = reinterpret_cast<const DstT*>(&raw);
+  v[0] = static_cast<float>(e[0]);
+  v[1] = static_cast<float>(e[1]);
+  v[2] = static_cast<float>(e[2]);
+}
+
+template <typename DstT>
+__global__ void __launch_bounds__(256)
+canvas_rescale_kernel(const DstT* __restrict__ src, int Hb, int Wb, DstT* __restrict__ dst, int Hp, int Wp, int nh, int nw,
+                      float ratio_h, float ratio_w, int flip, float fill, long long items_per_image, long long total) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int n = static_cast<int>(i / items_per_image);
+  const long long r = i - n * items_per_image;
+  const int W2p = Wp >> 1;
+  const int dy = static_cast<int>(r & 1);
+  const int X = static_cast<int>((r >> 1) % W2p), Y = static_cast<int>((r >> 1) / W2p);
+  const int y = 2 * Y + dy;
+  const DstT* img = src + static_cast<size_t>(n) * (Hb >> 1) * (Wb >> 1) * 16;
+  float f[2][3];
+  int y0 = 0, y1 = 0;
+  float ly = 0.f;
+  if (y < nh) src_coord(y, ratio_h, Hb, y0, y1, ly);
+  const float wy0 = 1.f - ly;
+#pragma unroll
+  for (int dx = 0; dx < 2; ++dx) {
+    const int x = 2 * X + dx;
+    if (y >= nh || x >= nw) {
+      f[dx][0] = f[dx][1] = f[dx][2] = fill;
+      continue;
+    }
+    int x0, x1;
+    float lx;
+    src_coord(x, ratio_w, Wb, x0, x1, lx);
+    if (flip) {
+      x0 = Wb - 1 - x0;
+      x1 = Wb - 1 - x1;
+    }
+    const float wx0 = 1.f - lx;
+    float p00[3], p01[3], p10[3], p11[3];
+    load_px4<DstT>(img, Wb >> 1, y0, x0, p00);
+    load_px4<DstT>(img, Wb >> 1, y0, x1, p01);
+    load_px4<DstT>(img, Wb >> 1, y1, x0, p10);
+    load_px4<DstT>(img, Wb >> 1, y1, x1, p11);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {   // sample_rgb's arithmetic: fp32, unfused, one rounding at the store
+      const float top = __fadd_rn(__fmul_rn(wx0, p00[c]), __fmul_rn(lx, p01[c]));
+      const float bot = __fadd_rn(__fmul_rn(wx0, p10[c]), __fmul_rn(lx, p11[c]));
+      f[dx][c] = __fadd_rn(__fmul_rn(wy0, top), __fmul_rn(ly, bot));
+    }
+  }
+  uint8_t* o = reinterpret_cast<uint8_t*>(dst + static_cast<size_t>(n) * (Hp >> 1) * W2p * 16) + r * 16;
+  *reinterpret_cast<uint4*>(o) = make_uint4(cvt_pack2<DstT>(f[0][0], f[0][1]), cvt_pack2<DstT>(f[0][2], 0.f),
+                                            cvt_pack2<DstT>(f[1][0], f[1][1]), cvt_pack2<DstT>(f[1][2], 0.f));
+}
+
 }  // namespace
 }  // namespace yb
+
+extern "C" int yb_canvas_rescale(int n, const void* src_dev, int dtype, int Hb, int Wb, int nh, int nw, int flip_lr,
+                                 float fill, void* dst_dev, int Hp, int Wp, void* stream_) {
+  using namespace yb;
+  YB_REQUIRE(n > 0 && src_dev && dst_dev, "canvas_rescale: null/empty arguments");
+  YB_REQUIRE(dtype == YB_F16 || dtype == YB_BF16, "canvas_rescale: canvas dtype must be fp16 or bf16");
+  YB_REQUIRE(Hb > 0 && Wb > 0 && Hp > 0 && Wp > 0 && Hb % 2 == 0 && Wb % 2 == 0 && Hp % 2 == 0 && Wp % 2 == 0,
+             "canvas_rescale: canvases must have positive, even sizes");
+  YB_REQUIRE(nh > 0 && nw > 0 && nh <= Hp && nw <= Wp, "canvas_rescale: resized area %dx%d does not fit %dx%d", nh, nw,
+             Hp, Wp);
+  YB_REQUIRE((reinterpret_cast<uintptr_t>(src_dev) & 7) == 0 && (reinterpret_cast<uintptr_t>(dst_dev) & 15) == 0,
+             "canvas_rescale: misaligned canvas");
+  // upsample_bilinear2d with an output size and no scale factor: ratio = float(in) / out (area_pixel_compute_scale)
+  const float ratio_h = static_cast<float>(Hb) / static_cast<float>(nh);
+  const float ratio_w = static_cast<float>(Wb) / static_cast<float>(nw);
+  const long long items = static_cast<long long>(Hp / 2) * (Wp / 2) * 2;
+  const long long total = items * n;
+  const unsigned blocks = static_cast<unsigned>((total + 255) / 256);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (dtype == YB_F16)
+    canvas_rescale_kernel<__half><<<blocks, 256, 0, stream>>>(static_cast<const __half*>(src_dev), Hb, Wb,
+                                                              static_cast<__half*>(dst_dev), Hp, Wp, nh, nw, ratio_h,
+                                                              ratio_w, flip_lr ? 1 : 0, fill, items, total);
+  else
+    canvas_rescale_kernel<__nv_bfloat16><<<blocks, 256, 0, stream>>>(
+        static_cast<const __nv_bfloat16*>(src_dev), Hb, Wb, static_cast<__nv_bfloat16*>(dst_dev), Hp, Wp, nh, nw, ratio_h,
+        ratio_w, flip_lr ? 1 : 0, fill, items, total);
+  YB_CHECK_CUDA(cudaGetLastError());
+  return YB_OK;
+}
 
 extern "C" int yb_letterbox_geometry(int n, const int32_t* src_hw, float min_size, float max_size,
                                      int size_divisible, const int32_t* fixed_shape,

@@ -1486,9 +1486,11 @@ class Engine:
             return 64 << 30
 
     def plan(self, N: int, H: int, W: int, post: Optional[dict] = None, keep_intermediates: bool = False,
-             chunked: bool = False) -> PlanInstance:
+             chunked: bool = False, slot: int = 0) -> PlanInstance:
         """`chunked`: a plan whose first ops can also run per image chunk (PlanInstance.run_front_chunk; the arena keeps
-        the front buffers live, so it is a separate instance from the plain plan of the same shape)."""
+        the front buffers live, so it is a separate instance from the plain plan of the same shape).  `slot` > 0: another
+        instance of the same shape with its own arena (test-time augmentation runs passes of equal canvas shape, each of
+        which must keep its head logits until the joint decode)."""
         check_fp8 = getattr(self.model, "_check_fp8", None)     # YOLO: a stale FP8 calibration raises
         if check_fp8 is not None:
             check_fp8()
@@ -1496,7 +1498,7 @@ class Engine:
         pkey = None if post is None else (post["score_thresh"], post["nms_thresh"], post["detections_per_img"],
                                           post["semantics"], post["num_classes"])
         chunked = bool(chunked and N % 4 == 0 and N >= 16 and not keep_intermediates)
-        key = (N, H, W, pkey, bool(keep_intermediates), chunked, bool(self.fuse_chains), self.fp8 is not None)
+        key = (N, H, W, pkey, bool(keep_intermediates), chunked, bool(self.fuse_chains), int(slot), self.fp8 is not None)
         inst = self._plans.get(key)
         if inst is not None:
             self._plans.move_to_end(key)

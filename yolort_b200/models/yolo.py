@@ -363,6 +363,69 @@ class YOLO(nn.Module):
         return _C.decode_nms(heads, "nhwc", pc["strides"], pc["anchors_px"], pc["score_thresh"], pc["nms_thresh"],
                              pc["detections_per_img"], pc["semantics"], rescale=rescale, num_classes=self.num_classes)
 
+    # -- test-time augmentation (yolort/v5/models/yolo.py:147-208) ------------------------------------------------------
+    def augment_unsupported(self) -> Optional[str]:
+        """Why `augment=True` cannot run on this model as it stands, or None."""
+        from ..relay.logits_decoder import LogitsDecoder
+
+        if self.training:
+            return "training mode (test-time augmentation is an inference path; call .eval())"
+        if self.has_hooks():
+            return ("forward hooks on backbone / head / post_process (the staged path that fires them runs one canvas; "
+                    "remove the hooks)")
+        if isinstance(self.post_process, LogitsDecoder):
+            return "a LogitsDecoder post-process (dense outputs are not merged across passes)"
+        bufs = self.engine().lowered().head_bufs
+        divs = [b.div for b in bufs]
+        if any(b != 2 * a for a, b in zip(divs, divs[1:])):
+            return (f"head maps at strides {divs}: _clip_augmented's level arithmetic needs each map half the previous "
+                    "one (the MobileNet FPN model's are not)")
+        A, K = self.anchor_generator.num_anchors, self.num_classes + 5
+        if max(b.C for b in bufs) * 2 > 512:
+            return (f"{self.num_classes} classes with {A} anchors: the multi-pass decode reads head rows of at most 256 "
+                    f"16-bit logits ({A} x {K} here; at most 80 classes with 3 anchors)")
+        return None
+
+    def tta_plans(self, N: int, Hb: int, Wb: int):
+        """(pass geometry, plan instance per pass) of augmented inference on an N x Hb x Wb canvas: (nh, nw, Hp, Wp) of
+        each pass (_C.tta_pass_geometry with gs = the largest stride); passes of equal canvas shape get distinct plan
+        instances (`slot`), so a later pass never overwrites an earlier pass's head logits."""
+        gs = int(max(self.anchor_generator.strides))
+        geo = _C.tta_pass_geometry(Hb, Wb, gs)
+        eng = self.engine()
+        plans, seen = [], {}
+        for (_, _, hp, wp) in geo:
+            slot = seen.get((hp, wp), 0)
+            seen[(hp, wp)] = slot + 1
+            plans.append(eng.plan(N, hp, wp, slot=slot))
+        return geo, plans
+
+    def detect_augmented(self, N: int, Hb: int, Wb: int, write_canvas: Callable[[Tensor], Any],
+                         rescale: Optional[Tensor] = None) -> List[Dict[str, Tensor]]:
+        """YOLOv5's augmented inference (_forward_augment, yolo.py:152-163) on the plans: `write_canvas(t)` letterboxes
+        the batch into the pass-0 canvas t; the pass-1 (0.83, mirrored) and pass-2 (0.67) canvases are rescaled from it
+        on the device (yb_canvas_rescale), the three plans run on the current stream, and one multi-pass decode + NMS
+        (yb_decode_nms_tta: descale, un-mirror, _clip_augmented, one candidate arena per image) gives the detections,
+        with a single device->host read of counts and status.  Always decodes stored logits (no fused epilogue)."""
+        why = self.augment_unsupported()
+        if why is not None:
+            raise NotImplementedError(f"test-time augmentation is not implemented for {why}")
+        self._check_fp8()
+        # the list holds all three plans for the whole call, so the plan cache's eviction cannot free one mid-call
+        geo, plans = self.tta_plans(N, Hb, Wb)
+        write_canvas(plans[0].input)
+        for q in (1, 2):
+            nh, nw, _, _ = geo[q]
+            _C.canvas_rescale(plans[0].input, plans[q].input, nh, nw, _C.TTA_FLIPS[q])
+        for pl in plans:
+            pl.run()
+        pc = self.post_config()
+        nl = len(plans[0].heads)
+        kept = [list(range(nl - 1)), list(range(nl)), list(range(1, nl))]     # _clip_augmented (yolo.py:197-205)
+        passes = [(pl.heads, kept[q], _C.TTA_SCALES[q], _C.TTA_FLIPS[q]) for q, pl in enumerate(plans)]
+        return _C.decode_nms_tta(passes, Wb, pc["strides"], pc["anchors_px"], pc["num_classes"], pc["score_thresh"],
+                                 pc["nms_thresh"], pc["detections_per_img"], pc["semantics"], rescale=rescale)
+
     def forward(self, samples: Tensor, targets: Optional[Tensor] = None):
         if samples.dim() != 4 or samples.shape[1] != 3:
             raise ValueError(f"samples must be [N,3,H,W], got {tuple(samples.shape)}")

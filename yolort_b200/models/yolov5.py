@@ -69,7 +69,12 @@ class YOLOv5(nn.Module):
         rescale = self.transform.rescale_params_device((Hb, Wb), original_image_sizes, plan.device)
         return plan, rescale
 
-    def forward(self, inputs: List[Tensor], targets: Optional[List[Dict[str, Tensor]]] = None):
+    def forward(self, inputs: List[Tensor], targets: Optional[List[Dict[str, Tensor]]] = None, augment: bool = False):
+        """`augment=True`: YOLOv5's test-time augmentation (upstream `--augment`, yolort/v5/models/yolo.py:152-208): the
+        letterboxed canvas, its 0.83x mirrored and its 0.67x copies through the network, their predictions descaled and
+        merged into one NMS per image (YOLO.detect_augmented).  About twice the inference time."""
+        if augment:
+            return self._forward_augment(inputs, targets)
         if self.training or self.model.has_hooks():
             # The reference's own staging (yolov5.py:155-189): transform -> model (backbone -> head -> post-process
             # through the callable sub-modules, so forward hooks fire) -> rescale.  Training mode letterboxes the
@@ -88,6 +93,26 @@ class YOLOv5(nn.Module):
         plan, rescale = self._prepare(inputs)
         return self.model.detect(plan, rescale)
 
+    def _forward_augment(self, inputs: List[Tensor], targets=None) -> List[Dict[str, Tensor]]:
+        if self.training:
+            raise NotImplementedError("test-time augmentation is not implemented for training mode (an inference path; "
+                                      "call .eval())")
+        if targets is not None:
+            raise NotImplementedError("targets are only used by the training path")
+        inputs = list(inputs)
+        if len(inputs) == 0:
+            raise ValueError("empty image list")
+        original_image_sizes = [(int(im.shape[-2]), int(im.shape[-1])) for im in inputs]
+        geoms, (Hb, Wb) = self.transform.geometry(inputs)
+
+        def write(canvas: Tensor) -> None:
+            self.transform.letterbox_into(inputs, geoms, Hb, Wb, canvas, _C.YB_LAYOUT_S2D16)
+
+        dev = next(self.parameters()).device
+        with _C.device_guard(dev):
+            rescale = self.transform.rescale_params_device((Hb, Wb), original_image_sizes, dev)
+            return self.model.detect_augmented(len(inputs), Hb, Wb, write, rescale)
+
     def forward_padded(self, inputs: List[Tensor], batch_hw: Optional[Tuple[int, int]] = None):
         """Same computation, fixed-shape device outputs and no host synchronisation:
         (boxes [n,D,4], scores [n,D], labels [n,D] int64, counts [n] int32, status [4] int64).
@@ -97,13 +122,14 @@ class YOLOv5(nn.Module):
         return self.model.detect_padded(plan, rescale)
 
     @torch.no_grad()
-    def predict(self, x: Any, image_loader: Optional[Callable] = None) -> List[Dict[str, Tensor]]:
+    def predict(self, x: Any, image_loader: Optional[Callable] = None, augment: bool = False) -> List[Dict[str, Tensor]]:
         image_loader = image_loader or self.default_loader
-        piped = self._predict_pipelined(x)
-        if piped is not None:
-            return piped
+        if not augment:
+            piped = self._predict_pipelined(x)
+            if piped is not None:
+                return piped
         images = self.collate_images(x, image_loader)
-        return self.forward(images)
+        return self.forward(images, augment=augment)
 
     # -- throughput API ---------------------------------------------------------------------------------------
     @torch.no_grad()
