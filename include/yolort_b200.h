@@ -689,6 +689,46 @@ int yb_augment_sample(int n_images, const yb_aug_sampler* transforms, int n_tran
                       const int32_t* box_start_dev, float* boxes_out_dev, int64_t* labels_out_dev, int32_t* counts_dev,
                       int32_t* status_dev, void* stream);
 
+/* YOLOv5's own augmentations (yolort/v5/utils/augmentations.py) on uint8 [H, W, 3] images, OpenCV's arithmetic:
+ * csrc/v5_augment.cu, restated in oracle/restate_v5aug.py.  An output pixel maps back through the flips, then
+ * through the inverse warp (OpenCV's fixed-point bilinear remap, border 114), then runs BGR->HSV, the image's LUT and
+ * HSV->BGR, then the last cutout rectangle holding it sets its value.  Each step runs when its bit is set. */
+#define YB_V5_MAX_RECTS 31
+#define YB_V5_AFFINE 1          /* warp: inv[0..5] is warpAffine's inverse 2x3 map                             */
+#define YB_V5_PERSPECTIVE 2     /* warp: inv[0..8] is warpPerspective's inverse 3x3 map                        */
+#define YB_V5_TO_HSV 4          /* COLOR_BGR2HSV (COLOR_RGB2HSV with YB_V5_RGB)                                */
+#define YB_V5_LUT 8             /* channel c <- lut[c][channel c]                                              */
+#define YB_V5_FROM_HSV 16       /* COLOR_HSV2BGR (COLOR_HSV2RGB with YB_V5_RGB)                                */
+#define YB_V5_RGB 32            /* the image holds r, g, b: the colour steps swap b and r                      */
+#define YB_V5_FLIP_LR 64        /* the output is mirrored left-right (np.fliplr) after the colour steps        */
+#define YB_V5_FLIP_UD 128       /* the output is mirrored up-down (np.flipud) after the colour steps           */
+
+typedef struct {
+  const uint8_t* src;          /* [src_h, src_w, 3] with element strides                                      */
+  uint8_t* dst;                /* [out_h, out_w, 3] with element strides; may be src when no warp or flip bit  */
+  int64_t src_stride_y, src_stride_x, src_stride_c;
+  int64_t dst_stride_y, dst_stride_x, dst_stride_c;
+  int32_t src_h, src_w, out_h, out_w;
+  int32_t ops;                 /* YB_V5_* bits                                                                */
+  int32_t n_rects;             /* cutout rectangles, applied in order                                         */
+  int32_t block_start;         /* filled by yb_v5_augment_prepare: the image's first block                    */
+  int32_t reserved;
+  double inv[9];
+  int32_t rects[YB_V5_MAX_RECTS][4];   /* y0, x0, y1, x1 (half-open) in output pixels                          */
+  uint32_t rect_color[YB_V5_MAX_RECTS];  /* c0 | c1<<8 | c2<<16, in the image's channel order               */
+  uint8_t lut[3][256];
+} yb_v5_image;
+
+/* Host-only: checks the descriptors and fills block_start; *total_blocks = the launch's blocks. */
+int yb_v5_augment_prepare(int n_images, yb_v5_image* images, int64_t* total_blocks);
+
+/* Computes every image in one launch.  images_dev: the prepared descriptors on the device.  No host
+ * synchronisation; a repeated call writes the same bits. */
+int yb_v5_augment(int n_images, const yb_v5_image* images_dev, int64_t total_blocks, void* stream);
+
+/* mixup: dst[i] = uint8(trunc(a[i] * r + b[i] * (1 - r))) in IEEE double, over n contiguous bytes. */
+int yb_v5_mixup(const uint8_t* a_dev, const uint8_t* b_dev, uint8_t* dst_dev, int64_t n, double r, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -70,6 +70,9 @@ EXPORTED_SYMBOLS = (
     "yb_augment_prepare",
     "yb_augment",
     "yb_augment_sample",
+    "yb_v5_augment_prepare",
+    "yb_v5_augment",
+    "yb_v5_mixup",
     "yb_conv_wgrad_workspace_bytes",
     "yb_conv_wgrad_config",
     "yb_conv_wgrad",
@@ -274,6 +277,25 @@ YB_LOSS_MATCH_INT32 = 24
 YB_WGRAD_MAX_PROBLEMS = 8
 
 
+YB_V5_MAX_RECTS = 31
+(YB_V5_AFFINE, YB_V5_PERSPECTIVE, YB_V5_TO_HSV, YB_V5_LUT, YB_V5_FROM_HSV, YB_V5_RGB, YB_V5_FLIP_LR,
+ YB_V5_FLIP_UD) = (1 << k for k in range(8))
+
+
+class V5Image(ctypes.Structure):
+    """yb_v5_image: one image of the YOLOv5 augmentation kernel (include/yolort_b200.h)."""
+    _fields_ = [
+        ("src", ctypes.c_void_p), ("dst", ctypes.c_void_p),
+        ("src_stride_y", ctypes.c_int64), ("src_stride_x", ctypes.c_int64), ("src_stride_c", ctypes.c_int64),
+        ("dst_stride_y", ctypes.c_int64), ("dst_stride_x", ctypes.c_int64), ("dst_stride_c", ctypes.c_int64),
+        ("src_h", ctypes.c_int32), ("src_w", ctypes.c_int32), ("out_h", ctypes.c_int32), ("out_w", ctypes.c_int32),
+        ("ops", ctypes.c_int32), ("n_rects", ctypes.c_int32), ("block_start", ctypes.c_int32),
+        ("reserved", ctypes.c_int32), ("inv", ctypes.c_double * 9),
+        ("rects", (ctypes.c_int32 * 4) * YB_V5_MAX_RECTS), ("rect_color", ctypes.c_uint32 * YB_V5_MAX_RECTS),
+        ("lut", (ctypes.c_uint8 * 256) * 3),
+    ]
+
+
 class WgradProblem(ctypes.Structure):
     """yb_wgrad_problem: one 1x1-convolution weight gradient (include/yolort_b200.h)."""
     _fields_ = [
@@ -378,6 +400,10 @@ def lib() -> ctypes.CDLL:
     L.yb_augment.argtypes = [ctypes.c_int, ctypes.POINTER(AugImage), ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32,
                              ctypes.c_void_p, ctypes.c_void_p]
     L.yb_augment_sample.argtypes = [ctypes.c_int, ctypes.POINTER(AugSampler), ctypes.c_int] + [ctypes.c_void_p] * 10
+    L.yb_v5_augment_prepare.argtypes = [ctypes.c_int, ctypes.POINTER(V5Image), ctypes.POINTER(ctypes.c_int64)]
+    L.yb_v5_augment.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
+    L.yb_v5_mixup.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_double,
+                              ctypes.c_void_p]
     L.yb_conv_wgrad_workspace_bytes.restype = ctypes.c_size_t
     L.yb_conv_wgrad_workspace_bytes.argtypes = [ctypes.POINTER(WgradProblem), ctypes.c_int]
     L.yb_conv_wgrad_config.argtypes = [ctypes.POINTER(WgradProblem), ctypes.c_int, ctypes.POINTER(ctypes.c_int32)]
@@ -1192,6 +1218,34 @@ def augment_sample(samplers, sources: Sequence[torch.Tensor], key: torch.Tensor,
 # ---------------------------------------------------------------------------------------------------
 # weight gradient of 1x1 convolutions
 # ---------------------------------------------------------------------------------------------------
+def v5_augment(descs, sources: Sequence[torch.Tensor], device: torch.device) -> None:
+    """Runs the YOLOv5 augmentation descriptors `descs` (V5Image array, pointers set) in one launch.  The descriptors
+    (LUTs included) cross to the device in one asynchronous copy from pinned memory; nothing synchronises."""
+    n = len(descs)
+    total = ctypes.c_int64(0)
+    check(lib().yb_v5_augment_prepare(n, descs, ctypes.byref(total)), "yb_v5_augment_prepare")
+    raw = torch.frombuffer(bytearray(ctypes.string_at(ctypes.addressof(descs), ctypes.sizeof(descs))), dtype=torch.uint8)
+    with device_guard(device):
+        d_descs = raw.pin_memory().to(device, non_blocking=True)
+        check(lib().yb_v5_augment(n, d_descs.data_ptr(), total.value, current_stream_ptr(device)), "yb_v5_augment")
+        stream = torch.cuda.current_stream(device)
+        seen = set()
+        for im in sources:
+            key = im.untyped_storage().data_ptr()
+            if key not in seen:
+                seen.add(key)
+                im.record_stream(stream)
+
+
+def v5_mixup(a: torch.Tensor, b: torch.Tensor, r: float) -> torch.Tensor:
+    """uint8(trunc(a * r + b * (1 - r))) in IEEE double, elementwise over two contiguous uint8 tensors of one shape."""
+    out = torch.empty_like(a, memory_format=torch.contiguous_format)
+    with device_guard(a.device):
+        check(lib().yb_v5_mixup(a.data_ptr(), b.data_ptr(), out.data_ptr(), a.numel(), float(r),
+                                current_stream_ptr(a.device)), "yb_v5_mixup")
+    return out
+
+
 def wgrad_problems(specs) -> "ctypes.Array":
     """yb_wgrad_problem array from (dy [P, >= Cout], x [P, >= Cin], dw [Cout, Cin], db [Cout] or None) tuples of
     row-major device tensors (unit column stride); dtypes are read from the tensors."""
