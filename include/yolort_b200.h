@@ -248,6 +248,8 @@ typedef struct {
 #define YB_CONV_NO_NSPLIT 8      /* do not split N over CTAs with resident weights (A/B timing, tests) */
 #define YB_CONV_ONE_CTA 16       /* keep one CTA per SM where the shape would take two (tests compare the two launches
                                     bit for bit) */
+#define YB_CONV_NO_TAIL_SPLIT 64 /* 1x1 / im2col kernel: run the last round's tiles whole instead of splitting them over
+                                    the idle CTAs (tests compare the two launches bit for bit, A/B timing) */
 /* ... and of an e4m3 YB_OP_CONV (see above), which takes these two only: */
 #define YB_CONV_E4M3_F16_OUT 16  /* fp16 output */
 #define YB_CONV_E4M3_BF16_OUT 32 /* bf16 output */
@@ -283,6 +285,8 @@ typedef struct {
   int32_t m_tiles;           /* output tiles along M */
   int32_t work_items;        /* tiles (halo patch: tasks) the grid walks */
   int32_t tail_n;            /* wgmma N of the chained tail, 0 without one */
+  int32_t tail_tiles;        /* 1x1 / im2col kernel: tiles of the last round that are split along N, 0 if none */
+  int32_t tail_split;        /* ... into this many sub-tasks each (1, or 0 from the other kernels: none) */
 } yb_conv_info;
 
 /* Host-only introspection of how a convolution would be launched (tests, tuning).  A convolution takes two CTAs per SM
@@ -292,7 +296,12 @@ typedef struct {
  * 2 x SMs tiles; the grid is then up to 2 x SMs.  Otherwise a 1x1 / im2col convolution takes two CTAs per SM of ONE
  * consumer warpgroup each (64-row tiles) when its one-CTA plan has a 256-column N tile and no chained tail and it has at
  * least 3 x SMs 128-row tiles: it then runs as two 128-column N tiles whose weights stay resident (at most 80 KB per N
- * tile, one N tile per CTA), in half of the SM's shared memory, on a grid of 2 x SMs.  Pure host logic. */
+ * tile, one N tile per CTA), in half of the SM's shared memory, on a grid of 2 x SMs.  A 1x1 / im2col convolution
+ * with 128-column N tiles, no chained tail or fused decode and a grid that is a multiple of its N tiles splits the
+ * r tiles of a partial last round in two when 2 r <= grid (64-row halves with two consumer warpgroups, 64-column halves
+ * with one), which the otherwise idle CTAs run (tail_tiles = r, tail_split = 2); a one-CTA plan whose 256-column N
+ * tile streams its weights over 2-4 rounds takes 128-column N tiles when that split then applies.  Reserved bit
+ * YB_CONV_NO_TAIL_SPLIT keeps the tiles whole (and 256 columns).  Pure host logic. */
 int yb_conv_config(const yb_op_desc* op, yb_conv_info* info);
 
 typedef struct yb_plan yb_plan;

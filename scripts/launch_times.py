@@ -6,7 +6,9 @@ For every launch: the median time over `reps` full-plan passes (an event pair ar
 the cache state of a real step), the algorithmic bytes (every input, output, residual and weight tensor once, from
 the descriptor's shapes), the FLOP, the least time the data-sheet H100 SXM could take (the larger of bytes / 3.35 TB/s
 and FLOP / 989 TFLOP/s dense FP16), which of the two bounds it, and the layout the launch was planned for
-(yb_conv_config): CTAs per SM x consumer warpgroups per CTA, 1x2, 2x2 (the 104-register instances) or 2x1.  The card's name and power limit are printed with the table."""
+(yb_conv_config): CTAs per SM x consumer warpgroups per CTA, 1x2, 2x2 (the 104-register instances) or 2x1, and the
+rounds of the persistent grid (work items / grid; "+s" when the tiles of a partial last round run as s column slices).
+The card's name and power limit are printed with the table."""
 import ctypes
 import subprocess
 import sys
@@ -77,7 +79,7 @@ torch.cuda.synchronize()
 
 print(f"# {name} batch {batch} {size}x{size} {dt} on {card()}")
 print(f"# per-launch us: median of {reps} full-plan passes; bound = max(bytes / 3.35 TB/s, FLOP / 989 TFLOP/s)")
-print(f"{'op':>3} {'us':>8} {'MB':>8} {'GFLOP':>7} {'bound us':>8} {'by':>4} {'of bound':>8} {'layout':>6}  launch")
+print(f"{'op':>3} {'us':>8} {'MB':>8} {'GFLOP':>7} {'bound us':>8} {'by':>4} {'of bound':>8} {'layout':>6} {'rounds':>7}  launch")
 tot = tot_bound = 0.0
 for i in range(n):
     ts = sorted(ev[r][i].elapsed_time(ev[r][i + 1]) * 1e3 for r in range(reps))
@@ -87,11 +89,15 @@ for i in range(n):
     fl = plan.op_flops[i]
     t_mem, t_mma = by / HBM_BPS * 1e6, fl / FP16_FLOPS * 1e6
     bound = max(t_mem, t_mma)
-    layout = _C.conv_config(d)["layout"] if d.kind == _C.YB_OP_CONV else "-"
+    layout = rounds = "-"
+    if d.kind == _C.YB_OP_CONV:
+        cfg = _C.conv_config(d)
+        layout = cfg["layout"]
+        rounds = f"{cfg['work_items'] / cfg['grid']:.2f}" + (f"+{cfg['tail_split']}" if cfg["tail_split"] > 1 else "")
     tot += t
     tot_bound += bound
     print(f"{i:3d} {t:8.1f} {by / 1e6:8.1f} {fl / 1e9:7.2f} {bound:8.1f} {'HBM' if t_mem >= t_mma else 'MMA':>4} "
-          f"{bound / t:8.2f} {layout:>6}  {plan.op_names[i]}")
+          f"{bound / t:8.2f} {layout:>6} {rounds:>7}  {plan.op_names[i]}")
 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
 e0.record()
 for _ in range(reps):

@@ -23,6 +23,7 @@ YB_OP_QUANTIZE = 7
 YB_ACT_NONE, YB_ACT_SILU, YB_ACT_HARDSWISH, YB_ACT_LEAKY01, YB_ACT_RELU = 0, 1, 2, 3, 4
 # yb_op_desc.reserved option bits of a convolution (fp16 / bf16; e4m3 convolutions take the last two only)
 YB_CONV_FORCE_IM2COL, YB_CONV_BAND_STEM, YB_CONV_FORCE_PLANES, YB_CONV_NO_NSPLIT, YB_CONV_ONE_CTA = 1, 2, 4, 8, 16
+YB_CONV_NO_TAIL_SPLIT = 64
 YB_CONV_E4M3_F16_OUT, YB_CONV_E4M3_BF16_OUT = 16, 32
 YB_CONV_KERNEL_IM2COL, YB_CONV_KERNEL_PATCH, YB_CONV_KERNEL_E4M3 = 0, 1, 2
 PATCH_TILINGS = {1: "classic", 2: "wrap", 3: "stride2"}      # yb_conv_info.tiling of the halo-patch kernel
@@ -126,7 +127,8 @@ class ConvInfo(ctypes.Structure):
     """yb_conv_info: how a convolution is launched (include/yolort_b200.h)."""
     _fields_ = [(name, ctypes.c_int32) for name in (
         "kernel", "block_n", "n_tiles", "weights_resident", "tiles_per_pass", "slots", "ring", "store_cols", "store_bufs",
-        "groups", "resident_ctas", "chained", "smem_bytes", "grid", "tiling", "m_tiles", "work_items", "tail_n")]
+        "groups", "resident_ctas", "chained", "smem_bytes", "grid", "tiling", "m_tiles", "work_items", "tail_n",
+        "tail_tiles", "tail_split")]
 
 
 class HeadDecode(ctypes.Structure):
@@ -557,7 +559,7 @@ def conv_config(op: "OpDesc") -> dict:
     patch = info.kernel == YB_CONV_KERNEL_PATCH
     cfg = {k: int(getattr(info, k)) for k in ("block_n", "n_tiles", "weights_resident", "tiles_per_pass", "slots", "ring",
                                                "store_cols", "smem_bytes", "grid", "chained", "resident_ctas", "m_tiles",
-                                               "work_items", "tail_n")}
+                                               "work_items", "tail_n", "tail_tiles", "tail_split")}
     cfg["patch_kernel"] = int(patch)
     cfg["e4m3_kernel"] = int(info.kernel == YB_CONV_KERNEL_E4M3)
     # the halo-patch kernel reports its staging buffers, the others their consumer warpgroups (which share two buffers)

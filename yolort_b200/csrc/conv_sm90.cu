@@ -56,6 +56,9 @@ struct ConvKernelParams {
   int b_resident;  // weights of the (single) N tile stay in shared memory for the CTA's lifetime
   uint32_t b_res_bytes;
   int n_tiles, num_tiles;
+  // Split tail: the tasks from full_tiles on are the last round's r = num_tiles - full_tiles tiles, each cut into `split`
+  // halves (kernel: 64-row or 64-column; split = 1: num_tasks = num_tiles, every task a whole tile)
+  int full_tiles, split, num_tasks;
   int ctas;        // CTAs per SM the launch is planned for (1 or 2): selects the kernel instance
   int groups;      // consumer warpgroups per CTA (2, or 1 with two CTAs per SM): selects the kernel instance
   int store_cols;  // columns per TMA store box: 64 / 32 / 16
@@ -72,6 +75,47 @@ struct ConvKernelParams {
 
 template <int kGroups>
 __device__ __forceinline__ void consumer_sync() { named_bar_sync(kConsumerBar, 128 * kGroups); }
+
+// Task t of the grid's walk: its tile's M tile and N tile, and which of the tile's `split` halves it computes
+// (piece 0 of 1 for a whole tile).  The tail sub-tasks are ordered so that task full_tiles + u, which CTA u runs, lies
+// in N tile u % n_tiles: a CTA keeps the N tile (and resident weights) of its full rounds, as the grid and full_tiles are
+// multiples of n_tiles (conv_plan).  Instances without tail halves (kSplits false) walk whole tiles only.
+struct ConvTask {
+  int m_tile, n_tile, piece, split;
+};
+template <bool kSplits>
+__device__ __forceinline__ ConvTask conv_task(const ConvKernelParams& p, int t) {
+  ConvTask k;
+  int tile = t;
+  k.piece = 0;
+  k.split = 1;
+  if (kSplits && t >= p.full_tiles) {
+    const int u = t - p.full_tiles;
+    const int q = u / p.n_tiles;
+    tile = p.full_tiles + (q / p.split) * p.n_tiles + (u - q * p.n_tiles);
+    k.piece = q % p.split;
+    k.split = p.split;
+  }
+  k.m_tile = tile / p.n_tiles;
+  k.n_tile = tile - k.m_tile * p.n_tiles;
+  return k;
+}
+
+// One pipeline stage's MMAs at the wgmma N kW (the tile's kN, or a tail half's kN / 2): `cnt` k-iterations
+// of A and B sub-tiles; returns the channel chunk the next stage starts at.
+template <bool kBf16, int kW>
+__device__ __forceinline__ int stage_mmas(float* acc, const ConvKernelParams& p, uint32_t a_lo0, uint32_t a_step16,
+                                          uint32_t b_lo0, uint32_t b_step16, uint64_t ab_hi, int cnt, int ch, int kk,
+                                          bool first) {
+  for (int j = 0; j < cnt; ++j) {
+    const int kc = ch == p.chunks - 1 ? p.kk_last : kk;
+    for (int k = 0; k < kc; ++k)
+      wgmma_mma<kBf16, kW>(acc, desc_lohi(a_lo0 + j * a_step16 + 2 * k, ab_hi), desc_lohi(b_lo0 + j * b_step16 + 2 * k, ab_hi),
+                           !first || (j | k) != 0);
+    if (++ch == p.chunks) ch = 0;
+  }
+  return ch;
+}
 
 // Fused post-processing front end (yolort/models/box_head.py:328-360,418) on the head's accumulator fragment.  Objectness
 // and box logits of every (row, anchor) go through a small shared-memory table (they sit in other lanes' registers);
@@ -170,12 +214,19 @@ template <bool kBf16, int kN, bool kDecode, int kN2, int kCtas, int kGroups = 2>
 __global__ void __launch_bounds__(cta_threads(kGroups), kCtas)
 conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_w2,
-                  const __grid_constant__ CUtensorMap tmap_out2, const ConvKernelParams p) {
+                  const __grid_constant__ CUtensorMap tmap_out2, const __grid_constant__ CUtensorMap tmap_a64,
+                  const __grid_constant__ CUtensorMap tmap_out64, const ConvKernelParams p) {
   static_assert(kGroups == 2 || (kGroups == 1 && kCtas == 2 && !kDecode), "one consumer warpgroup: two CTAs, no decode");
   constexpr bool kChain = kN2 != 0;
   constexpr int kAcc = (kN > kN2 ? kN : kN2) / 2;   // accumulator registers per thread
   constexpr int kBlockM = tile_rows(kGroups);
   constexpr int kStageBufBytes = stage_buf_bytes(kGroups);
+  // Tail halves in the 128-column instances only (the N = 256 instances spill their 128 accumulators with any of this
+  // code).  With two consumer warpgroups a half is 64 rows of the tile: both warpgroups multiply the same 64 A rows,
+  // each with its 64 columns of the tile, so the sub-task loads half the tile's A.  With one warpgroup (64-row tiles) a
+  // half is 64 columns of the tile.
+  constexpr bool kSplits = !kDecode && !kChain && kN == 128;
+  constexpr bool kRowHalves = kSplits && kGroups == 2;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
@@ -238,10 +289,13 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     // ===================== TMA producer (warp-uniform loop, one elected lane issues) =====================
     const uint32_t a_bytes = kBlockM * p.block_k * 2, b_bytes = p.block_n * p.block_k * 2;
     int kit = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      const int m_tile = tile / p.n_tiles;
-      const int n0 = (tile - m_tile * p.n_tiles) * p.block_n;
-      const int m0 = m_tile * kBlockM;
+    for (int t = blockIdx.x; t < p.num_tasks; t += gridDim.x) {
+      const ConvTask task = conv_task<kSplits>(p, t);   // a tail half loads the whole tile's B
+      const bool rows64 = kRowHalves && task.split != 1;   // a row half: 64 A rows through the 64-row map
+      const int n0 = task.n_tile * p.block_n;
+      const int m0 = task.m_tile * kBlockM + (rows64 ? task.piece * 64 : 0);
+      const CUtensorMap* map_a = rows64 ? &tmap_a64 : &tmap_a;
+      const uint32_t a_task_bytes = rows64 ? a_bytes / 2 : a_bytes;
       int cw = 0, ch = 0, cn = 0;
       if (p.mode == 1) {
         cn = m0 / p.HoWo;
@@ -259,17 +313,17 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         uint8_t* a_dst = tiles + s * stage_bytes;
         uint8_t* b_dst = a_dst + p.kpg * p.a_stage_bytes;
         if (YB_ELECT()) {
-          mbar_expect_tx(&full_bar[s], cnt * (a_bytes + (p.b_resident ? 0u : b_bytes)));
+          mbar_expect_tx(&full_bar[s], cnt * (a_task_bytes + (p.b_resident ? 0u : b_bytes)));
           for (int j = 0; j < cnt; ++j) {
             const int it = it0 + j;
             const int tap = it / p.chunks;
             const int chunk = it - tap * p.chunks;
             if (p.mode == 0) {
-              tma_load_2d(&tmap_a, &full_bar[s], a_dst + j * p.a_stage_bytes, chunk * p.block_k, m0);
+              tma_load_2d(map_a, &full_bar[s], a_dst + j * p.a_stage_bytes, chunk * p.block_k, m0);
             } else {
               const int r = tap / p.ksize;
               const int sx = tap - r * p.ksize;
-              tma_load_im2col_4d(&tmap_a, &full_bar[s], a_dst + j * p.a_stage_bytes, chunk * p.block_k, cw, ch, cn,
+              tma_load_im2col_4d(map_a, &full_bar[s], a_dst + j * p.a_stage_bytes, chunk * p.block_k, cw, ch, cn,
                                  static_cast<uint16_t>(sx), static_cast<uint16_t>(r));
             }
             if (!p.b_resident) tma_load_2d(&tmap_b, &full_bar[s], b_dst + j * p.b_stage_bytes, it * p.block_k, n0);
@@ -314,14 +368,26 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   if constexpr (kChain) mbar_wait(&w2_full, 0);
 
   int kit = 0, store_idx = 0;
-  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-    const int m_tile = tile / p.n_tiles;
-    const int n0 = (tile - m_tile * p.n_tiles) * p.block_n;
-    const int m0 = m_tile * kBlockM;
-    if (!fixed_n) {   // the previous tile's epilogue has finished with the bias (and the staging boxes)
-      consumer_sync<kGroups>();
-      for (int i = ctid; i < p.block_n; i += 128 * kGroups) s_bias[i] = (n0 + i < p.bias_len) ? __ldg(p.bias + n0 + i) : 0.f;
+  for (int t = blockIdx.x; t < p.num_tasks; t += gridDim.x) {
+    const ConvTask task = conv_task<kSplits>(p, t);
+    const bool half = kSplits && task.split != 1;
+    const bool rows64 = kRowHalves && half;
+    const int width = half ? bn / 2 : bn;   // columns this warpgroup computes and stores
+    // this warpgroup's first column in the tile: a column half's, or (row halves) the warpgroup's half of the columns
+    const int col0 = half ? (rows64 ? g : task.piece) * width : 0;
+    const int n0 = task.n_tile * p.block_n + col0;
+    const int m0 = task.m_tile * kBlockM + (rows64 ? task.piece * 64 : 0);
+    const bool load_bias = !fixed_n || (half && !rows64);   // s_bias holds the task's columns from s_bias[0]
+    if (load_bias) {
+      consumer_sync<kGroups>();   // the previous tile's epilogue has finished with the bias (and the staging boxes)
+      const int nb = rows64 ? n0 - col0 : n0, wb = rows64 ? bn : width;
+      for (int i = ctid; i < wb; i += 128 * kGroups) s_bias[i] = (nb + i < p.bias_len) ? __ldg(p.bias + nb + i) : 0.f;
     }
+    const float* bias_cols = s_bias + (rows64 ? col0 : 0);
+    // the task's rows of the tile's B sub-tiles (multiples of 64 rows keep the 8-row swizzle phase); a row half's two
+    // warpgroups read the same 64 A rows
+    const uint32_t b_piece16 = (col0 * row_bytes) >> 4;
+    const uint32_t a_group16 = rows64 ? 0u : g * a_half16;
 
     // ---- main loop: stage s is released once the MMAs that read it have completed (one stage in flight) ----
     int chunk = 0, prev_s = -1;
@@ -329,17 +395,15 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       const int cnt = min(p.kpg, p.num_k_iters - it0);
       const int s = kit % p.stages;
       mbar_wait(&full_bar[s], (kit / p.stages) & 1);
-      const uint32_t a_lo0 = smem_lo16(tiles + s * stage_bytes) + g * a_half16;
-      const uint32_t b_lo0 = p.b_resident ? b_res_lo0 + it0 * b_step16 : smem_lo16(tiles + s * stage_bytes) + p.kpg * a_step16;
+      const uint32_t a_lo0 = smem_lo16(tiles + s * stage_bytes) + a_group16;
+      const uint32_t b_lo0 =
+          (p.b_resident ? b_res_lo0 + it0 * b_step16 : smem_lo16(tiles + s * stage_bytes) + p.kpg * a_step16) + b_piece16;
       wgmma_fence();
-      int ch = chunk;
-      for (int j = 0; j < cnt; ++j) {
-        const int kc = ch == p.chunks - 1 ? p.kk_last : kk;
-        for (int k = 0; k < kc; ++k)
-          wgmma_mma<kBf16, kN>(acc, desc_lohi(a_lo0 + j * a_step16 + 2 * k, ab_hi), desc_lohi(b_lo0 + j * b_step16 + 2 * k, ab_hi),
-                            (it0 | j | k) != 0);
-        if (++ch == p.chunks) ch = 0;
-      }
+      int ch;
+      if (!kSplits || width == bn)
+        ch = stage_mmas<kBf16, kN>(acc, p, a_lo0, a_step16, b_lo0, b_step16, ab_hi, cnt, chunk, kk, it0 == 0);
+      else
+        ch = stage_mmas<kBf16, kSplits ? kN / 2 : kN>(acc, p, a_lo0, a_step16, b_lo0, b_step16, ab_hi, cnt, chunk, kk, it0 == 0);
       wgmma_commit();
       wgmma_wait<1>();
       if (prev_s >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev_s]);
@@ -349,10 +413,11 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     wgmma_wait<0>();
     fence_acc<kN / 2>(acc);
     if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev_s]);
-    if (!fixed_n) consumer_sync<kGroups>();   // bias visible
+    if (load_bias) consumer_sync<kGroups>();   // bias visible
 
-    fr.row[0] = static_cast<long long>(m0) + fr.loc[0];
-    fr.row[1] = static_cast<long long>(m0) + fr.loc[1];
+    // fr.loc is the row in the staging box; a row half's warpgroups both hold rows m0 .. m0 + 63
+    fr.row[0] = static_cast<long long>(m0) + fr.loc[0] - (rows64 ? g * 64 : 0);
+    fr.row[1] = static_cast<long long>(m0) + fr.loc[1] - (rows64 ? g * 64 : 0);
     fr.ok[0] = fr.row[0] < p.M;
     fr.ok[1] = fr.row[1] < p.M;
     if constexpr (kDecode) {
@@ -364,18 +429,26 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       if (issuer) tma_store_wait_read<0>();
       consumer_sync<kGroups>();
     }
-    for (int c0 = 0; c0 < bn; c0 += store_cols, ++store_idx) {
+    for (int c0 = 0; c0 < width; c0 += store_cols, ++store_idx) {
       // Two staging buffers, one barrier per box: before the barrier below the issuer waits until the PREVIOUS
       // store has finished reading its buffer, which is the one the next box will overwrite.
       uint8_t* buf = staging + (kChain ? (c0 / store_cols) : (store_idx & 1)) * kStageBufBytes;
-      epilogue_box<kBf16, kN>(p.ep, acc, c0, store_cols, s_bias, fr, n0, buf, lane);
+      epilogue_box<kBf16, kN>(p.ep, acc, c0, store_cols, bias_cols, fr, n0, buf, lane);
       fence_proxy_async_smem();
       if constexpr (!kChain) {
         if (issuer) tma_store_wait_read<0>();
       }
       consumer_sync<kGroups>();
       if (issuer) {
-        if ((!kChain || p.ch.store_first) && n0 + c0 < p.ep.Cout) tma_store_2d(&tmap_out, buf, n0 + c0, m0);
+        if (rows64) {   // each warpgroup's 64 x 64 box: rows 0-63 / 64-127 of the staging buffer
+          const int nt = task.n_tile * p.block_n;
+          if (m0 < p.M) {
+            if (nt + c0 < p.ep.Cout) tma_store_2d(&tmap_out64, buf, nt + c0, m0);
+            if (nt + width + c0 < p.ep.Cout) tma_store_2d(&tmap_out64, buf + 64 * store_cols * 2, nt + width + c0, m0);
+          }
+        } else if ((!kChain || p.ch.store_first) && n0 + c0 < p.ep.Cout) {
+          tma_store_2d(&tmap_out, buf, n0 + c0, m0);
+        }
         tma_store_commit();
       }
     }
@@ -416,7 +489,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 }
 
 using ConvKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
-                              const ConvKernelParams);
+                              const CUtensorMap, const CUtensorMap, const ConvKernelParams);
 
 // One kernel per (dtype, N tile, fused decode, chained tail N, CTAs per SM, consumer warpgroups): the MMA width and the
 // accumulator size are compile-time constants of every instance, so the accumulators stay in registers while the wgmma
@@ -473,7 +546,8 @@ static int conv_plan(const yb_op_desc& d, int ctas, int groups, ConvKernelParams
 // Validation of an fp16 / bf16 convolution descriptor, shared with the halo-patch kernel (pure host logic).
 int conv_validate(const yb_op_desc& d) {
   YB_REQUIRE(d.dtype == YB_F16 || d.dtype == YB_BF16, "conv: dtype must be f16 or bf16");
-  YB_REQUIRE((d.reserved & ~31) == 0, "conv: reserved bits 5 and up must be zero, got 0x%x", d.reserved);
+  YB_REQUIRE((d.reserved & ~(31 | YB_CONV_NO_TAIL_SPLIT)) == 0, "conv: reserved bits 5 and 7 and up must be zero, got 0x%x",
+             d.reserved);
   YB_REQUIRE(d.ksize >= 1 && d.ksize <= 7 && d.stride >= 1 && d.stride <= 2, "conv: ksize/stride");
   YB_REQUIRE(d.act >= YB_ACT_NONE && d.act <= YB_ACT_RELU, "conv: unknown activation %d", d.act);
   YB_REQUIRE(d.Cin % 8 == 0 && d.in_cstride % 8 == 0 && d.in_cstride >= d.Cin,
@@ -536,6 +610,17 @@ static int conv_plan(const yb_op_desc& d, int ctas, int groups, ConvKernelParams
     // with at least 3 x SMs 128-row tiles (DESIGN.md section 3: measured gains at 400 and 1600 such tiles, none at 100)
     if (block_n != 256 || d.chain != nullptr || m_tiles128 < 3 * sms) return YB_ERR_INVALID;
     block_n = 128;
+  }
+  // A one-CTA 256-column plan that streams its weights (more than 80 KB) and runs 2-4 rounds, the last one partial,
+  // takes 128-column N tiles instead when the split tail then applies (see below): with so few rounds the idle part of
+  // the last one is a large share of the launch.  c2's ops 8 and 27 (3.03 rounds) measured 145 -> 114 and 106 -> 73 us;
+  // launches with more rounds keep 256 columns (not measured).
+  // The bits that pin a plan for bit-for-bit comparisons (YB_CONV_ONE_CTA, YB_CONV_NO_TAIL_SPLIT) keep 256 columns.
+  if (groups == 2 && ctas == 1 && block_n == 256 && d.chain == nullptr && d.decode == nullptr &&
+      !(d.reserved & (YB_CONV_NO_TAIL_SPLIT | YB_CONV_ONE_CTA)) && static_cast<size_t>(d.ksize) * d.ksize * d.Cin_pad * 256 * 2 > 80 * 1024 &&
+      m_tiles > sms && m_tiles < 4 * sms && m_tiles % sms != 0) {
+    const int n128 = (d.Cout + 127) / 128, r128 = (m_tiles * n128) % sms;
+    if (sms % n128 == 0 && r128 > 0 && 2 * r128 <= sms) block_n = 128;
   }
   int n_tiles = (d.Cout + block_n - 1) / block_n;
   YB_REQUIRE(mma_n(block_n) == block_n && block_n <= kMaxBlockN, "conv: N tile %d is not a wgmma N", block_n);
@@ -618,6 +703,18 @@ static int conv_plan(const yb_op_desc& d, int ctas, int groups, ConvKernelParams
   }
   const int max_grid = ctas * sms;   // a grid that is not a multiple of the N tiles loads the bias per tile
   grid = dim3(kp.num_tiles < max_grid ? kp.num_tiles : max_grid, 1, 1);
+  // Split tail: when the tiles are not a whole number of rounds of the grid, the r tiles of the last round would leave
+  // G - r CTAs idle for a whole tile time.  With 128-column N tiles each of them becomes two sub-tasks, which the idle
+  // CTAs run: 64-row halves (both warpgroups on the same 64 A rows, 64 columns each) with two consumer warpgroups,
+  // 64-column halves with one.  Each warpgroup keeps the wgmma M of 64 rows and the k16 sequence, so every output
+  // element is computed as in the whole tile and the results are bit-identical.  A last round fuller than G / 2 cannot
+  // be halved within one round and stays.
+  const int G = static_cast<int>(grid.x);
+  const int r = kp.num_tiles % G;
+  kp.split = !(d.reserved & YB_CONV_NO_TAIL_SPLIT) && !kp.decode_on && !kp.ch.on && kp.block_n == 128 &&
+                     G % kp.n_tiles == 0 && r > 0 && 2 * r <= G ? 2 : 1;
+  kp.full_tiles = kp.split > 1 ? kp.num_tiles - r : kp.num_tiles;
+  kp.num_tasks = kp.full_tiles + (kp.num_tiles - kp.full_tiles) * kp.split;
   smem_bytes = pipe.smem;
   return YB_OK;
 }
@@ -646,19 +743,21 @@ int im2col_conv_config(const yb_op_desc& d, yb_conv_info* info) {
     info->m_tiles = kp.num_tiles / kp.n_tiles;
     info->work_items = kp.num_tiles;
     info->tail_n = kp.ch.n2;
+    info->tail_tiles = kp.split > 1 ? kp.num_tiles - kp.full_tiles : 0;
+    info->tail_split = kp.split;
   }
   return rc;
 }
 
 struct Im2colConvOp final : ConvOp {
-  CUtensorMap tmap_a, tmap_b, tmap_out, tmap_w2, tmap_out2;
+  CUtensorMap tmap_a, tmap_b, tmap_out, tmap_w2, tmap_out2, tmap_a64, tmap_out64;
   ConvKernelParams kp;
   ConvKernelFn fn = nullptr;
   dim3 grid;
   size_t smem_bytes;
   int launch(cudaStream_t stream) const override {
     YB_CHECK_CUDA(launch_pdl(fn, grid, dim3(cta_threads(kp.groups)), smem_bytes, stream, tmap_a, tmap_b, tmap_out, tmap_w2,
-                             tmap_out2, kp));
+                             tmap_out2, tmap_a64, tmap_out64, kp));
     return YB_OK;
   }
 };
@@ -683,6 +782,16 @@ int im2col_conv_create(const yb_op_desc& d, ConvOp** out) {
                      CU_TENSOR_MAP_L2_PROMOTION_NONE);
   op->tmap_w2 = op->tmap_b;      // placeholders when nothing is chained (never dereferenced)
   op->tmap_out2 = op->tmap_out;
+  op->tmap_a64 = op->tmap_a;     // ... and when no tail tile is split into row halves
+  op->tmap_out64 = op->tmap_out;
+  if (rc == YB_OK && kp.split > 1 && kp.groups == 2) {   // the row halves' 64-row A and output boxes
+    rc = kp.mode == 0 ? tmap_matrix(&op->tmap_a64, "conv input (tail halves)", dt, d.in, d.Cin, kp.M, d.in_cstride,
+                                    kp.block_k, 64, CU_TENSOR_MAP_L2_PROMOTION_L2_128B)
+                      : tmap_im2col(&op->tmap_a64, "conv input (tail halves)", dt, d, kp.block_k, 64);
+    if (rc == YB_OK)
+      rc = tmap_matrix(&op->tmap_out64, "conv output (tail halves)", dt, d.out, d.Cout, kp.M, d.out_cstride, kp.store_cols,
+                       64, CU_TENSOR_MAP_L2_PROMOTION_NONE);
+  }
   if (rc == YB_OK && kp.ch.on) {
     const yb_conv_chain& c = *d.chain;
     rc = tmap_matrix(&op->tmap_w2, "conv chained tail weights", dt, c.weight, c.K_pad, c.Cout_pad, c.K_pad,
