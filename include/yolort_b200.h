@@ -738,6 +738,68 @@ int yb_v5_augment(int n_images, const yb_v5_image* images_dev, int64_t total_blo
 /* mixup: dst[i] = uint8(trunc(a[i] * r + b[i] * (1 - r))) in IEEE double, over n contiguous bytes. */
 int yb_v5_mixup(const uint8_t* a_dev, const uint8_t* b_dev, uint8_t* dst_dev, int64_t n, double r, void* stream);
 
+/* YOLOv5's mosaic training batches (the augment=True, rect=False branch of upstream v6.0's
+ * LoadImagesAndLabels.__getitem__: load_image, load_mosaic or letterbox, random_perspective, mixup, augment_hsv, the
+ * flips; yolort_b200/v5/utils/datasets.py draws every parameter).  Two launches:
+ *
+ * yb_v5_resize: load_image's cv2.resize(INTER_LINEAR) of uint8 [H, W, 3] images, OpenCV 4.x's 8-bit fixed-point
+ * arithmetic (11-bit coefficients, horizontal then vertical pass, the vertical pass in the (S >> 4) * b >> 16 form of
+ * VResizeLinearVec_32s8u), and its INTER_AREA average for an exact 2x downscale. */
+typedef struct {
+  const uint8_t* src;          /* [src_h, src_w, 3] with element strides                                      */
+  uint8_t* dst;                /* dense [dst_h, dst_w, 3]                                                     */
+  int64_t src_stride_y, src_stride_x, src_stride_c;
+  int32_t src_h, src_w, dst_h, dst_w;
+  int32_t block_start;         /* filled by yb_v5_resize_prepare: the job's first block                       */
+  int32_t reserved;
+} yb_v5_resize_job;
+
+/* Host-only: checks the jobs and fills block_start; *total_blocks = the launch's blocks. */
+int yb_v5_resize_prepare(int n_jobs, yb_v5_resize_job* jobs, int64_t* total_blocks);
+
+/* Resizes every job in one launch.  jobs_dev: the prepared jobs on the device.  No job may read another's dst. */
+int yb_v5_resize(int n_jobs, const yb_v5_resize_job* jobs_dev, int64_t total_blocks, void* stream);
+
+/* yb_v5_compose: one training sample per descriptor.  The warp reads a virtual canvas: up to YB_V5_MAX_PLACES
+ * rectangles, each a view of a (resized) image placed at an offset, and the value 114 everywhere else; the canvas
+ * itself is never written.  An output pixel maps back through the flips, then through each canvas's warp (or reads
+ * the canvas at the same place), blends the two canvases of a mixup in IEEE double, runs the colour steps and stores
+ * channel k at dst + y * dst_stride_y + x * dst_stride_x + k * dst_stride_c (a negative dst_stride_c reverses the
+ * channels: CHW RGB from a BGR sample). */
+#define YB_V5_MAX_PLACES 4
+
+typedef struct {
+  const uint8_t* src;          /* [h, w, 3] with element strides                                             */
+  int64_t stride_y, stride_x, stride_c;
+  int32_t y0, x0, y1, x1;      /* the canvas rectangle [y0, y1) x [x0, x1) it covers                          */
+  int32_t oy, ox;              /* canvas pixel (y, x) of the rectangle is src[y - oy, x - ox]                 */
+} yb_v5_place;
+
+typedef struct {
+  double inv[9];               /* inverse map, as yb_v5_image's                                               */
+  int32_t warp;                /* 0 (no warp: the output is the canvas), YB_V5_AFFINE or YB_V5_PERSPECTIVE     */
+  int32_t n_places;            /* 0..YB_V5_MAX_PLACES, disjoint rectangles                                    */
+  yb_v5_place places[YB_V5_MAX_PLACES];
+} yb_v5_canvas;
+
+typedef struct {
+  uint8_t* dst;
+  int64_t dst_stride_y, dst_stride_x, dst_stride_c;
+  int32_t out_h, out_w;        /* the same for every sample of a launch                                       */
+  int32_t ops;                 /* YB_V5_TO_HSV, _LUT, _FROM_HSV, _RGB, _FLIP_LR, _FLIP_UD                      */
+  int32_t n_canvases;          /* 1, or 2: mixup of canvas 0 (ratio mix_r) and canvas 1 (1 - mix_r)           */
+  double mix_r, mix_omr;       /* r and 1 - r as numpy computes it                                            */
+  yb_v5_canvas canvas[2];
+  uint8_t lut[3][256];
+} yb_v5_sample;
+
+/* Host-only: checks the descriptors; *blocks_per_sample = the launch's blocks per sample. */
+int yb_v5_compose_prepare(int n_samples, const yb_v5_sample* samples, int64_t* blocks_per_sample);
+
+/* Computes every sample in one launch.  samples_dev: the descriptors on the device.  No host synchronisation; a
+ * repeated call writes the same bits. */
+int yb_v5_compose(int n_samples, const yb_v5_sample* samples_dev, int64_t blocks_per_sample, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -74,6 +74,10 @@ EXPORTED_SYMBOLS = (
     "yb_v5_augment_prepare",
     "yb_v5_augment",
     "yb_v5_mixup",
+    "yb_v5_resize_prepare",
+    "yb_v5_resize",
+    "yb_v5_compose_prepare",
+    "yb_v5_compose",
     "yb_conv_wgrad_workspace_bytes",
     "yb_conv_wgrad_config",
     "yb_conv_wgrad",
@@ -298,6 +302,48 @@ class V5Image(ctypes.Structure):
     ]
 
 
+YB_V5_MAX_PLACES = 4
+
+
+class V5ResizeJob(ctypes.Structure):
+    """yb_v5_resize_job: one cv2.resize(INTER_LINEAR) of load_image (include/yolort_b200.h)."""
+    _fields_ = [
+        ("src", ctypes.c_void_p), ("dst", ctypes.c_void_p),
+        ("src_stride_y", ctypes.c_int64), ("src_stride_x", ctypes.c_int64), ("src_stride_c", ctypes.c_int64),
+        ("src_h", ctypes.c_int32), ("src_w", ctypes.c_int32), ("dst_h", ctypes.c_int32), ("dst_w", ctypes.c_int32),
+        ("block_start", ctypes.c_int32), ("reserved", ctypes.c_int32),
+    ]
+
+
+class V5Place(ctypes.Structure):
+    """yb_v5_place: one image placed on a virtual canvas (include/yolort_b200.h)."""
+    _fields_ = [
+        ("src", ctypes.c_void_p),
+        ("stride_y", ctypes.c_int64), ("stride_x", ctypes.c_int64), ("stride_c", ctypes.c_int64),
+        ("y0", ctypes.c_int32), ("x0", ctypes.c_int32), ("y1", ctypes.c_int32), ("x1", ctypes.c_int32),
+        ("oy", ctypes.c_int32), ("ox", ctypes.c_int32),
+    ]
+
+
+class V5Canvas(ctypes.Structure):
+    """yb_v5_canvas: a virtual canvas and its inverse warp (include/yolort_b200.h)."""
+    _fields_ = [
+        ("inv", ctypes.c_double * 9), ("warp", ctypes.c_int32), ("n_places", ctypes.c_int32),
+        ("places", V5Place * YB_V5_MAX_PLACES),
+    ]
+
+
+class V5Sample(ctypes.Structure):
+    """yb_v5_sample: one training sample of the compose kernel (include/yolort_b200.h)."""
+    _fields_ = [
+        ("dst", ctypes.c_void_p),
+        ("dst_stride_y", ctypes.c_int64), ("dst_stride_x", ctypes.c_int64), ("dst_stride_c", ctypes.c_int64),
+        ("out_h", ctypes.c_int32), ("out_w", ctypes.c_int32), ("ops", ctypes.c_int32), ("n_canvases", ctypes.c_int32),
+        ("mix_r", ctypes.c_double), ("mix_omr", ctypes.c_double), ("canvas", V5Canvas * 2),
+        ("lut", (ctypes.c_uint8 * 256) * 3),
+    ]
+
+
 class WgradProblem(ctypes.Structure):
     """yb_wgrad_problem: one 1x1-convolution weight gradient (include/yolort_b200.h)."""
     _fields_ = [
@@ -406,6 +452,10 @@ def lib() -> ctypes.CDLL:
     L.yb_v5_augment.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
     L.yb_v5_mixup.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_double,
                               ctypes.c_void_p]
+    L.yb_v5_resize_prepare.argtypes = [ctypes.c_int, ctypes.POINTER(V5ResizeJob), ctypes.POINTER(ctypes.c_int64)]
+    L.yb_v5_resize.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
+    L.yb_v5_compose_prepare.argtypes = [ctypes.c_int, ctypes.POINTER(V5Sample), ctypes.POINTER(ctypes.c_int64)]
+    L.yb_v5_compose.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
     L.yb_conv_wgrad_workspace_bytes.restype = ctypes.c_size_t
     L.yb_conv_wgrad_workspace_bytes.argtypes = [ctypes.POINTER(WgradProblem), ctypes.c_int]
     L.yb_conv_wgrad_config.argtypes = [ctypes.POINTER(WgradProblem), ctypes.c_int, ctypes.POINTER(ctypes.c_int32)]
@@ -1246,6 +1296,45 @@ def v5_mixup(a: torch.Tensor, b: torch.Tensor, r: float) -> torch.Tensor:
         check(lib().yb_v5_mixup(a.data_ptr(), b.data_ptr(), out.data_ptr(), a.numel(), float(r),
                                 current_stream_ptr(a.device)), "yb_v5_mixup")
     return out
+
+
+def _descs_to_device(descs, device: torch.device) -> torch.Tensor:
+    raw = torch.frombuffer(bytearray(ctypes.string_at(ctypes.addressof(descs), ctypes.sizeof(descs))), dtype=torch.uint8)
+    return raw.pin_memory().to(device, non_blocking=True)
+
+
+def _keep_alive(tensors: Sequence[torch.Tensor], device: torch.device) -> None:
+    stream = torch.cuda.current_stream(device)
+    seen = set()
+    for t in tensors:
+        key = t.untyped_storage().data_ptr()
+        if key not in seen:
+            seen.add(key)
+            t.record_stream(stream)
+
+
+def v5_resize(jobs, tensors: Sequence[torch.Tensor], device: torch.device) -> None:
+    """Runs the load_image resize jobs `jobs` (V5ResizeJob array, pointers set) in one launch; `tensors` are the
+    sources and destinations they point into.  Nothing synchronises."""
+    n = len(jobs)
+    total = ctypes.c_int64(0)
+    check(lib().yb_v5_resize_prepare(n, jobs, ctypes.byref(total)), "yb_v5_resize_prepare")
+    with device_guard(device):
+        d_jobs = _descs_to_device(jobs, device)
+        check(lib().yb_v5_resize(n, d_jobs.data_ptr(), total.value, current_stream_ptr(device)), "yb_v5_resize")
+        _keep_alive(tensors, device)
+
+
+def v5_compose(samples, tensors: Sequence[torch.Tensor], device: torch.device) -> None:
+    """Runs the training-sample descriptors `samples` (V5Sample array, pointers set) in one launch; `tensors` are the
+    placed images and the outputs they point into.  Nothing synchronises."""
+    n = len(samples)
+    blocks = ctypes.c_int64(0)
+    check(lib().yb_v5_compose_prepare(n, samples, ctypes.byref(blocks)), "yb_v5_compose_prepare")
+    with device_guard(device):
+        d_samples = _descs_to_device(samples, device)
+        check(lib().yb_v5_compose(n, d_samples.data_ptr(), blocks.value, current_stream_ptr(device)), "yb_v5_compose")
+        _keep_alive(tensors, device)
 
 
 def wgrad_problems(specs) -> "ctypes.Array":
