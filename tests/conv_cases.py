@@ -16,6 +16,7 @@ from typing import Callable, Optional
 import torch
 import torch.nn.functional as F
 
+from stagewise import act_ref
 from yolort_b200 import _C
 from yolort_b200.engine import pack_bias, pack_weight
 
@@ -307,18 +308,6 @@ def ulp_out(a: torch.Tensor, dtype) -> torch.Tensor:
     return torch.ldexp(torch.ones_like(a), (e - 1 - mant).to(torch.int32))
 
 
-def _act64(v: torch.Tensor, act: int) -> torch.Tensor:
-    if act == SILU:
-        return v * torch.sigmoid(v)
-    if act == HSWISH:
-        return F.hardswish(v)
-    if act == LEAKY:
-        return F.leaky_relu(v, 0.1)
-    if act == RELU:
-        return torch.relu(v)
-    return v
-
-
 def _nchw(t: torch.Tensor) -> torch.Tensor:
     return t.double().permute(0, 3, 1, 2)
 
@@ -417,7 +406,7 @@ def check_case(case: Case, device=torch.device("cuda:0"), legacy_tol=None) -> di
     b = t["b32"].double()
     pre = F.conv2d(x, w, b, c.s, c.pad)
     mag = F.conv2d(x.abs(), w.abs(), b.abs(), c.s, c.pad)
-    ref = _act64(pre, c.act)
+    ref = act_ref(pre, c.act)
     if c.residual:
         r = _nchw(t["res"][..., c.res_off:c.res_off + c.Cout])
         ref, mag = ref + r, mag + r.abs()
@@ -431,7 +420,7 @@ def check_case(case: Case, device=torch.device("cuda:0"), legacy_tol=None) -> di
         a2 = torch.cat([own, out[:c.N, ..., c.extra_off:c.extra_off + ch.c_own]], -1) if ch.extra else own
         a2 = _nchw(a2)
         w2, b2 = t["w2_4"].double(), t["b2_32"].double()
-        ref2 = _act64(F.conv2d(a2, w2, b2), ch.act2)
+        ref2 = act_ref(F.conv2d(a2, w2, b2), ch.act2)
         mag2 = F.conv2d(a2.abs(), w2.abs(), b2.abs())
         got2 = out2[:c.N, ..., :ch.C2].permute(0, 3, 1, 2)
         worst["tail"] = _report("tail", got2, ref2, mag2, a2.shape[1], c.dtype, legacy_tol)

@@ -51,6 +51,36 @@ def assert_dets_close(got, ref, box_atol, score_atol, allow_tie_swaps=False):
     np.testing.assert_allclose(gb, rb, atol=box_atol, rtol=0)
 
 
+def rel_rms(got, ref):
+    """Root mean square of got - ref over that of ref."""
+    return float(np.sqrt(((got - ref) ** 2).mean()) / np.sqrt((ref ** 2).mean()))
+
+
+def head_logits(plan, i, anchors=3, outputs=85):
+    """Head buffer i of `plan` as the reference's [N, A, H, W, K] logits (numpy, fp32)."""
+    h = plan.heads[i][..., :anchors * outputs].float().cpu()
+    n, hh, ww, _ = h.shape
+    return h.view(n, hh, ww, anchors, outputs).permute(0, 3, 1, 2, 4).numpy()
+
+
+def assert_repeat_and_graph_replay_bit_identical(plan):
+    """`plan` (input written) run twice eagerly, then twice as one CUDA graph with its heads zeroed before each replay:
+    every run gives the first run's heads bit for bit."""
+    plan.run()
+    torch.cuda.synchronize()
+    eager = [h.clone() for h in plan.heads]
+    plan.run()
+    torch.cuda.synchronize()
+    assert all(torch.equal(a, b) for a, b in zip(eager, plan.heads))
+    plan.use_graph = True
+    for _ in range(2):
+        for h in plan.heads:
+            h.zero_()
+        plan.run()
+        torch.cuda.synchronize()
+        assert all(torch.equal(a, b) for a, b in zip(eager, plan.heads))
+
+
 def to_np(d):
     return {k: (v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else v) for k, v in d.items()}
 

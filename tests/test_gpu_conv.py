@@ -3,6 +3,7 @@ import pytest
 import torch
 
 import conv_cases as C
+import stagewise as S
 from yolort_b200 import _C
 
 pytestmark = pytest.mark.gpu
@@ -22,11 +23,7 @@ def run_conv(N, H, W, Cin, Cout, k, s, p, dtype=torch.float16, act=True, residua
                   out_off=out_pad // 2 // 8 * 8, seed=seed, bias_scale=bias_scale,
                   reserved=((_C.YB_CONV_FORCE_IM2COL if force_im2col else 0) |
                             (_C.YB_CONV_FORCE_PLANES if force_planes else 0)), **kw)
-    return C.check_case(case, DEV, legacy_tol=_stagewise_tol(dtype))
-
-
-def _stagewise_tol(dtype):
-    return 2.0 ** -9 if dtype == torch.float16 else 2.0 ** -6   # SURVEY.md section 8c stage-wise bound
+    return C.check_case(case, DEV, legacy_tol=S.TOL[dtype])
 
 
 @pytest.mark.parametrize("cin,cout", [(64, 128), (128, 64), (32, 32), (16, 32), (256, 256), (512, 256), (48, 96), (80, 160)])
@@ -177,7 +174,7 @@ def run_chain(N, H, W, Cin, C1, k, c_own, C2, extra=False, residual=False, dtype
     chain = C.Chain(c_own, C2, extra=extra, store_first=store_first, act2=C.SILU if act2 else C.NONE)
     case = C.Case(f"chain N{N} {H}x{W} {Cin}->{C1} k{k} -> [{c_own}{'+' + str(c_own) if extra else ''}]->{C2}",
                   N, H, W, Cin, C1, k=k, dtype=dtype, residual=residual, seed=seed, chain=chain)
-    return C.check_case(case, DEV, legacy_tol=_stagewise_tol(dtype))
+    return C.check_case(case, DEV, legacy_tol=S.TOL[dtype])
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])

@@ -6,7 +6,6 @@ import os
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 import parity_util as util
 import stagewise as S
@@ -16,7 +15,6 @@ from yolort_b200 import _C
 from yolort_b200.models import darknet as D
 
 DEV = "cuda:0"
-MANT = {torch.float16: 10, torch.bfloat16: 7}
 LOGIT_TOL = {torch.float16: 1e-2, torch.bfloat16: 8e-2}
 
 
@@ -31,17 +29,10 @@ def _model(arch, dtype, seed=0, conv_gain=None):
     return m.to(DEV, dtype)
 
 
-def _ulp(r: torch.Tensor, dtype) -> torch.Tensor:
-    """One unit in the last place of the (already rounded) values r of `dtype`, as fp64."""
-    tiny = torch.finfo(dtype).tiny
-    e = torch.floor(torch.log2(r.double().abs().clamp_min(tiny)))
-    return torch.exp2(e - MANT[dtype])
-
-
 def assert_within_1ulp(got, ref64, dtype, what):
     rounded = ref64.to(dtype).double()
     err = (got.double() - rounded).abs()
-    bad = int((err > _ulp(rounded, dtype)).sum())
+    bad = int((err > S.ulp(rounded, dtype)).sum())
     assert bad == 0, f"{what}: {bad} values more than 1 ulp from the fp64 mean (max err {float(err.max()):.3e})"
 
 
@@ -77,52 +68,6 @@ def test_gpu_avgpool_vs_fp64_mean(N, H, W, C, dtype):
     assert torch.equal(ob.view(torch.int16), first.view(torch.int16))
 
 
-def _stem_ref(model, plan, op):
-    """The stem launch against the module's convolution rewritten over the space-to-depth canvas (exact), in fp32."""
-    from yolort_b200.engine import focus_to_s2d, fold_conv_bn, stem_to_s2d
-    from yolort_b200.models.common import Focus
-
-    stem = model.features[0]
-    if isinstance(stem, Focus):
-        w, b = fold_conv_bn(stem.conv)
-        w = focus_to_s2d(w)
-    else:
-        w, b = fold_conv_bn(stem)
-        w = stem_to_s2d(w)
-    return S._act(F.conv2d(S._nchw(plan.input), w.to(plan.dtype).float(), b.float(), 1, 1), op.act)
-
-
-def check_classifier_stagewise(model, plan):
-    """Every launch of a classifier plan right after it ran, against fp32 on its own rounded input: the stem against its
-    s2d rewrite, AVGPOOL against the fp64 mean (1 ulp), every other launch through stagewise._check_op."""
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
-    L = plan._low.L
-    tol = S.TOL[plan.dtype]
-    out = []
-    for li, grp in enumerate(plan.launch_ops):
-        snaps = {i: plan.buffers[L.ops[i].residual.buf.name][..., L.ops[i].residual.ch0:
-                                                              L.ops[i].residual.ch0 + L.ops[i].residual.C].clone()
-                 for i in grp if L.ops[i].residual is not None}
-        plan.run(li, 1)
-        torch.cuda.synchronize()
-        for i in grp:
-            op = L.ops[i]
-            dst = plan.buffers[op.dst.buf.name][..., op.dst.ch0: op.dst.ch0 + op.dst.C]
-            if op.kind == _C.YB_OP_AVGPOOL:
-                src = plan.buffers[op.src.buf.name][..., op.src.ch0: op.src.ch0 + op.src.C]
-                assert_within_1ulp(dst[:, 0, 0], src.double().mean((1, 2)), plan.dtype, op.name)
-                out.append((op.name, 0, 0.0))
-            elif op.pack > 1:
-                ref = _stem_ref(model, plan, op)
-                got = S._nchw(dst)
-                err = (got - ref).abs()
-                out.append((op.name, int((err > tol * (1.0 + ref.abs())).sum()), float(err.max())))
-            else:
-                S._check_op(None, plan, op, snaps.get(i), tol, True, out, fused=len(grp) > 1)
-    return out
-
-
 # darknet_x_r6_0 (12 bottlenecks in its third stage) takes a smaller synthetic gain than the default 1.8 of r6.0: with
 # 1.8 its final features reach 2e4 at 224^2 (1.5: absmax 11), far outside what trained weights produce.
 STAGE_GAIN = {"darknet_x_r6_0": 1.5}
@@ -142,9 +87,9 @@ def test_gpu_stagewise_darknet(arch, N, hw, dtype):
     g = torch.Generator(device=DEV).manual_seed(5)
     plan.input.copy_(torch.rand(plan.input.shape, generator=g, device=DEV).to(dtype))
     plan.input[..., 3::4] = 0
-    res = check_classifier_stagewise(m, plan)
+    res = S.check_plan_stagewise(plan, m.features[0])
     assert len(res) == len(plan._low.L.ops)
-    bad = [r for r in res if r[1]]
+    bad = [r for r in res if r.violations]
     assert not bad, bad
 
 
@@ -211,15 +156,4 @@ def test_gpu_graph_replay_and_repeat_are_bit_identical_darknet():
     g = torch.Generator(device=DEV).manual_seed(6)
     plan.input.copy_(torch.rand(plan.input.shape, generator=g, device=DEV).half())
     plan.input[..., 3::4] = 0
-    plan.run()
-    torch.cuda.synchronize()
-    eager = plan.heads[0].clone()
-    plan.run()
-    torch.cuda.synchronize()
-    assert torch.equal(eager, plan.heads[0])
-    plan.use_graph = True
-    for _ in range(2):
-        plan.heads[0].zero_()
-        plan.run()
-        torch.cuda.synchronize()
-        assert torch.equal(eager, plan.heads[0])
+    util.assert_repeat_and_graph_replay_bit_identical(plan)

@@ -5,22 +5,14 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from stagewise import TOL, act_ref
 from yolort_b200 import _C
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda:0")
-TOL = {torch.float16: 2.0 ** -9, torch.bfloat16: 2.0 ** -6}
 CHANNELS = [8, 16, 40, 72, 88, 120, 144, 288, 576]
 SENTINEL = 7.0
 ACTS = [_C.YB_ACT_NONE, _C.YB_ACT_RELU, _C.YB_ACT_HARDSWISH]
-
-
-def _act(y, code):
-    if code == _C.YB_ACT_RELU:
-        return F.relu(y)
-    if code == _C.YB_ACT_HARDSWISH:
-        return F.hardswish(y)
-    return y
 
 
 def _strided(N, H, W, C, lead, tail, dtype, g):
@@ -68,7 +60,7 @@ def test_dwconv_matches_fp32_conv2d(C, k, s, dtype):
         d.weight, d.bias = wp.data_ptr(), b.data_ptr()
         _C.Plan([d], DEV).run()
         torch.cuda.synchronize()
-        ref = _act(F.conv2d(x.float().permute(0, 3, 1, 2), w.float(), b, s, p, 1, C), act)
+        ref = act_ref(F.conv2d(x.float().permute(0, 3, 1, 2), w.float(), b, s, p, 1, C), act)
         got = dst_buf[..., 16:16 + C].float().permute(0, 3, 1, 2)
         err = (got - ref).abs()
         bad = int((err > tol * (1.0 + ref.abs())).sum())

@@ -1,13 +1,7 @@
 """FP8 (e4m3) inference on the H100: the e4m3 convolution, QUANTIZE, SPP and upsample kernels against fp32 PyTorch on
 the dequantised operands, every launch of FP8 plans at real shapes, and the model-level behaviour (calibration,
-precision switching, hooks, graph replay, stale calibrations).
-
-Bound for e4m3 outputs: within one e4m3 ulp of the fp32 reference v / s_out (floor 2^-9, the subnormal spacing) plus
-2^-10 of sum|x_i w_i| m / s_out, and exactly +-448 where |v / s_out| > 448 (saturation; torch's float8 cast does not
-saturate, so references are clamped).  The second term is the tensor core's: Hopper's e4m3 wgmma does not add the
-products of an instruction in full fp32 (about 13 bits are kept after aligning them, as DeepSeek-V3's report, section
-3.3.2, describes for the same hardware), so where the products cancel, the exact fp32 sum of the reference and the
-kernel's accumulator differ by a few 2^-13 of the magnitude sum.  Measured worst cases are printed."""
+precision switching, hooks, graph replay, stale calibrations).  The bounds of e4m3 and of 16-bit outputs are
+tests/stagewise.py's (e4m3_bound, bound16); measured worst cases are printed."""
 import os
 import sys
 
@@ -15,6 +9,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from stagewise import act_ref, bound16, check_plan_stagewise, compare, e4m3_bound, to_e4m3
 from yolort_b200 import _C
 from yolort_b200.engine import e4m3_scale, pack_weight_e4m3
 
@@ -32,52 +27,6 @@ A = _C
 def _no_tf32():
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
-
-
-def to_e4m3(v):
-    return v.clamp(-448.0, 448.0).to(F8)
-
-
-def ulp_e4m3(v):
-    _, e = torch.frexp(v.abs().clamp(min=2.0 ** -6))
-    return torch.exp2((e - 4).float())
-
-
-def act(y, code):
-    if code == A.YB_ACT_SILU:
-        return F.silu(y)
-    if code == A.YB_ACT_HARDSWISH:
-        return F.hardswish(y)
-    if code == A.YB_ACT_LEAKY01:
-        return F.leaky_relu(y, 0.1)
-    if code == A.YB_ACT_RELU:
-        return F.relu(y)
-    return y
-
-
-def check_e4m3(got_q, ref_scaled, mag_scaled, what):
-    """got_q: e4m3 tensor; ref_scaled: fp32 reference already divided by the output scale; mag_scaled: sum|x_i w_i| m
-    over the same scale.  Returns the worst error over the bound, and the fraction of outputs beyond one ulp."""
-    got = got_q.float()
-    ref = ref_scaled.float()
-    sat = ref.abs() > 448.0 + 2.0 ** -10 * mag_scaled
-    assert torch.equal(got[sat], torch.sign(ref[sat]) * 448.0), f"{what}: saturation"
-    refc = ref.clamp(-448.0, 448.0)
-    err = (got - refc).abs()
-    ulp = torch.maximum(ulp_e4m3(refc), torch.full_like(refc, 2.0 ** -9))
-    bound = ulp + 2.0 ** -10 * mag_scaled
-    bad = int((err > bound).sum())
-    assert bad == 0, f"{what}: {bad}/{err.numel()} outside the bound, max err {float(err.max()):.3e}"
-    return float((err / bound).max()), float((err > ulp).float().mean())
-
-
-def check_wide(got, ref, what, mag=None):
-    """fp16 / bf16 outputs (the heads): the stage-wise bound of the fp16 / bf16 plans, 2^-9 / 2^-6 x (1 + |ref|), plus
-    the accumulation term 2^-10 sum|x_i w_i| m when `mag` is given."""
-    tol = 2.0 ** -9 if got.dtype == torch.float16 else 2.0 ** -6
-    err = (got.float() - ref).abs()
-    bad = int((err > tol * (1.0 + ref.abs()) + (0.0 if mag is None else 2.0 ** -10 * mag)).sum())
-    assert bad == 0, f"{what}: {bad}/{err.numel()} outside {tol} (1 + |ref|), max err {float(err.max()):.3e}"
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -123,7 +72,7 @@ def conv_case(k, s, cin, cout, out, residual, act_code, shape, seed=0):
     m = (s_w * s_in).float().to(DEV)
     xs = xbuf[..., PAD:PAD + cin].float().permute(0, 3, 1, 2)
     ws = wq[:cout, :, :cin].float().view(cout, k, k, cin).permute(0, 3, 1, 2)
-    v = act(F.conv2d(xs, ws, None, s, p) * m.view(1, -1, 1, 1) + bias.float().to(DEV).view(1, -1, 1, 1), act_code)
+    v = act_ref(F.conv2d(xs, ws, None, s, p) * m.view(1, -1, 1, 1) + bias.float().to(DEV).view(1, -1, 1, 1), act_code)
     mag = F.conv2d(xs.abs(), ws.abs(), None, s, p) * m.view(1, -1, 1, 1)
     s_res, rbuf = 0.0, None
     if residual:
@@ -164,12 +113,14 @@ def test_e4m3_conv_matches_fp32_on_dequantised_operands(case):
     d, keep, v, s_out, obuf = conv_case(*case)
     _C.Plan([d], DEV).run()
     torch.cuda.synchronize()
-    got = obuf[..., PAD:PAD + cout].permute(0, 3, 1, 2)
+    got = obuf[..., PAD:PAD + cout].permute(0, 3, 1, 2).float()
     if out == "e4m3":
-        worst, beyond_ulp = check_e4m3(got, v / s_out, keep[-1] / s_out, str(case))
-        print(f"{case}: worst {worst:.3f} of the bound, {beyond_ulp:.2e} of the outputs beyond one ulp")
+        ref, bound = e4m3_bound(v / s_out, keep[-1] / s_out)
     else:
-        check_wide(got, v, str(case), keep[-1])
+        ref, bound = v, bound16(v, obuf.dtype, keep[-1])
+    bad, mx, worst = compare(got, ref, bound)
+    print(f"{case}: worst {worst:.3f} of the bound")
+    assert bad == 0, f"{case}: {bad}/{got.numel()} outside the bound, max err {mx:.3e}"
     full = obuf.float()
     assert torch.all(full[..., :PAD] == full[0, 0, 0, 0]) and torch.all(full[..., PAD + cout:] == full[0, 0, 0, 0])
     assert float(full[0, 0, 0, 0]) == (1.75 if out == "e4m3" else 7.0), "sentinels overwritten"
@@ -246,56 +197,6 @@ def test_upsample2x_e4m3_exact():
 # ---------------------------------------------------------------------------------------------------------------------
 # every launch of FP8 plans at real shapes
 # ---------------------------------------------------------------------------------------------------------------------
-def check_fp8_plan_stagewise(plan):
-    """`plan`: an FP8 plan with keep_intermediates=True and its input written.  Runs it one launch at a time and checks
-    each launch on its own inputs: QUANTIZE / SPP / upsample exactly, e4m3 convolutions within one e4m3 ulp, the heads'
-    fp16 / bf16 logits within 2^-9 (1 + |ref|).  The stem is the fp16 / bf16 kernel of the other plans."""
-    Lw = plan._low.L
-    worst, beyond = 0.0, 0.0
-    for li, grp in enumerate(plan.launch_ops):
-        op = Lw.ops[grp[0]]
-        res = None
-        if op.residual is not None:
-            r = op.residual
-            res = plan.buffers[r.buf.name][..., r.ch0:r.ch0 + r.C].clone()
-        plan.run(li, 1)
-        torch.cuda.synchronize()
-        if op.kind == A.YB_OP_CONV and op.dtype is None:
-            continue
-        src = plan.buffers[op.src.buf.name][..., op.src.ch0:op.src.ch0 + op.src.C]
-        dst = plan.buffers[op.dst.buf.name][..., op.dst.ch0:op.dst.ch0 + op.dst.C]
-        if op.kind == A.YB_OP_QUANTIZE:
-            assert torch.equal(_bits(dst), _bits(to_e4m3(src.float() * float(op.bias[0])))), op.name
-        elif op.kind == A.YB_OP_SPP_POOL:
-            x = src.float().permute(0, 3, 1, 2)
-            ref = torch.cat([F.max_pool2d(x, k, 1, k // 2) for k in (5, 9, 13)], 1)
-            assert torch.equal(dst.float().permute(0, 3, 1, 2), ref), op.name
-        elif op.kind == A.YB_OP_UPSAMPLE2X:
-            ref = src.view(torch.uint8).repeat_interleave(2, 1).repeat_interleave(2, 2)
-            assert torch.equal(dst.view(torch.uint8), ref), op.name
-        else:
-            co, ci, k = op.dst.C, op.src.C, op.ksize
-            co_pad = op.weight.shape[0]
-            w = op.weight[:co, :, :ci].float().view(co, k, k, ci).permute(0, 3, 1, 2)
-            tail = op.bias
-            xs = src.float().permute(0, 3, 1, 2)
-            mul = tail[co_pad:co_pad + co].view(1, -1, 1, 1)
-            v = act(F.conv2d(xs, w, None, op.stride, op.pad) * mul + tail[:co].view(1, -1, 1, 1), op.act)
-            if res is not None:
-                v = v + res.float().permute(0, 3, 1, 2) * float(tail[2 * co_pad])
-            got = dst.permute(0, 3, 1, 2)
-            inv = float(tail[2 * co_pad + 1])
-            mag = F.conv2d(xs.abs(), w.abs(), None, op.stride, op.pad) * mul * inv
-            if op.dst.buf.esz == 1:
-                r, f = check_e4m3(got, v * inv, mag, op.name)
-                worst, beyond = max(worst, r), max(beyond, f)
-            else:
-                check_wide(got, v, op.name, mag)
-            del mag
-            del v, w, xs
-    return worst, beyond
-
-
 def _fp8_model(ctor_name, gain=None, dtype=torch.float16, **kw):
     import bench
     from yolort_b200 import models
@@ -327,9 +228,10 @@ def test_every_launch_of_fp8_plans(ctor, version, gain, batch, size):
     assert plan._low.fp8
     geoms, (Hb, Wb) = m.transform.geometry(ims, None)
     m.transform.letterbox_into(ims, geoms, Hb, Wb, plan.input, _C.YB_LAYOUT_S2D16)
-    worst, beyond = check_fp8_plan_stagewise(plan)
-    print(f"{ctor} {version} b{batch} {size}: worst error {worst:.3f} of the bound; at most {beyond:.2e} of a launch's "
-          f"outputs beyond one e4m3 ulp")
+    res = check_plan_stagewise(plan, m.model.backbone.body["0"])
+    assert len(res) == len(plan._low.L.ops)
+    bad = [r for r in res if r.violations]
+    assert not bad, bad
 
 
 # ---------------------------------------------------------------------------------------------------------------------

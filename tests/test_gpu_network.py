@@ -13,7 +13,7 @@ DEV = "cuda:0"
 
 def _stats(name, got, ref):
     err = np.abs(got - ref)
-    rel_rms = float(np.sqrt((err ** 2).mean()) / (np.sqrt((ref ** 2).mean()) + 1e-12))
+    rel_rms = util.rel_rms(got, ref)
     print(f"{name}: max_abs={err.max():.4f} rel_rms={rel_rms:.2e} ref_rms={np.sqrt((ref ** 2).mean()):.3f}")
     return float(err.max()), rel_rms
 
@@ -38,10 +38,7 @@ def test_features_and_heads_vs_reference_fixture():
         mx, rr = _stats(key, got, z[key])
         assert rr < 1.5e-2      # fp16 activations through 20-30 layers vs the fp32 reference
     for i in range(3):
-        h = plan.heads[i][..., :255].float().cpu()
-        n, hh, ww, _ = h.shape
-        got = h.view(n, hh, ww, 3, 85).permute(0, 3, 1, 2, 4).numpy()
-        mx, rr = _stats(f"head{i}", got, z[f"h{i}"])
+        mx, rr = _stats(f"head{i}", util.head_logits(plan, i), z[f"h{i}"])
         assert rr < 1.5e-2
     ref = util.dets_from_npz(z, 1)[0]
     frac = util.match_fraction(util.to_np(dets[0]), ref, iou_thr=0.9, side=128)

@@ -13,6 +13,7 @@ import torch
 import torch.nn.functional as F
 
 import parity_util as util
+import stagewise as S
 from oracle import restate_lite as RL
 from oracle.make_golden_lite import (NUM_CLASSES, SCORE_THRESH, SIZE, e2e_input, network_input, stored_part,
                                      synth_state_dict_lite)
@@ -300,75 +301,6 @@ def _model():
     return m.to(DEV)
 
 
-def _act(y, code):
-    if code == _C.YB_ACT_RELU:
-        return F.relu(y)
-    if code == _C.YB_ACT_HARDSWISH:
-        return F.hardswish(y)
-    return y
-
-
-def _stagewise_lite(model, plan):
-    """Every launch of a lite plan right after it ran, against fp32 on its own rounded input (tests/stagewise.py's
-    check).  Handled here: the stem (against the module's own 3x3/s2 convolution over the canvas), the ReLU
-    convolutions, the depthwise convolutions (F.conv2d(groups=C) with the op's rounded weights) and SE (in place: against
-    its input snapshot).  Every other launch goes through stagewise._check_op."""
-    import stagewise as S
-    from yolort_b200.engine import _fold_conv_norm, _split_conv_norm_act
-
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
-    L = plan._low.L
-    tol = S.TOL[plan.dtype]
-    out = []
-    for li, grp in enumerate(plan.launch_ops):
-        assert len(grp) == 1
-        op = L.ops[grp[0]]
-
-        def view(v):
-            return plan.buffers[v.buf.name][..., v.ch0: v.ch0 + v.C]
-
-        snap = view(op.src).clone() if op.kind in (_C.YB_OP_SE, _C.YB_OP_DWCONV) or op.act == _C.YB_ACT_RELU else None
-        res = view(op.residual).clone() if op.residual is not None else None
-        plan.run(li, 1)
-        torch.cuda.synchronize()
-        got = S._nchw(view(op.dst))
-        if op.pack > 1:
-            conv, bn, _ = _split_conv_norm_act("stem", model.backbone.body["0"])
-            w, b = _fold_conv_norm(conv, bn)
-            s2d = plan.input.float()
-            n, h2, w2, _ = s2d.shape
-            x = s2d.view(n, h2, w2, 2, 2, 4)[..., :3].permute(0, 5, 1, 3, 2, 4).reshape(n, 3, 2 * h2, 2 * w2)
-            ref = _act(F.conv2d(x, w.to(plan.dtype).float(), b.float(), 2, 1), op.act)
-        elif op.kind == _C.YB_OP_DWCONV:
-            C, k = op.src.C, op.ksize
-            w = op.weight.float().t().reshape(C, 1, k, k)
-            ref = _act(F.conv2d(S._nchw(snap), w, op.bias, op.stride, op.pad, 1, C), op.act)
-        elif op.kind == _C.YB_OP_SE:
-            C, Sq = op.src.C, op.ksize
-            w1 = op.weight[:C * Sq].view(C, Sq).t()
-            w2 = op.weight[C * Sq:].view(Sq, C).t()
-            b1, b2 = op.bias[:Sq], op.bias[Sq:]
-            xf = S._nchw(snap)
-            gate = F.hardsigmoid(F.relu(xf.mean((2, 3)) @ w1.t() + b1) @ w2.t() + b2)
-            ref = xf * gate[:, :, None, None]
-        elif op.act == _C.YB_ACT_RELU:
-            co, ci, k = op.dst.C, op.src.C, op.ksize
-            w = op.weight[:co, :, :ci].float().view(co, k, k, ci).permute(0, 3, 1, 2).contiguous()
-            ref = F.relu(F.conv2d(S._nchw(snap), w, op.bias[:co], op.stride, op.pad))
-            if res is not None:
-                ref = ref + S._nchw(res)
-        else:
-            S._check_op(model, plan, op, res, tol, True, out)
-            continue
-        err = (got - ref).abs()
-        bad = int((err > tol * (1.0 + ref.abs())).sum())
-        if bad:
-            print(f"  stage {op.name}: violations {bad}/{err.numel()} max_abs_err {float(err.max()):.3e}")
-        out.append((op.name, bad, float(err.max())))
-    return out
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("N,hw,dtype", [(32, 640, torch.float16), (8, 1280, torch.bfloat16)])
 def test_gpu_stagewise_lite(N, hw, dtype):
@@ -380,14 +312,10 @@ def test_gpu_stagewise_lite(N, hw, dtype):
     g = torch.Generator(device=DEV).manual_seed(3)
     plan.input.copy_(torch.rand(plan.input.shape, generator=g, device=DEV).to(dtype))
     plan.input[..., 3::4] = 0
-    res = _stagewise_lite(m, plan)
-    assert len(res) == 55
-    bad = [r for r in res if r[1]]
+    res = S.check_plan_stagewise(plan, m.backbone.body["0"])
+    assert len(res) == len(plan._low.L.ops) == 55
+    bad = [r for r in res if r.violations]
     assert not bad, bad
-
-
-def _rel_rms(got, ref):
-    return float(np.sqrt(((got - ref) ** 2).mean()) / np.sqrt((ref ** 2).mean()))
 
 
 @pytest.mark.gpu
@@ -401,10 +329,8 @@ def test_gpu_heads_vs_reference_fixture_lite():
     torch.cuda.synchronize()
     for i, key in enumerate(("0", "1", "2", "pool")):
         got = plan.features[key].float().permute(0, 3, 1, 2).cpu().numpy()
-        rr = _rel_rms(stored_part(f"f{i}", got), z[f"f{i}"])
-        h = plan.heads[i][..., :255].float().cpu()
-        goth = h.view(*h.shape[:3], 3, 85).permute(0, 3, 1, 2, 4).numpy()
-        rh = _rel_rms(stored_part(f"h{i}", goth), z[f"h{i}"])
+        rr = util.rel_rms(stored_part(f"f{i}", got), z[f"f{i}"])
+        rh = util.rel_rms(stored_part(f"h{i}", util.head_logits(plan, i)), z[f"h{i}"])
         print(f"lite f{i} rel_rms {rr:.2e}  h{i} rel_rms {rh:.2e}")
         assert rr < 2e-2 and rh < 2e-2
     frac = util.match_fraction(util.to_np(dets[0]), util.dets_from_npz(z, 1)[0], iou_thr=0.9)
@@ -458,16 +384,4 @@ def test_gpu_graph_replay_and_repeat_are_bit_identical_lite():
     g = torch.Generator(device=DEV).manual_seed(4)
     plan.input.copy_(torch.rand(plan.input.shape, generator=g, device=DEV).half())
     plan.input[..., 3::4] = 0
-    plan.run()
-    torch.cuda.synchronize()
-    eager = [h.clone() for h in plan.heads]
-    plan.run()
-    torch.cuda.synchronize()
-    assert all(torch.equal(a, b) for a, b in zip(eager, plan.heads))
-    plan.use_graph = True
-    for _ in range(2):
-        for h in plan.heads:
-            h.zero_()
-        plan.run()
-        torch.cuda.synchronize()
-        assert all(torch.equal(a, b) for a, b in zip(eager, plan.heads))
+    util.assert_repeat_and_graph_replay_bit_identical(plan)

@@ -10,9 +10,9 @@ import os
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 import parity_util as util
+import stagewise as S
 from oracle import restate_ts as RT
 from oracle.make_golden_ts import SCORE_THRESH, SIZE, e2e_images, network_input, stored_part, synth_state_dict_ts
 from oracle.restate import postprocess
@@ -228,55 +228,6 @@ def _model():
     return m.to(DEV)
 
 
-def _stagewise_ts(model_yolo, plan):
-    """Stage-wise parity of a yolov5ts plan (the check of tests/stagewise.py, launch by launch right after it ran).
-    Two launches are checked here: the r4.0 Focus stem, as the 3x3/s1/p1 convolution over the space-to-depth canvas
-    (focus_to_s2d), and the attention op, against fp32 SDPA on its own rounded q | k | v with the error scale
-    1 + A(|V|) (its outputs are sums of values of both signs and can cancel).  Every other launch goes through
-    stagewise._check_op."""
-    import stagewise as S
-    from yolort_b200.engine import fold_conv_bn, focus_to_s2d
-
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
-    L = plan._low.L
-    tol = S.TOL[plan.dtype]
-    out = []
-    for li, grp in enumerate(plan.launch_ops):
-        snaps = {}
-        for i in grp:
-            op = L.ops[i]
-            if op.residual is not None:
-                snaps[i] = plan.buffers[op.residual.buf.name][..., op.residual.ch0: op.residual.ch0 + op.residual.C].clone()
-        plan.run(li, 1)
-        torch.cuda.synchronize()
-        for i in grp:
-            op = L.ops[i]
-            dst = plan.buffers[op.dst.buf.name][..., op.dst.ch0: op.dst.ch0 + op.dst.C]
-            if op.pack > 1:
-                w, b = fold_conv_bn(model_yolo.backbone.body["0"].conv)
-                ref = S._act(F.conv2d(S._nchw(plan.input), focus_to_s2d(w).to(plan.dtype).float(), b.float(), 1, 1), op.act)
-                scale = 1.0 + ref.abs()
-            elif op.kind == _C.YB_OP_ATTENTION:
-                src = plan.buffers[op.src.buf.name][..., op.src.ch0: op.src.ch0 + op.src.C]
-                n, h, w, _ = src.shape
-                E, heads = op.dst.C, op.ksize
-                qkv = src.float().reshape(n, h * w, 3, heads, E // heads).permute(2, 0, 3, 1, 4)
-                o = F.scaled_dot_product_attention(qkv[0], qkv[1], qkv[2])
-                oa = F.scaled_dot_product_attention(qkv[0], qkv[1], qkv[2].abs())
-                ref = o.permute(0, 2, 1, 3).reshape(n, h, w, E).permute(0, 3, 1, 2)
-                scale = 1.0 + oa.permute(0, 2, 1, 3).reshape(n, h, w, E).permute(0, 3, 1, 2)
-            else:
-                S._check_op(model_yolo, plan, op, snaps.get(i), tol, True, out, fused=len(grp) > 1)
-                continue
-            err = (S._nchw(dst) - ref).abs()
-            bad = int((err > tol * scale).sum())
-            if bad:
-                print(f"  stage {op.name}: violations {bad}/{err.numel()} max_abs_err {float(err.max()):.3e}")
-            out.append((op.name, bad, float(err.max())))
-    return out
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("N,hw,dtype", [(32, 640, torch.float16), (4, 1280, torch.bfloat16)])
 def test_gpu_stagewise_ts(N, hw, dtype):
@@ -291,10 +242,11 @@ def test_gpu_stagewise_ts(N, hw, dtype):
     g = torch.Generator(device=DEV).manual_seed(3)
     plan.input.copy_(torch.rand(plan.input.shape, generator=g, device=DEV).to(dtype))
     plan.input[..., 3::4] = 0
-    res = _stagewise_ts(m.model, plan)
-    att = [r for r in res if "attention" in r[0]]
+    res = S.check_plan_stagewise(plan, m.model.backbone.body["0"])
+    assert len(res) == len(plan._low.L.ops)
+    att = [r for r in res if "attention" in r.name]
     assert len(att) == 1
-    bad = [r for r in res if r[1]]
+    bad = [r for r in res if r.violations]
     assert not bad, bad
 
 
@@ -307,16 +259,10 @@ def test_gpu_heads_vs_reference_fixture_ts():
     plan = m.model.get_plan(1, *SIZE)
     m.model.run_plan(plan)
     torch.cuda.synchronize()
-
-    def rel_rms(got, ref):
-        return float(np.sqrt(((got - ref) ** 2).mean()) / np.sqrt((ref ** 2).mean()))
-
     for i in range(3):
         got = plan.features[f"p{i + 3}"].float().permute(0, 3, 1, 2).cpu().numpy()
-        rr = rel_rms(stored_part(f"p{i + 3}", got), z[f"p{i + 3}"])
-        h = plan.heads[i][..., :255].float().cpu()
-        goth = h.view(*h.shape[:3], 3, 85).permute(0, 3, 1, 2, 4).numpy()
-        rh = rel_rms(stored_part(f"h{i}", goth), z[f"h{i}"])
+        rr = util.rel_rms(stored_part(f"p{i + 3}", got), z[f"p{i + 3}"])
+        rh = util.rel_rms(stored_part(f"h{i}", util.head_logits(plan, i)), z[f"h{i}"])
         print(f"ts p{i + 3} rel_rms {rr:.2e}  h{i} rel_rms {rh:.2e}")
         assert rr < 2e-2 and rh < 2e-2
     frac = util.match_fraction(util.to_np(dets[0]), util.dets_from_npz(z, 1)[0], iou_thr=0.9)
@@ -351,16 +297,4 @@ def test_gpu_graph_replay_and_repeat_are_bit_identical_ts():
     g = torch.Generator(device=DEV).manual_seed(4)
     plan.input.copy_(torch.rand(plan.input.shape, generator=g, device=DEV).half())
     plan.input[..., 3::4] = 0
-    plan.run()
-    torch.cuda.synchronize()
-    eager = [h.clone() for h in plan.heads]
-    plan.run()
-    torch.cuda.synchronize()
-    assert all(torch.equal(a, b) for a, b in zip(eager, plan.heads))
-    plan.use_graph = True
-    for _ in range(2):
-        for h in plan.heads:
-            h.zero_()
-        plan.run()
-        torch.cuda.synchronize()
-        assert all(torch.equal(a, b) for a, b in zip(eager, plan.heads))
+    util.assert_repeat_and_graph_replay_bit_identical(plan)

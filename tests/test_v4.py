@@ -118,12 +118,8 @@ def test_gpu_heads_vs_reference_fixture_v4(tag, ver):
     torch.cuda.synchronize()
     for i in range(3):
         got = plan.features[f"p{i + 3}"].float().permute(0, 3, 1, 2).cpu().numpy()
-        ref = z[f"p{i + 3}"]
-        rr = float(np.sqrt(((got - ref) ** 2).mean()) / np.sqrt((ref ** 2).mean()))
-        h = plan.heads[i][..., :255].float().cpu()
-        goth = h.view(*h.shape[:3], 3, 85).permute(0, 3, 1, 2, 4).numpy()
-        refh = z[f"h{i}"]
-        rh = float(np.sqrt(((goth - refh) ** 2).mean()) / np.sqrt((refh ** 2).mean()))
+        rr = util.rel_rms(got, z[f"p{i + 3}"])
+        rh = util.rel_rms(util.head_logits(plan, i), z[f"h{i}"])
         print(f"{tag} p{i + 3} rel_rms {rr:.2e}  h{i} rel_rms {rh:.2e}")
         assert rr < 2e-2 and rh < 2e-2
     ref = util.dets_from_npz(z, 1)[0]
