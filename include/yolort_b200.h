@@ -800,6 +800,40 @@ int yb_v5_compose_prepare(int n_samples, const yb_v5_sample* samples, int64_t* b
  * repeated call writes the same bits. */
 int yb_v5_compose(int n_samples, const yb_v5_sample* samples_dev, int64_t blocks_per_sample, void* stream);
 
+/* YOLOv5's AutoAnchor (yolort/v5/utils/autoanchor.py; yolort_b200/v5/utils/autoanchor.py draws every random number on
+ * the host): csrc/autoanchor.cu, restated in oracle/restate_autoanchor.py.  Labels are float32 (w, h) pairs. */
+#define YB_AA_MAX_ANCHORS 64
+#define YB_AA_METRIC_WORKSPACE 65536
+
+/* The ratio metric of n labels against n_anchors (w, h) anchors: x = min(r, 1 / r) over both sides, r = label / anchor,
+ * best = max over the anchors.  f64 = 0: in float32 (the anchors hold float32 values), the threshold compared as float32;
+ * f64 = 1: in float64.  counts_dev[2] = {labels with best > thr, (label, anchor) pairs with x > thr};
+ * sums_dev[3] = {sum x, sum best, sum of x > thr} in float64, added in a fixed order.  workspace: YB_AA_METRIC_WORKSPACE
+ * bytes of device memory. */
+int yb_anchor_metric(const float* wh_dev, int64_t n, const double* anchors_dev, int n_anchors, int f64, double thr,
+                     int64_t* counts_dev, double* sums_dev, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Device bytes yb_kmeans needs for n_obs observations, k codes and `trials` trials (0: invalid). */
+size_t yb_kmeans_workspace_bytes(int64_t n_obs, int k, int trials);
+
+/* scipy.cluster.vq.kmeans's trials (_kmeans from each starting book guess_dev[trials, k, 2]) over the float64 (x, y)
+ * observations, all trials at once, bit for bit.  Outputs per trial: books_dev[trials, k, 2] (the first sizes_dev[t]
+ * rows hold the final book), dist_dev[trials] (the final mean distortion); *iters: iterations launched.  The host
+ * reads a device count of live trials every check_every iterations and never otherwise waits. */
+int yb_kmeans(const double* obs_dev, int64_t n_obs, int k, int trials, const double* guess_dev, double thresh,
+              int check_every, double* books_dev, int32_t* sizes_dev, double* dist_dev, int32_t* iters,
+              void* workspace, size_t workspace_bytes, void* stream);
+
+/* kmean_anchors' genetic evolution, `gen` generations in one cooperative launch.  k0_dev[n_anchors, 2]: the starting
+ * anchors (float64); v_dev[gen, n_anchors, 2]: the mutation factors drawn on the host.  Generation g evaluates
+ * kg = max(k * v[g], 2) in float64, its float32 fitness fl32(fl32(S) / n) with S the exact sum of the labels' best
+ * ratios above thr (float32 arithmetic), and keeps kg when the fitness is larger.  unit_exp: floor(log2(thr)) - 23,
+ * the fixed-point unit of that sum.  Outputs: fit_dev[gen + 1] (the fitness after each generation, [0]: the start),
+ * accepted_dev[gen] (1 where kg was kept), k_out_dev[n_anchors, 2].  workspace: (gen + 1) * 8 bytes. */
+int yb_anchor_evolve(const float* wh_dev, int64_t n, int n_anchors, const double* k0_dev, const double* v_dev, int gen,
+                     double thr, int unit_exp, float* fit_dev, uint8_t* accepted_dev, double* k_out_dev,
+                     void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

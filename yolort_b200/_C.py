@@ -81,6 +81,10 @@ EXPORTED_SYMBOLS = (
     "yb_conv_wgrad_workspace_bytes",
     "yb_conv_wgrad_config",
     "yb_conv_wgrad",
+    "yb_anchor_metric",
+    "yb_kmeans_workspace_bytes",
+    "yb_kmeans",
+    "yb_anchor_evolve",
 )
 
 
@@ -461,6 +465,17 @@ def lib() -> ctypes.CDLL:
     L.yb_conv_wgrad_config.argtypes = [ctypes.POINTER(WgradProblem), ctypes.c_int, ctypes.POINTER(ctypes.c_int32)]
     L.yb_conv_wgrad.argtypes = [ctypes.POINTER(WgradProblem), ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t,
                                 ctypes.c_void_p]
+    L.yb_anchor_metric.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                   ctypes.c_double, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t,
+                                   ctypes.c_void_p]
+    L.yb_kmeans_workspace_bytes.restype = ctypes.c_size_t
+    L.yb_kmeans_workspace_bytes.argtypes = [ctypes.c_int64, ctypes.c_int, ctypes.c_int]
+    L.yb_kmeans.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_double,
+                            ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                            ctypes.POINTER(ctypes.c_int32), ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
+    L.yb_anchor_evolve.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
+                                   ctypes.c_int, ctypes.c_double, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
+                                   ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
     _lib = L
     return L
 
@@ -1384,3 +1399,66 @@ def conv_wgrad(specs, device: torch.device) -> None:
     with device_guard(device):
         ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=device)
         check(lib().yb_conv_wgrad(probs, n, ws.data_ptr(), ws_bytes, current_stream_ptr(device)), "yb_conv_wgrad")
+
+
+# ---------------------------------------------------------------------------------------------------
+# AutoAnchor (csrc/autoanchor.cu)
+YB_AA_MAX_ANCHORS = 64
+YB_AA_METRIC_WORKSPACE = 65536
+
+
+def anchor_metric(wh: torch.Tensor, anchors: torch.Tensor, thr: float, f64: bool):
+    """(counts int64[2], sums float64[3]) of the ratio metric: labels with best > thr, (label, anchor) pairs with
+    x > thr; sum x, sum best, sum of the x > thr.  wh: float32 [n, 2] on the device; anchors: float64 [na, 2] (holding
+    float32 values when f64 is False)."""
+    require_cuda(wh, "anchor_metric")
+    dev = wh.device
+    anchors = anchors.to(dev, torch.float64).contiguous()
+    counts = torch.empty(2, dtype=torch.int64, device=dev)
+    sums = torch.empty(3, dtype=torch.float64, device=dev)
+    ws = torch.empty(YB_AA_METRIC_WORKSPACE, dtype=torch.uint8, device=dev)
+    with device_guard(dev):
+        check(lib().yb_anchor_metric(wh.data_ptr(), wh.shape[0], anchors.data_ptr(), anchors.shape[0], int(f64),
+                                     float(thr), counts.data_ptr(), sums.data_ptr(), ws.data_ptr(), ws.numel(),
+                                     current_stream_ptr(dev)), "yb_anchor_metric")
+    return counts, sums
+
+
+def kmeans(obs: torch.Tensor, guesses: torch.Tensor, thresh: float = 1e-5, check_every: int = 8):
+    """scipy.cluster.vq._kmeans from each starting book guesses[t] (float64 [trials, k, 2]) over the float64 [n, 2]
+    observations on the device: (books [trials, k, 2], sizes int32 [trials], distortions float64 [trials], iterations)."""
+    require_cuda(obs, "kmeans")
+    dev = obs.device
+    trials, k = int(guesses.shape[0]), int(guesses.shape[1])
+    guesses = guesses.to(dev, torch.float64).contiguous()
+    books = torch.empty_like(guesses)
+    sizes = torch.empty(trials, dtype=torch.int32, device=dev)
+    dist = torch.empty(trials, dtype=torch.float64, device=dev)
+    nbytes = lib().yb_kmeans_workspace_bytes(obs.shape[0], k, trials)
+    if nbytes == 0:
+        raise ValueError(f"kmeans: {obs.shape[0]} observations, {k} codes, {trials} trials")
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    iters = ctypes.c_int32(0)
+    with device_guard(dev):
+        check(lib().yb_kmeans(obs.data_ptr(), obs.shape[0], k, trials, guesses.data_ptr(), float(thresh), int(check_every),
+                              books.data_ptr(), sizes.data_ptr(), dist.data_ptr(), ctypes.byref(iters), ws.data_ptr(),
+                              nbytes, current_stream_ptr(dev)), "yb_kmeans")
+    return books, sizes, dist, iters.value
+
+
+def anchor_evolve(wh: torch.Tensor, k0: torch.Tensor, v: torch.Tensor, thr: float, unit_exp: int):
+    """kmean_anchors' evolution on the device: (k float64 [na, 2], fitness float32 [gen + 1], accepted uint8 [gen])."""
+    require_cuda(wh, "anchor_evolve")
+    dev = wh.device
+    k0 = k0.to(dev, torch.float64).contiguous()
+    v = v.to(dev, torch.float64).contiguous()
+    gen = int(v.shape[0])
+    k = torch.empty_like(k0)
+    fit = torch.empty(gen + 1, dtype=torch.float32, device=dev)
+    acc = torch.empty(max(gen, 1), dtype=torch.uint8, device=dev)
+    ws = torch.empty(gen + 1, dtype=torch.int64, device=dev)
+    with device_guard(dev):
+        check(lib().yb_anchor_evolve(wh.data_ptr(), wh.shape[0], k0.shape[0], k0.data_ptr(), v.data_ptr(), gen,
+                                     float(thr), int(unit_exp), fit.data_ptr(), acc.data_ptr(), k.data_ptr(),
+                                     ws.data_ptr(), ws.numel() * 8, current_stream_ptr(dev)), "yb_anchor_evolve")
+    return k, fit, acc[:gen]

@@ -1467,6 +1467,11 @@ class Engine:
         self._low = None
         self._low8 = None
 
+    def drop_plans(self) -> None:
+        """Forget the plan instances (their fused head epilogues bake the post-processing constants) and keep the
+        lowered weights."""
+        self._plans.clear()
+
     def set_fp8(self, calib) -> None:
         """Run plans in FP8 with the scales of `calib` (None: in `dtype`).  FP8 plans are cached apart from the others,
         so switching back finds the `dtype` plans as they were."""

@@ -5,6 +5,7 @@ factories `yolov5_darknet_pan_{n,s,m,l,x}_r60` (`:468-619`).  `forward(samples[N
 batch to the plan's input layout with the letterbox kernel (identity geometry), runs the plan and the
 decode+NMS kernels; nothing is computed by PyTorch ops.
 """
+import math
 import os
 import warnings
 from typing import Any, Callable, Dict, List, Optional
@@ -167,6 +168,27 @@ class YOLO(nn.Module):
             self._fp8_stale = True
             raise RuntimeError("the FP8 calibration is stale: the weights changed after it was set; recalibrate with "
                                "quantization.calibrate_fp8 and call set_fp8 (or set_fp8(None) for fp16 / bf16)")
+
+    # -- anchors -------------------------------------------------------------------------------------
+    def set_anchor_grids(self, anchor_grids) -> None:
+        """Replace the anchors, per level [aw0, ah0, aw1, ah1, ...] in pixels (float32 values, as upstream's Detect holds
+        them in stride units: anchors_px() gives the bits it decodes with).  Every copy follows: the anchor generator,
+        the post-process's (or LogitsDecoder's) anchors_px, the criterion's anchor_grids; plan instances, whose fused
+        head epilogues bake the anchors, are dropped; the lowered weights are kept."""
+        ag = self.anchor_generator
+        grids = [[float(v) for v in a] for a in anchor_grids]
+        if len(grids) != ag.num_layers or any(len(a) != 2 * ag.num_anchors for a in grids):
+            raise ValueError(f"anchor_grids must hold {ag.num_layers} levels of {ag.num_anchors} (w, h) pairs")
+        if not all(math.isfinite(v) and v > 0 for a in grids for v in a):
+            raise ValueError("anchor sizes must be positive and finite")
+        ag.anchor_grids = grids
+        px = ag.anchors_px()
+        if getattr(self.post_process, "anchors_px", None) is not None:
+            self.post_process.anchors_px = px
+        if getattr(self.compute_loss, "anchor_grids", None) is not None:
+            self.compute_loss.anchor_grids = px
+        if self._engine is not None:
+            self._engine.drop_plans()
 
     # -- stages --------------------------------------------------------------------------------------
     def post_config(self) -> dict:

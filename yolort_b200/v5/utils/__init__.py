@@ -1,1 +1,1 @@
-"""yolort/v5/utils on the GPU: augmentations and the mosaic training loader (datasets)."""
+"""yolort/v5/utils on the GPU: augmentations, the mosaic training loader (datasets) and AutoAnchor (autoanchor)."""
