@@ -250,6 +250,9 @@ typedef struct {
                                     bit for bit) */
 #define YB_CONV_NO_TAIL_SPLIT 64 /* 1x1 / im2col kernel: run the last round's tiles whole instead of splitting them over
                                     the idle CTAs (tests compare the two launches bit for bit, A/B timing) */
+#define YB_CONV_PAIR_N64 128     /* halo-patch kernel: keep streamed-weight pair tasks at 64 columns on two consumer
+                                    warpgroups instead of 128 columns on four (tests compare the two launches bit for
+                                    bit, A/B timing) */
 /* ... and of an e4m3 YB_OP_CONV (see above), which takes these two only: */
 #define YB_CONV_E4M3_F16_OUT 16  /* fp16 output */
 #define YB_CONV_E4M3_BF16_OUT 32 /* bf16 output */
@@ -276,7 +279,8 @@ typedef struct {
   int32_t ring;              /* k-iterations per stage (halo patch: weight-ring slabs, 0 with resident weights) */
   int32_t store_cols;        /* store-box columns */
   int32_t store_bufs;        /* staging buffers per epilogue group */
-  int32_t groups;            /* consumer warpgroups per CTA: 2, or 1 (1x1 / im2col kernel, 64-row tiles) */
+  int32_t groups;            /* consumer warpgroups per CTA: 2, 1 (1x1 / im2col kernel, 64-row tiles) or 4 (halo patch:
+                                128-column pair tasks) */
   int32_t resident_ctas;     /* CTAs resident per SM: 1 or 2 */
   int32_t chained;           /* a chained tail is fused */
   int32_t smem_bytes;        /* dynamic shared memory per CTA */
@@ -301,7 +305,10 @@ typedef struct {
  * r tiles of a partial last round in two when 2 r <= grid (64-row halves with two consumer warpgroups, 64-column halves
  * with one), which the otherwise idle CTAs run (tail_tiles = r, tail_split = 2); a one-CTA plan whose 256-column N
  * tile streams its weights over 2-4 rounds takes 128-column N tiles when that split then applies.  Reserved bit
- * YB_CONV_NO_TAIL_SPLIT keeps the tiles whole (and 256 columns).  Pure host logic. */
+ * YB_CONV_NO_TAIL_SPLIT keeps the tiles whole (and 256 columns).  A halo-patch convolution with streamed weights (pair
+ * tasks) whose Cout is a multiple of 128 runs its pairs with 128-column N tiles on one CTA of four consumer warpgroups
+ * (groups = 4) when the grid is a multiple of the N tiles and its T tasks satisfy T >= SMs and T mod SMs = 0 or
+ * > SMs / 2; reserved bit YB_CONV_PAIR_N64 keeps the 64-column pairs.  Pure host logic. */
 int yb_conv_config(const yb_op_desc* op, yb_conv_info* info);
 
 typedef struct yb_plan yb_plan;

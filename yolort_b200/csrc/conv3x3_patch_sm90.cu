@@ -20,7 +20,8 @@
 //
 // Roles (one persistent CTA per SM, two for the narrow shallow levels, see patch_conv_configure; 384 threads): warp 0 = patch (A) producer, warp 2 = weight (B) producer (unless
 // the weights are resident in shared memory), warpgroups 1-2 = consumers: each multiplies 64 of the tile's 128
-// accumulator rows with wgmma (fp32 accumulators in registers) and runs the epilogue on its fragment.
+// accumulator rows with wgmma (fp32 accumulators in registers) and runs the epilogue on its fragment.  Pair tasks with
+// 128-column N tiles run on a lean instance of four consumer warpgroups (conv3x3_patch_quad_kernel, 640 threads).
 #include <cstdlib>
 
 #include "common.cuh"
@@ -497,6 +498,209 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
   if (issuer) tma_store_wait_all<0>();
 }
 
+// ===================== four consumer warpgroups: 128-column pair tasks =====================
+// The stride-1 layers whose weights are streamed (pair tasks) with a Cout that splits into 128-column N tiles.  A task
+// is a pair of M tiles times one 128-column N tile; consumer warpgroup w multiplies rows 64 (w mod 2) .. +63 of tile
+// w / 2 with m64n128k16 (64 accumulators per thread, as many as a 64-column pair), and all four read the same weight
+// slab per tap.  Per FLOP the weight and patch streams are those of the 64-column pairs, the MMAs are twice as wide
+// (an m64n128k16 reads 96 B of shared memory per clock against the 64-column MMA's 128 B), and the main loop keeps one
+// commit group in flight across channel chunks: a patch slot is released once the group of the chunk's last tap has
+// completed, not after a drain.  Every output element gets the k16 steps of the 64-column pair launch in the same
+// order (chunk, tap, k), so the outputs are the same bits.  Warpgroups 2w and 2w + 1 form team w: they own tile w's
+// epilogue, staging buffers and named barrier.  Only what this path needs is compiled: no chained tail, banded stem,
+// stride 2, resident weights or per-task bias reload (every CTA keeps one N tile, see patch_conv_plan).
+constexpr int kQuadConsumers = 4;
+constexpr int kQuadThreads = 128 * (1 + kQuadConsumers);   // 640
+constexpr uint32_t kQuadAllBar = 3;                          // the 512 consumer threads; teams use barriers 1 and 2
+// 227 KB per CTA (the H100's opt-in maximum) less this kernel's static shared memory (barriers + bias, ptxas -v)
+constexpr size_t kQuadStaticSmem = (2 * kMaxA + 2 * kMaxB) * 8 + kMaxBlockN * 4;
+constexpr size_t kQuadSmemBudget = 227 * 1024 - kQuadStaticSmem;
+
+template <bool kBf16>
+__global__ void __launch_bounds__(kQuadThreads, 1)
+conv3x3_patch_quad_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                          const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap,
+                          const __grid_constant__ CUtensorMap, const __grid_constant__ CUtensorMap, const PatchParams p) {
+  constexpr int kN = 128;
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t a_full[kMaxA], a_empty[kMaxA];
+  __shared__ __align__(8) uint64_t b_full[kMaxB], b_empty[kMaxB];
+  __shared__ __align__(16) float s_bias[kN];
+
+  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  uint8_t* a_buf = base;                                                        // [a_slots][a_stride]
+  uint8_t* b_buf = a_buf + static_cast<size_t>(p.a_slots) * p.a_stride;          // ring [b_stages][b_sub_bytes]
+  uint8_t* staging = b_buf + static_cast<size_t>(p.b_stages) * p.b_sub_bytes;   // [2 teams][store_bufs][stage_buf_bytes]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int taps_total = 9 * p.chunks;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    tma_prefetch_desc(&tmap_out);
+    for (int s = 0; s < p.a_slots; ++s) {
+      mbar_init(&a_full[s], 1);
+      mbar_init(&a_empty[s], 2);                // the two warpgroups of the team whose tile the patch is
+    }
+    for (int s = 0; s < kMaxB; ++s) {
+      mbar_init(&b_full[s], 1);
+      mbar_init(&b_empty[s], kQuadConsumers);   // every consumer warpgroup reads every slab
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+  // programmatic dependent launch as in conv3x3_patch_kernel: the weight producer does not wait for the previous grid
+  if (warp != 2) asm volatile("griddepcontrol.wait;" ::: "memory");
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  // 640 threads start with 96 registers each; 128 x 24 + 512 x 112 = 60 416 <= 640 x 96.  The producers lower their
+  // budget and return before the consumers raise theirs.
+  if (warp < 4) asm volatile("setmaxnreg.dec.sync.aligned.u32 24;\n" ::: "memory");
+
+  if (warp == 0) {
+    // ===================== patch (A) producer: the two tiles of a pair per channel chunk =====================
+    int ka = 0;
+    for (int task = blockIdx.x; task < p.num_tasks; task += gridDim.x) {
+      const int m_first = (task / p.n_tiles) * 2;
+      const int cnt = min(2, p.m_tiles - m_first);
+      for (int c = 0; c < p.chunks; ++c) {
+        for (int j = 0; j < cnt; ++j, ++ka) {
+          int n_img, y0, x0;
+          tile_coords(p, m_first + j, n_img, y0, x0);
+          const int s = ka % p.a_slots;
+          mbar_wait(&a_empty[s], ((ka / p.a_slots) & 1) ^ 1);
+          if (YB_ELECT()) {
+            mbar_expect_tx(&a_full[s], p.a_bytes);
+            tma_load_tiled_4d(&tmap_a, &a_full[s], a_buf + static_cast<size_t>(s) * p.a_stride, c * p.block_k, x0 - 1,
+                              y0 - 1, n_img);
+          }
+        }
+      }
+    }
+    return;
+  }
+  if (warp == 2) {
+    // ===================== weight (B) producer: one 128-column slab per (chunk, tap) =====================
+    const uint32_t b_bytes = p.block_n * p.block_k * 2;
+    int kb = 0;
+    for (int task = blockIdx.x; task < p.num_tasks; task += gridDim.x) {
+      const int n0 = (task % p.n_tiles) * p.block_n;
+      for (int i = 0; i < taps_total; ++i, ++kb) {
+        const int s = kb % p.b_stages;
+        mbar_wait(&b_empty[s], ((kb / p.b_stages) & 1) ^ 1);
+        if (YB_ELECT()) {
+          mbar_expect_tx(&b_full[s], b_bytes);
+          tma_load_2d(&tmap_b, &b_full[s], b_buf + static_cast<size_t>(s) * p.b_sub_bytes,
+                      ((i % 9) * p.chunks + i / 9) * p.block_k, n0);
+        }
+      }
+    }
+    return;
+  }
+  if (warp < 4) return;
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 112;\n" ::: "memory");
+
+  // ===================== consumers =====================
+  const int cw = (warp >> 2) - 1;   // consumer warpgroup 0..3
+  const int team = cw >> 1, half = cw & 1;
+  const int wq = warp & 3;
+  const int ctid = threadIdx.x - 128;
+  const bool issuer = (ctid & 255) == 0;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  FragRows fr;
+  fr.loc[0] = half * 64 + wq * 16 + (lane >> 2);
+  fr.loc[1] = fr.loc[0] + 8;
+  float acc[kN / 2];
+
+  // grid % n_tiles == 0 (host): task % n_tiles, the N tile, is the same for every task of this CTA
+  const int n0 = (blockIdx.x % p.n_tiles) * p.block_n;
+  for (int i = ctid; i < kN; i += 128 * kQuadConsumers) s_bias[i] = (n0 + i < p.bias_len) ? __ldg(p.bias + n0 + i) : 0.f;
+  named_bar_sync(kQuadAllBar, 128 * kQuadConsumers);
+
+  int ka = 0, kb = 0, store_idx = 0;
+  for (int task = blockIdx.x; task < p.num_tasks; task += gridDim.x) {
+    const int m_first = (task / p.n_tiles) * 2;
+    const int cnt = min(2, p.m_tiles - m_first);
+    // Team 1 has no tile in the odd last pair.  It still issues its MMAs, on whatever its next patch slot holds, without
+    // waiting for or releasing that slot, and discards the result: a branch around the MMAs would make ptxas serialise
+    // every wgmma of the kernel (C7520).  It reads and releases every weight slab like the other warpgroups.
+    const bool active = team < cnt;
+    int prev_sb = -1, prev_sa = -1;   // slab / patch slot read by the commit group still in flight
+    // descriptor constants, derived per task rather than held through the epilogue (registers are short)
+    const uint32_t row_bytes = p.block_k * 2;
+    const uint32_t sbo = p.tg.sbo_rows * row_bytes;
+    const uint32_t a_wg16 = (8 * sbo * half) >> 4;   // this warpgroup's 64 rows: 8 groups of 8 further into every view
+    const uint32_t row16 = row_bytes >> 4;
+    const uint32_t a_hi = desc_hi(row_bytes, sbo);
+    const uint32_t b_hi = desc_hi(row_bytes, 8 * row_bytes);
+    const uint32_t b_lo0 = smem_lo16(b_buf);
+    const uint32_t b_step16 = p.b_sub_bytes >> 4;
+    for (int c = 0; c < p.chunks; ++c) {
+      const int sa = (ka + team) % p.a_slots;
+      if (active) mbar_wait(&a_full[sa], ((ka + team) / p.a_slots) & 1);
+      const uint32_t a_lo = smem_lo16(a_buf + static_cast<size_t>(sa) * p.a_stride) + a_wg16;
+      const int kc = c == p.chunks - 1 ? p.kk_last : (p.block_k >> 4);
+      wgmma_fence();
+      for (int tap = 0; tap < 9; ++tap, ++kb) {
+        const int sb = kb % p.b_stages;
+        mbar_wait(&b_full[sb], (kb / p.b_stages) & 1);
+        const int dy = tap / 3, dx = tap - dy * 3;
+        const uint32_t a_tap = a_lo + static_cast<uint32_t>(dy * p.tg.pitch + dx) * row16;
+        const uint32_t b_lo = b_lo0 + static_cast<uint32_t>(sb) * b_step16;
+        for (int k = 0; k < kc; ++k)
+          wgmma_mma<kBf16, kN>(acc, desc_lohi(a_tap + 2 * k, a_hi), desc_lohi(b_lo + 2 * k, b_hi),
+                               !(c == 0 && tap == 0 && k == 0));
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous group (previous tap, possibly of the previous chunk) has completed
+        if (wg_leader) {
+          if (prev_sb >= 0) mbar_arrive(&b_empty[prev_sb]);
+          if (prev_sa >= 0) mbar_arrive(&a_empty[prev_sa]);
+        }
+        prev_sb = sb;
+        prev_sa = -1;
+      }
+      prev_sa = active ? sa : -1;   // released once the group of this chunk's last tap has completed
+      ka += cnt;
+    }
+    wgmma_wait<0>();
+    if (wg_leader) {
+      mbar_arrive(&b_empty[prev_sb]);
+      if (prev_sa >= 0) mbar_arrive(&a_empty[prev_sa]);
+    }
+    fence_acc<kN / 2>(acc);
+
+    // an inactive team runs the epilogue too (a branch around it would put the next task's MMAs on a divergent path,
+    // C7520), with no rows in range and no store
+    int n_img, y0, x0;
+    tile_coords(p, m_first + team, n_img, y0, x0);
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {   // the row's place in the tile, recomputed here: registers are short
+      const int grp = fr.loc[rr] >> 3;
+      const int yy = grp / p.tg.gpr, xx = (grp - yy * p.tg.gpr) * 8 + (fr.loc[rr] & 7);
+      const int y = y0 + yy, x = x0 + xx;
+      fr.ok[rr] = active && yy < p.tg.tile_h && y < p.H && x < p.W;
+      fr.row[rr] = (static_cast<long long>(n_img) * p.H + y) * p.W + x;
+    }
+    uint8_t* team_staging = staging + static_cast<size_t>(team) * p.store_bufs * p.stage_buf_bytes;
+    // the team's tile in two boxes of 64 columns through its two staging buffers (as store_tile: before the barrier
+    // the issuer waits until the previous store has read its buffer, which the next box overwrites).  Unrolled, so
+    // that the first box's 32 accumulators are dead while the second box is written.
+#pragma unroll
+    for (int c0 = 0; c0 < kN; c0 += 64, ++store_idx) {
+      uint8_t* buf = team_staging + (store_idx & 1) * p.stage_buf_bytes;
+      epilogue_box<kBf16, kN>(p.ep, acc, c0, 64, s_bias, fr, n0, buf, lane);
+      fence_proxy_async_smem();
+      if (issuer) tma_store_wait_read<0>();
+      named_bar_sync(1 + team, 256);   // the team's barrier
+      if (issuer) {
+        if (active && n0 + c0 < p.ep.Cout) tma_store_4d(&tmap_out, buf, n0 + c0, x0, y0, n_img);
+        tma_store_commit();
+      }
+    }
+  }
+  if (issuer) tma_store_wait_all<0>();
+}
+
 }  // namespace
 
 using PatchKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
@@ -504,8 +708,12 @@ using PatchKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUten
 
 // One kernel per (dtype, N tile, chained tail N, CTAs per SM): the MMA width and the accumulator size are compile-time
 // constants of every instance.  patch_conv_configure admits exactly these shapes.
+// Pair tasks with a 128-column N tile run on four consumer warpgroups (the plan caps the two-group pairs at 64 columns).
+static bool quad_plan(const PatchParams& kp) { return kp.pair == 2 && !kp.s2 && kp.block_n == 128; }
+
 template <bool kBf16>
 PatchKernelFn select_patch_kernel_t(const PatchParams& kp) {
+  if (quad_plan(kp)) return conv3x3_patch_quad_kernel<kBf16>;
   if (kp.ctas == 2) {
     // two CTAs per SM: the instances whose consumers fit in 104 registers without spilling (N = 32 / 64, N = 32 with a
     // 64-column tail; DESIGN.md section 3)
@@ -673,7 +881,19 @@ static int patch_conv_plan(const yb_op_desc& d, int ctas, PatchParams& kp, dim3&
   // tasks hold the accumulators of two tiles in registers, so their N tile is at most 64 columns (stride-2 tasks with
   // streamed weights: 128).
   kp.pair = (!kp.b_resident && !kp.band && !kp.s2 && kp.m_tiles >= 2) ? 2 : 1;
-  const int n_cap = kp.pair == 2 ? 64 : 128;
+  // Pairs whose Cout splits into 128-column N tiles run on four consumer warpgroups instead (conv3x3_patch_quad_kernel)
+  // when the grid is a multiple of the N tiles (one N tile per CTA), the 128-column tasks fill the grid (T >= G) and
+  // cost no extra round of it: T tasks of 128 columns run ceil(T / G) rounds of twice the work of the 2T tasks of 64
+  // columns, which run ceil(2T / G) rounds, so 2 ceil(T / G) <= ceil(2T / G), i.e. T mod G = 0 or T mod G > G / 2.
+  // c2 on 132 SMs: the 40² layers (240 tasks) take it, the 20² ones (128 tasks) do not.  YB_CONV_PAIR_N64 keeps the
+  // 64-column pairs.
+  const int quad_tiles = d.Cout / 128;
+  const int quad_tasks = ((kp.m_tiles + 1) / 2) * quad_tiles;
+  const int grid_q = quad_tasks < sms ? quad_tasks : sms;
+  const bool quad = ctas == 1 && kp.pair == 2 && d.chain == nullptr && d.Cout % 128 == 0 &&
+                    !(d.reserved & YB_CONV_PAIR_N64) && grid_q % quad_tiles == 0 && quad_tasks >= sms &&
+                    2 * ((quad_tasks + sms - 1) / sms) <= (2 * quad_tasks + sms - 1) / sms;
+  const int n_cap = kp.pair == 2 && !quad ? 64 : 128;
   if ((kp.pair == 2 || (kp.s2 && !kp.b_resident)) && block_n > n_cap) {
     n_tiles = (d.Cout + n_cap - 1) / n_cap;
     block_n = mma_n((d.Cout + n_tiles - 1) / n_tiles);
@@ -720,6 +940,16 @@ static int patch_conv_plan(const yb_op_desc& d, int ctas, PatchParams& kp, dim3&
     int a_st = static_cast<int>((avail_ns - b_total) / kp.a_stride);
     kp.a_slots = a_st > kMaxA ? kMaxA : a_st;
     kp.b_stages = 1;
+  } else if (quad) {
+    // four patch slots (this chunk's two tiles and the next chunk's) and two 16 KB staging buffers per team; the weight
+    // ring gets the rest of the 227 KB: 231 680 - 1024 - 4 x 23 552 - 65 536 = 70 912 B with classic tiles, 66 816 B
+    // with wrap tiles (24 KB patches), i.e. four 16 KB slabs (a slab feeds 16 MMAs, about 0.55 us at the dense rate)
+    kp.a_slots = 4;
+    staging_ns = 2 * staging;
+    const size_t used = 1024 + static_cast<size_t>(kp.a_slots) * kp.a_stride + staging_ns;
+    const int b_st = used < kQuadSmemBudget ? static_cast<int>((kQuadSmemBudget - used) / kp.b_sub_bytes) : 0;
+    kp.b_stages = b_st > kMaxB ? kMaxB : b_st;
+    YB_REQUIRE(kp.b_stages >= 2, "patch conv: not enough shared memory for the weight ring of four consumer warpgroups");
   } else {
     // patch slots: a pair task holds two at a time, a third (fourth) lets the next chunk's patches stream in meanwhile;
     // the weight ring gets the rest (every slab is consumed within ~0.1-0.3 us, the ring covers the L2 latency)
@@ -747,7 +977,8 @@ static int patch_conv_plan(const yb_op_desc& d, int ctas, PatchParams& kp, dim3&
   YB_REQUIRE(!(kp.b_resident && n_tiles > 1) || grid.x % n_tiles == 0, "patch conv: N-split grid %u not a multiple of %d", grid.x, n_tiles);
   const size_t b_region = kp.b_resident ? kp.b_res_bytes : static_cast<size_t>(kp.b_stages) * kp.b_sub_bytes;
   const size_t smem = static_cast<size_t>(kp.a_slots) * kp.a_stride + b_region + staging_ns + chain_bytes + 1024;
-  YB_REQUIRE(smem <= budget, "patch conv: %zu bytes of shared memory needed, %zu available", smem, budget);
+  YB_REQUIRE(smem <= (quad ? kQuadSmemBudget : budget), "patch conv: %zu bytes of shared memory needed, %zu available",
+             smem, quad ? kQuadSmemBudget : budget);
   smem_bytes = smem;
   return YB_OK;
 }
@@ -768,7 +999,7 @@ int patch_conv_config(const yb_op_desc& d, yb_conv_info* info) {
     info->ring = kp.b_resident ? 0 : kp.b_stages;
     info->store_cols = kp.store_cols;
     info->store_bufs = kp.store_bufs;
-    info->groups = kConsumers;
+    info->groups = quad_plan(kp) ? kQuadConsumers : kConsumers;
     info->resident_ctas = kp.ctas;
     info->chained = kp.ch.on;
     info->smem_bytes = static_cast<int>(smem);
@@ -788,8 +1019,8 @@ struct PatchConvOp final : ConvOp {
   dim3 grid;
   size_t smem_bytes;
   int launch(cudaStream_t stream) const override {
-    YB_CHECK_CUDA(launch_pdl(fn, grid, dim3(kThreads), smem_bytes, stream, tmap_a, tmap_b, tmap_out, tmap_w2, tmap_x,
-                             tmap_out2, kp));
+    YB_CHECK_CUDA(launch_pdl(fn, grid, dim3(quad_plan(kp) ? kQuadThreads : kThreads), smem_bytes, stream, tmap_a, tmap_b,
+                             tmap_out, tmap_w2, tmap_x, tmap_out2, kp));
     return YB_OK;
   }
 };
@@ -848,8 +1079,21 @@ int patch_conv_create(const yb_op_desc& d, ConvOp** out) {
   }
   if (rc == YB_OK) {
     op->fn = select_patch_kernel(kp);
-    rc = set_smem_attributes(reinterpret_cast<const void*>(op->fn), kSmemBudget, kp.ctas, op->smem_bytes, kThreads,
-                             "patch conv");
+    const bool quad = quad_plan(kp);
+    rc = set_smem_attributes(reinterpret_cast<const void*>(op->fn), quad ? kQuadSmemBudget : kSmemBudget, kp.ctas,
+                             op->smem_bytes, quad ? kQuadThreads : kThreads, "patch conv");
+    if (rc == YB_OK && quad) {   // the 640-thread CTA with up to 227 KB of shared memory must fit on an SM
+      int per_sm = 0;
+      const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, op->fn, kQuadThreads, op->smem_bytes);
+      if (e != cudaSuccess) {
+        set_error("patch conv: cudaOccupancyMaxActiveBlocksPerMultiprocessor failed: %s", cudaGetErrorString(e));
+        rc = YB_ERR_CUDA;
+      } else if (per_sm < 1) {
+        set_error("patch conv: the four-warpgroup CTA (%d threads, %zu bytes of shared memory) does not fit on an SM",
+                  kQuadThreads, op->smem_bytes);
+        rc = YB_ERR_INVALID;
+      }
+    }
   }
   if (rc != YB_OK) {
     delete op;
