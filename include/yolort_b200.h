@@ -251,8 +251,12 @@ typedef struct {
 #define YB_CONV_NO_TAIL_SPLIT 64 /* 1x1 / im2col kernel: run the last round's tiles whole instead of splitting them over
                                     the idle CTAs (tests compare the two launches bit for bit, A/B timing) */
 #define YB_CONV_PAIR_N64 128     /* halo-patch kernel: keep streamed-weight pair tasks at 64 columns on two consumer
-                                    warpgroups instead of 128 columns on four (tests compare the two launches bit for
+                                    warpgroups instead of 128 columns on four, and two-team launches on two consumer
+                                    warpgroups: every launch on four runs on two (tests compare the two launches bit for
                                     bit, A/B timing) */
+#define YB_CONV_NO_TEAMS 256     /* halo-patch kernel: keep chained and banded-stem launches on two consumer warpgroups
+                                    instead of two teams of two (tests compare the two launches bit for bit, A/B
+                                    timing) */
 /* ... and of an e4m3 YB_OP_CONV (see above), which takes these two only: */
 #define YB_CONV_E4M3_F16_OUT 16  /* fp16 output */
 #define YB_CONV_E4M3_BF16_OUT 32 /* bf16 output */
@@ -280,7 +284,7 @@ typedef struct {
   int32_t store_cols;        /* store-box columns */
   int32_t store_bufs;        /* staging buffers per epilogue group */
   int32_t groups;            /* consumer warpgroups per CTA: 2, 1 (1x1 / im2col kernel, 64-row tiles) or 4 (halo patch:
-                                128-column pair tasks) */
+                                128-column pair tasks, or two teams of single-tile tasks) */
   int32_t resident_ctas;     /* CTAs resident per SM: 1 or 2 */
   int32_t chained;           /* a chained tail is fused */
   int32_t smem_bytes;        /* dynamic shared memory per CTA */
@@ -308,7 +312,11 @@ typedef struct {
  * YB_CONV_NO_TAIL_SPLIT keeps the tiles whole (and 256 columns).  A halo-patch convolution with streamed weights (pair
  * tasks) whose Cout is a multiple of 128 runs its pairs with 128-column N tiles on one CTA of four consumer warpgroups
  * (groups = 4) when the grid is a multiple of the N tiles and its T tasks satisfy T >= SMs and T mod SMs = 0 or
- * > SMs / 2; reserved bit YB_CONV_PAIR_N64 keeps the 64-column pairs.  Pure host logic. */
+ * > SMs / 2; reserved bit YB_CONV_PAIR_N64 keeps the 64-column pairs.  A halo-patch convolution with resident weights
+ * in one N tile, single-tile classic-tiled tasks and either a chained tail after a 64-column N tile or the banded stem
+ * runs on one CTA of two consumer teams of two warpgroups each (groups = 4, tiles_per_pass 1) when it has at least
+ * 8 x SMs tasks and the two teams' staging buffers fit in shared memory; reserved bit YB_CONV_NO_TEAMS keeps two
+ * consumer warpgroups, as does YB_CONV_PAIR_N64.  Pure host logic. */
 int yb_conv_config(const yb_op_desc* op, yb_conv_info* info);
 
 typedef struct yb_plan yb_plan;

@@ -25,6 +25,7 @@ YB_ACT_NONE, YB_ACT_SILU, YB_ACT_HARDSWISH, YB_ACT_LEAKY01, YB_ACT_RELU = 0, 1, 
 YB_CONV_FORCE_IM2COL, YB_CONV_BAND_STEM, YB_CONV_FORCE_PLANES, YB_CONV_NO_NSPLIT, YB_CONV_ONE_CTA = 1, 2, 4, 8, 16
 YB_CONV_NO_TAIL_SPLIT = 64
 YB_CONV_PAIR_N64 = 128
+YB_CONV_NO_TEAMS = 256
 YB_CONV_E4M3_F16_OUT, YB_CONV_E4M3_BF16_OUT = 16, 32
 YB_CONV_KERNEL_IM2COL, YB_CONV_KERNEL_PATCH, YB_CONV_KERNEL_E4M3 = 0, 1, 2
 PATCH_TILINGS = {1: "classic", 2: "wrap", 3: "stride2"}      # yb_conv_info.tiling of the halo-patch kernel
@@ -646,7 +647,8 @@ def conv_config(op: "OpDesc") -> dict:
     # CTAs per SM x consumer warpgroups: "1x2", "2x2" (the 104-register instances) or "2x1"; "ctas_per_sm" names the
     # 104-register layout only
     cfg["layout"] = f"{info.resident_ctas}x{info.groups}"
-    # consumer warpgroups per CTA: 2, 1 (the 2x1 layout) or 4 (halo patch: 128-column pair tasks)
+    # consumer warpgroups per CTA: 2, 1 (the 2x1 layout) or 4 (halo patch: 128-column pair tasks, or two consumer teams
+    # of single-tile tasks: tiles_per_pass 1)
     cfg["consumer_groups"] = int(info.groups)
     cfg["ctas_per_sm"] = 2 if cfg["layout"] == "2x2" else 1
     if patch:

@@ -21,7 +21,10 @@
 // Roles (one persistent CTA per SM, two for the narrow shallow levels, see patch_conv_configure; 384 threads): warp 0 = patch (A) producer, warp 2 = weight (B) producer (unless
 // the weights are resident in shared memory), warpgroups 1-2 = consumers: each multiplies 64 of the tile's 128
 // accumulator rows with wgmma (fp32 accumulators in registers) and runs the epilogue on its fragment.  Pair tasks with
-// 128-column N tiles run on a lean instance of four consumer warpgroups (conv3x3_patch_quad_kernel, 640 threads).
+// 128-column N tiles run on a lean instance of four consumer warpgroups (conv3x3_patch_quad_kernel, 640 threads).  The
+// banded stem and the chains after a 64-column N tile, whose resident weights leave room for one CTA per SM only, run
+// large launches on another 640-thread instance: two teams of two consumer warpgroups take the CTA's single-tile tasks
+// alternately, so one team's epilogue and chained tail overlap the other team's MMAs (conv3x3_patch_team_kernel).
 #include <cstdlib>
 
 #include "common.cuh"
@@ -68,6 +71,7 @@ struct PatchParams {
   int s2;                 // 1: stride-2 convolution over two column-parity planes (H, W are the OUTPUT extent)
   int band;               // 1: banded super-pixel weights (stem), see the band MMA loop
   int ctas;               // CTAs per SM the launch is planned for (1 or 2): selects the kernel instance
+  int teams;              // 1: two consumer teams of two warpgroups share the CTA (conv3x3_patch_team_kernel)
   int store_cols, store_bufs, bias_len;
   int stage_buf_bytes;    // bytes between the staging buffers (16 KB; 8 KB for the N-split variant)
   int kk_last;            // K=16 steps of the last channel chunk (TMA zero-fills past Cin, the MMA skips)
@@ -701,6 +705,290 @@ conv3x3_patch_quad_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gr
   if (issuer) tma_store_wait_all<0>();
 }
 
+// ===================== two consumer teams: single-tile tasks over one resident weight copy =====================
+// The one-CTA launches with resident weights that cannot take two CTAs per SM (two copies of the weights do not fit):
+// the banded stem (kN = 128, kN2 = 0) and the chained 3x3 launches after a 64-column N tile (kN = 64, tail of kN2
+// columns).  The quad instance's layout: one producer warpgroup and four consumer warpgroups; warpgroups 2t and 2t + 1
+// form team t, which owns a whole 128-row tile exactly as the two consumer warpgroups of conv3x3_patch_kernel do.
+// The teams walk the CTA's task list alternately (team t takes positions t, t + 2, ...), so one team's epilogue, tail
+// GEMM and store waits overlap the other team's MMAs.  Shared: the resident weights (3x3 or stem band), the tail
+// weights, the bias vectors and the patch producer; per team: a named barrier (1 + t), two 16 KB staging buffers, the
+// extra operand's mbarrier and a TMA-store issuer, whose bulk async-groups are its own.  The patch ring is shared and
+// filled in task order; a slot is released by the team that read it.  Its slot count is a multiple of 2 x chunks
+// (patch_conv_plan), so every slot is only ever filled for one team: a team's parity wait on a slot then follows the
+// fill it waited on last, whereas a slot whose previous fill was the other team's could still have that fill in
+// flight, and the parity of the fill before it would let the wait pass.  Every output element gets the MMA sequence
+// and epilogue of conv3x3_patch_kernel, so the outputs are the same bits.  Only what these launches need is compiled:
+// stride 1, classic tiles, one N tile with resident weights, single-tile tasks, the chained tail or the band loop.
+constexpr uint32_t kTeamAllBar = 3;   // the 512 consumer threads; the teams use barriers 1 and 2
+constexpr int kTeamMinTasksPerSm = 8;  // patch_conv_plan
+constexpr size_t kTeamStaticSmem = (2 * kMaxA + 4) * 8 + 2 * kMaxBlockN * 4;
+constexpr size_t kTeamSmemBudget = 227 * 1024 - kTeamStaticSmem;
+
+template <bool kBf16, int kN, int kN2>
+__global__ void __launch_bounds__(kQuadThreads, 1)
+conv3x3_patch_team_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                          const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_w2,
+                          const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_out2,
+                          const PatchParams p) {
+  constexpr bool kChain = kN2 != 0;
+  constexpr bool kBand = !kChain;   // the stem has no tail; every chained launch here has a 64-column N tile
+  // chains: the 64-column first output, plus (128-column tails) the extra operand block, as 64-channel K chunks
+  constexpr int kTailChunks = kN2 == 128 ? 2 : 1;
+  static_assert(kBand ? kN == 128 : kN == 64, "team instances: the stem (N = 128) or a chain after N = 64");
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t a_full[kMaxA], a_empty[kMaxA];
+  __shared__ __align__(8) uint64_t b_full, w2_full;
+  __shared__ __align__(8) uint64_t x_full[2];   // per team: the extra operand block has landed
+  __shared__ __align__(16) float s_bias[kN];
+  __shared__ __align__(16) float s_bias2[kChain ? kN2 : 4];
+
+  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  uint8_t* a_buf = base;                                              // [a_slots][a_stride]
+  uint8_t* b_buf = a_buf + static_cast<size_t>(p.a_slots) * p.a_stride;  // resident [9 * chunks] or the band's [6]
+  uint8_t* staging = b_buf + p.b_res_bytes;                           // [2 teams][2][kStageBufBytes]
+  uint8_t* w2_res = staging + 4 * kStageBufBytes;                     // chain: tail weights
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    tma_prefetch_desc(&tmap_out);
+    for (int s = 0; s < p.a_slots; ++s) {
+      mbar_init(&a_full[s], 1);
+      mbar_init(&a_empty[s], 2);   // the two warpgroups of the team whose tile the patch is
+    }
+    mbar_init(&b_full, 1);
+    mbar_init(&w2_full, 1);
+    mbar_init(&x_full[0], 1);
+    mbar_init(&x_full[1], 1);
+    mbar_fence_init();
+  }
+  __syncthreads();
+  // programmatic dependent launch as in conv3x3_patch_kernel: the weight producer does not wait for the previous grid
+  if (warp != 2) asm volatile("griddepcontrol.wait;" ::: "memory");
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  // the quad instance's split: 128 x 24 + 512 x 112 <= 640 x 96; the producers lower their budget and return before
+  // the consumers raise theirs
+  if (warp < 4) asm volatile("setmaxnreg.dec.sync.aligned.u32 24;\n" ::: "memory");
+
+  if (warp == 0) {
+    // ===================== patch (A) producer: the CTA's tasks in order, whichever team runs them =====================
+    int ka = 0;
+    for (int task = blockIdx.x; task < p.num_tasks; task += gridDim.x) {
+      int n_img, y0, x0;
+      tile_coords(p, task, n_img, y0, x0);
+      for (int c = 0; c < p.chunks; ++c, ++ka) {
+        const int s = ka % p.a_slots;
+        mbar_wait(&a_empty[s], ((ka / p.a_slots) & 1) ^ 1);
+        if (YB_ELECT()) {
+          mbar_expect_tx(&a_full[s], p.a_bytes);
+          tma_load_tiled_4d(&tmap_a, &a_full[s], a_buf + static_cast<size_t>(s) * p.a_stride, c * p.block_k, x0 - 1,
+                            y0 - 1, n_img);
+        }
+      }
+    }
+    return;
+  }
+  if (warp == 2) {
+    // ===================== weights, once: the 3x3 slabs or the stem band, and the tail's =====================
+    if (lane == 0) {
+      const uint32_t b_bytes = p.block_n * p.block_k * 2;
+      if constexpr (kChain) {
+        tma_prefetch_desc(&tmap_w2);
+        tma_prefetch_desc(&tmap_out2);
+        if (p.ch.extra_on) tma_prefetch_desc(&tmap_x);
+        mbar_expect_tx(&w2_full, p.ch.w2_chunks * p.ch.n2 * p.ch.w2_row_bytes);
+        for (int j = 0; j < p.ch.w2_chunks; ++j)
+          tma_load_2d(&tmap_w2, &w2_full, w2_res + j * p.ch.w2_sub_bytes, j * (p.ch.w2_row_bytes >> 1), 0);
+        const int taps_total = 9 * p.chunks;
+        mbar_expect_tx(&b_full, taps_total * b_bytes);
+        for (int i = 0; i < taps_total; ++i)   // i = chunk*9 + tap ; weight column block = tap*chunks + chunk
+          tma_load_2d(&tmap_b, &b_full, b_buf + static_cast<size_t>(i) * p.b_sub_bytes,
+                      ((i % 9) * p.chunks + i / 9) * p.block_k, 0);
+      } else {   // banded stem weights: 3 filter rows x 2 blocks of 64 K-columns
+        mbar_expect_tx(&b_full, 6 * b_bytes);
+        for (int i = 0; i < 6; ++i)
+          tma_load_2d(&tmap_b, &b_full, b_buf + static_cast<size_t>(i) * p.b_sub_bytes, i * p.block_k, 0);
+      }
+    }
+    return;
+  }
+  if (warp < 4) return;
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 112;\n" ::: "memory");
+
+  // ===================== consumers: team t, warpgroup `half` of it multiplies rows 64 half .. +63 =====================
+  const int cw = (warp >> 2) - 1;
+  const int team = cw >> 1, half = cw & 1;
+  const int wq = warp & 3;
+  const int ctid = threadIdx.x - 128;
+  const bool issuer = (ctid & 255) == 0;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  const uint32_t team_bar = 1 + team;
+  FragRows fr;
+  fr.loc[0] = half * 64 + wq * 16 + (lane >> 2);
+  fr.loc[1] = fr.loc[0] + 8;
+  uint8_t* team_staging = staging + static_cast<size_t>(team) * 2 * kStageBufBytes;
+  float acc[kN / 2];
+
+  for (int i = ctid; i < kN; i += 128 * kQuadConsumers) s_bias[i] = (i < p.bias_len) ? __ldg(p.bias + i) : 0.f;
+  if constexpr (kChain) {
+    for (int i = ctid; i < kN2; i += 128 * kQuadConsumers) s_bias2[i] = (i < p.ch.bias2_len) ? __ldg(p.ch.bias2 + i) : 0.f;
+  }
+  named_bar_sync(kTeamAllBar, 128 * kQuadConsumers);
+  mbar_wait(&b_full, 0);
+  if constexpr (kChain) mbar_wait(&w2_full, 0);
+
+  uint32_t xph = 0;
+  // this team's tasks: positions team, team + 2, ... of the CTA's list; ka = the position's first patch
+  for (int task = blockIdx.x + team * gridDim.x, ka = team * p.chunks; task < p.num_tasks;
+       task += 2 * gridDim.x, ka += 2 * p.chunks) {
+    {
+      // descriptor constants, derived per task rather than held through the epilogue (registers are short)
+      const uint32_t row_bytes = p.block_k * 2;
+      const uint32_t sbo = p.tg.sbo_rows * row_bytes;
+      const uint32_t a_wg16 = (8 * sbo * half) >> 4;   // this warpgroup's 64 rows: 8 groups of 8 further into every view
+      const uint32_t row16 = row_bytes >> 4;
+      const uint32_t a_hi = desc_hi(row_bytes, sbo);
+      const uint32_t b_hi = desc_hi(row_bytes, 8 * row_bytes);
+      const uint32_t b_lo0 = smem_lo16(b_buf);
+      const uint32_t b_step16 = p.b_sub_bytes >> 4;
+      // The first MMA overwrites the accumulators; zeroing them first tells ptxas that the previous task's values are
+      // dead, which it cannot see through the run-time accumulate flag (otherwise they stay live across the tail GEMM
+      // and spill).  The band loop's flag is a compile-time constant.
+      if constexpr (kChain) {
+#pragma unroll
+        for (int i = 0; i < kN / 2; ++i) acc[i] = 0.f;
+      }
+      for (int c = 0; c < p.chunks; ++c) {
+        const int kq = ka + c;
+        const int sa = kq % p.a_slots;
+        mbar_wait(&a_full[sa], (kq / p.a_slots) & 1);
+        const uint32_t a_lo = smem_lo16(a_buf + static_cast<size_t>(sa) * p.a_stride) + a_wg16;
+        wgmma_fence();
+        if constexpr (kBand) {
+          // the band MMA loop of conv3x3_patch_kernel: per filter row six K=16 steps over 192 contiguous patch bytes
+          const uint32_t prow16 = static_cast<uint32_t>(p.tg.pitch) * row16;
+          for (int ky = 0; ky < 3; ++ky) {
+            for (int j = 0; j < 6; ++j) {
+              const uint32_t al = a_lo + ky * prow16 + 6 + 2 * j;
+              const uint32_t b_lo = b_lo0 + static_cast<uint32_t>(ky * 2 + (j >> 2)) * b_step16 + 2 * (j & 3);
+              wgmma_mma<kBf16, kN>(acc, desc_lohi(al, a_hi), desc_lohi(b_lo, b_hi), ky != 0 || j != 0);
+            }
+          }
+        } else {
+          // whole 64-channel chunks (patch_conv_plan): four K steps per tap, a fixed count (C7520 as in the tail)
+          const uint32_t b_lo_chunk = b_lo0 + static_cast<uint32_t>(c * 9) * b_step16;
+          for (int tap = 0; tap < 9; ++tap) {
+            const int dy = tap / 3, dx = tap - dy * 3;
+            const uint32_t a_tap = a_lo + static_cast<uint32_t>(dy * p.tg.pitch + dx) * row16;
+            const uint32_t b_lo = b_lo_chunk + static_cast<uint32_t>(tap) * b_step16;
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+              wgmma_mma<kBf16, kN>(acc, desc_lohi(a_tap + 2 * k, a_hi), desc_lohi(b_lo + 2 * k, b_hi),
+                                   !(c == 0 && tap == 0 && k == 0));
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        if (wg_leader) mbar_arrive(&a_empty[sa]);
+      }
+    }
+    fence_acc<kN / 2>(acc);
+
+    int n_img, y0, x0;
+    tile_coords(p, task, n_img, y0, x0);
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {   // the row's place in the tile (classic tiles: one 8-pixel group per tile row)
+      const int y = y0 + (fr.loc[rr] >> 3), x = x0 + (fr.loc[rr] & 7);
+      fr.ok[rr] = y < p.H && x < p.W;
+      // the stem has no shortcut (patch_conv_plan), so its epilogue never reads the row address
+      fr.row[rr] = kBand ? 0 : (static_cast<long long>(n_img) * p.H + y) * p.W + x;
+    }
+    if constexpr (kBand) {
+      // two boxes of 64 columns through the team's two staging buffers, box b in buffer b (as store_tile, whose box
+      // count per task is even here: before the barrier the issuer waits until the previous store has read its buffer,
+      // which the next box overwrites)
+#pragma unroll
+      for (int c0 = 0; c0 < kN; c0 += 64) {
+        uint8_t* buf = team_staging + (c0 / 64) * kStageBufBytes;
+        epilogue_box<kBf16, kN>(p.ep, acc, c0, 64, s_bias, fr, 0, buf, lane);
+        fence_proxy_async_smem();
+        if (issuer) tma_store_wait_read<0>();
+        named_bar_sync(team_bar, 256);
+        if (issuer) {
+          if (c0 < p.ep.Cout) tma_store_4d(&tmap_out, buf, c0, x0, y0, n_img);
+          tma_store_commit();
+        }
+      }
+    } else {
+      // the first output in one box (staging buffer 0), the extra operand block in buffer 1; both stay put until the
+      // tail GEMM has read them, so the team's previous stores must have drained the buffers first
+      if (issuer) {
+        tma_store_wait_read<0>();
+        if (p.ch.extra_on) {   // the cv2 half of the concat for this tile's pixels: same box as the output tile
+          mbar_expect_tx(&x_full[team], p.ch.extra_bytes);
+          tma_load_tiled_4d(&tmap_x, &x_full[team], team_staging + p.ch.own_chunks * kStageBufBytes, 0, x0, y0, n_img);
+        }
+      }
+      named_bar_sync(team_bar, 256);
+      epilogue_box<kBf16, kN>(p.ep, acc, 0, p.store_cols, s_bias, fr, 0, team_staging, lane);
+      fence_proxy_async_smem();
+      named_bar_sync(team_bar, 256);
+      if (issuer) {
+        if (p.ch.store_first) tma_store_4d(&tmap_out, team_staging, 0, x0, y0, n_img);
+        tma_store_commit();
+      }
+      if (p.ch.extra_on) {
+        mbar_wait(&x_full[team], xph);
+        xph ^= 1u;
+      }
+      const uint32_t a2_hi = desc_hi(p.ch.own_row_bytes, 8 * p.ch.own_row_bytes);
+      const uint32_t x_hi = desc_hi(p.ch.extra_row_bytes, 8 * p.ch.extra_row_bytes);
+      const uint32_t w2_lo0 = smem_lo16(w2_res);
+      float acc2[kChain ? kN2 / 2 : 8];   // the tail's own accumulator: the tile's is dead by now
+      wgmma_fence();
+      // the chunk count and their 64 channels are fixed per instance (patch_conv_plan): with run-time loop bounds here
+      // ptxas serialises the wgmmas (C7520)
+#pragma unroll
+      for (int j = 0; j < kTailChunks; ++j) {
+        const bool own = j == 0;
+        const uint32_t rb = own ? p.ch.own_row_bytes : p.ch.extra_row_bytes;
+        const uint32_t a_lo = smem_lo16(team_staging + j * kStageBufBytes) + ((64 * half * rb) >> 4);
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_mma<kBf16, kChain ? kN2 : 16>(acc2, desc_lohi(a_lo + 2 * k, own ? a2_hi : x_hi),
+                                              desc_lohi(w2_lo0 + j * (p.ch.w2_sub_bytes >> 4) + 2 * k,
+                                                        desc_hi(p.ch.w2_row_bytes, 8 * p.ch.w2_row_bytes)),
+                                              (j | k) != 0);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_acc<kChain ? kN2 / 2 : 8>(acc2);
+      // the tail's boxes reuse the team's staging buffers: the operand blocks are dead (both warpgroups' tail GEMMs
+      // have completed), but the store of the first output may still be reading buffer 0
+      if (issuer) tma_store_wait_read<0>();
+      named_bar_sync(team_bar, 256);
+      EpilogueParams ep2 = p.ch.ep2;
+      ep2.residual = nullptr;   // never set for a tail (chain_setup); known here, the epilogue drops its row addresses
+#pragma unroll
+      for (int c0 = 0; c0 < (kChain ? kN2 : 16); c0 += 64) {
+        uint8_t* buf = team_staging + ((c0 / 64) & 1) * kStageBufBytes;
+        epilogue_box<kBf16, kChain ? kN2 : 16>(ep2, acc2, c0, 64, s_bias2, fr, 0, buf, lane);
+        fence_proxy_async_smem();
+        if (issuer) tma_store_wait_read<0>();   // box k + 1 overwrites the buffer of box k - 1
+        named_bar_sync(team_bar, 256);
+        if (issuer) {
+          if (c0 < p.ch.ep2.Cout) tma_store_4d(&tmap_out2, buf, c0, x0, y0, n_img);
+          tma_store_commit();
+        }
+      }
+    }
+  }
+  if (issuer) tma_store_wait_all<0>();
+}
+
 }  // namespace
 
 using PatchKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
@@ -711,9 +999,16 @@ using PatchKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUten
 // Pair tasks with a 128-column N tile run on four consumer warpgroups (the plan caps the two-group pairs at 64 columns).
 static bool quad_plan(const PatchParams& kp) { return kp.pair == 2 && !kp.s2 && kp.block_n == 128; }
 
+// Two consumer teams run the banded stem and the chains after a 64-column N tile (patch_conv_plan sets kp.teams).
+static bool four_groups(const PatchParams& kp) { return quad_plan(kp) || kp.teams; }
+
 template <bool kBf16>
 PatchKernelFn select_patch_kernel_t(const PatchParams& kp) {
   if (quad_plan(kp)) return conv3x3_patch_quad_kernel<kBf16>;
+  if (kp.teams) {
+    if (kp.band) return conv3x3_patch_team_kernel<kBf16, 128, 0>;
+    return kp.ch.n2 == 64 ? conv3x3_patch_team_kernel<kBf16, 64, 64> : conv3x3_patch_team_kernel<kBf16, 64, 128>;
+  }
   if (kp.ctas == 2) {
     // two CTAs per SM: the instances whose consumers fit in 104 registers without spilling (N = 32 / 64, N = 32 with a
     // 64-column tail; DESIGN.md section 3)
@@ -936,7 +1231,29 @@ static int patch_conv_plan(const yb_op_desc& d, int ctas, PatchParams& kp, dim3&
   if (ctas == 2 && !(kp.b_resident && n_tiles == 1 && kp.pair == 1 && !kp.band && kp.num_tasks >= 2 * sms &&
                      select_patch_kernel(kp) != nullptr))
     return YB_ERR_INVALID;
-  if (kp.b_resident) {
+  // Two consumer teams (conv3x3_patch_team_kernel) for the one-CTA launches with resident weights in one N tile and
+  // single-tile classic tasks that are the 128-column banded stem, or a chain after a 64-column N tile over whole
+  // 64-channel chunks whose tail reads one 64-channel chunk (64-column tails) or two (128-column tails: the first
+  // output and the extra operand) -- the shapes the team instances compile -- when each team's two staging buffers
+  // and one patch slot per channel chunk fit next to the weights in 227 KB and the launch has at least
+  // kTeamMinTasksPerSm tasks per SM.
+  // The threshold keeps the smaller launches (the fingerprint plans' stems and chains, about 800 tasks) on two
+  // warpgroups; DESIGN.md section 3 has the measured sweep.  YB_CONV_NO_TEAMS keeps two consumer warpgroups, and so
+  // does YB_CONV_PAIR_N64, which names the two-warpgroup launch of every four-warpgroup one.
+  const bool team_chain = kp.ch.on && block_n == 64 && kp.block_k == 64 && kp.kk_last == 4 && kp.ch.ksteps == 4 &&
+                          kp.ch.w2_chunks == (kp.ch.n2 == 128 ? 2 : 1);
+  const size_t team_fixed = b_total + 2 * staging + chain_bytes + 1024;
+  kp.teams = ctas == 1 && !(d.reserved & (YB_CONV_NO_TEAMS | YB_CONV_PAIR_N64)) && kp.b_resident && n_tiles == 1 &&
+             kp.pair == 1 && !kp.s2 && tg.x_step == 8 && ((kp.band && block_n == 128) || team_chain) &&
+             kp.num_tasks >= kTeamMinTasksPerSm * sms && 2 * kp.chunks <= kMaxA &&
+             team_fixed + 2 * static_cast<size_t>(kp.chunks) * kp.a_stride <= kTeamSmemBudget;
+  if (kp.teams) {
+    // a multiple of 2 x chunks patch slots: each slot then serves one team only (see conv3x3_patch_team_kernel)
+    const int a_st = static_cast<int>((kTeamSmemBudget - team_fixed) / kp.a_stride);
+    kp.a_slots = (a_st > kMaxA ? kMaxA : a_st) / (2 * kp.chunks) * (2 * kp.chunks);
+    kp.b_stages = 1;
+    staging_ns = 2 * staging;
+  } else if (kp.b_resident) {
     int a_st = static_cast<int>((avail_ns - b_total) / kp.a_stride);
     kp.a_slots = a_st > kMaxA ? kMaxA : a_st;
     kp.b_stages = 1;
@@ -967,6 +1284,8 @@ static int patch_conv_plan(const yb_op_desc& d, int ctas, PatchParams& kp, dim3&
     }
   }
   YB_REQUIRE(kp.a_slots >= 2, "patch conv: fewer than two patch slots fit in shared memory (block_n=%d)", block_n);
+  YB_REQUIRE(!kp.teams || kp.a_slots % (2 * kp.chunks) == 0, "patch conv: %d patch slots do not divide between two teams",
+             kp.a_slots);
   kp.ep.Cout = d.Cout;
   kp.ep.act = d.act;
   kp.ep.residual = d.residual;
@@ -977,8 +1296,8 @@ static int patch_conv_plan(const yb_op_desc& d, int ctas, PatchParams& kp, dim3&
   YB_REQUIRE(!(kp.b_resident && n_tiles > 1) || grid.x % n_tiles == 0, "patch conv: N-split grid %u not a multiple of %d", grid.x, n_tiles);
   const size_t b_region = kp.b_resident ? kp.b_res_bytes : static_cast<size_t>(kp.b_stages) * kp.b_sub_bytes;
   const size_t smem = static_cast<size_t>(kp.a_slots) * kp.a_stride + b_region + staging_ns + chain_bytes + 1024;
-  YB_REQUIRE(smem <= (quad ? kQuadSmemBudget : budget), "patch conv: %zu bytes of shared memory needed, %zu available",
-             smem, quad ? kQuadSmemBudget : budget);
+  const size_t cap = quad ? kQuadSmemBudget : (kp.teams ? kTeamSmemBudget : budget);
+  YB_REQUIRE(smem <= cap, "patch conv: %zu bytes of shared memory needed, %zu available", smem, cap);
   smem_bytes = smem;
   return YB_OK;
 }
@@ -999,7 +1318,7 @@ int patch_conv_config(const yb_op_desc& d, yb_conv_info* info) {
     info->ring = kp.b_resident ? 0 : kp.b_stages;
     info->store_cols = kp.store_cols;
     info->store_bufs = kp.store_bufs;
-    info->groups = quad_plan(kp) ? kQuadConsumers : kConsumers;
+    info->groups = four_groups(kp) ? kQuadConsumers : kConsumers;
     info->resident_ctas = kp.ctas;
     info->chained = kp.ch.on;
     info->smem_bytes = static_cast<int>(smem);
@@ -1019,7 +1338,7 @@ struct PatchConvOp final : ConvOp {
   dim3 grid;
   size_t smem_bytes;
   int launch(cudaStream_t stream) const override {
-    YB_CHECK_CUDA(launch_pdl(fn, grid, dim3(quad_plan(kp) ? kQuadThreads : kThreads), smem_bytes, stream, tmap_a, tmap_b,
+    YB_CHECK_CUDA(launch_pdl(fn, grid, dim3(four_groups(kp) ? kQuadThreads : kThreads), smem_bytes, stream, tmap_a, tmap_b,
                              tmap_out, tmap_w2, tmap_x, tmap_out2, kp));
     return YB_OK;
   }
@@ -1079,8 +1398,9 @@ int patch_conv_create(const yb_op_desc& d, ConvOp** out) {
   }
   if (rc == YB_OK) {
     op->fn = select_patch_kernel(kp);
-    const bool quad = quad_plan(kp);
-    rc = set_smem_attributes(reinterpret_cast<const void*>(op->fn), quad ? kQuadSmemBudget : kSmemBudget, kp.ctas,
+    const bool quad = four_groups(kp);
+    rc = set_smem_attributes(reinterpret_cast<const void*>(op->fn),
+                             quad_plan(kp) ? kQuadSmemBudget : (kp.teams ? kTeamSmemBudget : kSmemBudget), kp.ctas,
                              op->smem_bytes, quad ? kQuadThreads : kThreads, "patch conv");
     if (rc == YB_OK && quad) {   // the 640-thread CTA with up to 227 KB of shared memory must fit on an SM
       int per_sm = 0;

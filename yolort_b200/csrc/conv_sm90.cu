@@ -546,7 +546,8 @@ static int conv_plan(const yb_op_desc& d, int ctas, int groups, ConvKernelParams
 // Validation of an fp16 / bf16 convolution descriptor, shared with the halo-patch kernel (pure host logic).
 int conv_validate(const yb_op_desc& d) {
   YB_REQUIRE(d.dtype == YB_F16 || d.dtype == YB_BF16, "conv: dtype must be f16 or bf16");
-  YB_REQUIRE((d.reserved & ~(31 | YB_CONV_NO_TAIL_SPLIT | YB_CONV_PAIR_N64)) == 0, "conv: reserved bits 5 and 8 and up must be zero, got 0x%x",
+  YB_REQUIRE((d.reserved & ~(31 | YB_CONV_NO_TAIL_SPLIT | YB_CONV_PAIR_N64 | YB_CONV_NO_TEAMS)) == 0,
+             "conv: reserved bits 5 and 9 and up must be zero, got 0x%x",
              d.reserved);
   YB_REQUIRE(d.ksize >= 1 && d.ksize <= 7 && d.stride >= 1 && d.stride <= 2, "conv: ksize/stride");
   YB_REQUIRE(d.act >= YB_ACT_NONE && d.act <= YB_ACT_RELU, "conv: unknown activation %d", d.act);
