@@ -251,12 +251,12 @@ typedef struct {
 #define YB_CONV_NO_TAIL_SPLIT 64 /* 1x1 / im2col kernel: run the last round's tiles whole instead of splitting them over
                                     the idle CTAs (tests compare the two launches bit for bit, A/B timing) */
 #define YB_CONV_PAIR_N64 128     /* halo-patch kernel: keep streamed-weight pair tasks at 64 columns on two consumer
-                                    warpgroups instead of 128 columns on four, and two-team launches on two consumer
-                                    warpgroups: every launch on four runs on two (tests compare the two launches bit for
-                                    bit, A/B timing) */
-#define YB_CONV_NO_TEAMS 256     /* halo-patch kernel: keep chained and banded-stem launches on two consumer warpgroups
-                                    instead of two teams of two (tests compare the two launches bit for bit, A/B
-                                    timing) */
+                                    warpgroups instead of 128 columns on four; either kernel: keep two-team launches on
+                                    two consumer warpgroups: every launch on four runs on two (tests compare the two
+                                    launches bit for bit, A/B timing) */
+#define YB_CONV_NO_TEAMS 256     /* halo-patch and 1x1 / im2col kernels: keep chained and banded-stem launches on two
+                                    consumer warpgroups instead of two teams of two (tests compare the two launches bit
+                                    for bit, A/B timing) */
 /* ... and of an e4m3 YB_OP_CONV (see above), which takes these two only: */
 #define YB_CONV_E4M3_F16_OUT 16  /* fp16 output */
 #define YB_CONV_E4M3_BF16_OUT 32 /* bf16 output */
@@ -279,12 +279,12 @@ typedef struct {
   int32_t n_tiles;           /* N tiles */
   int32_t weights_resident;  /* the weights of the CTA's N tile stay in shared memory */
   int32_t tiles_per_pass;    /* M tiles per weight pass (halo patch: 2 when pairs of tiles share each weight slab) */
-  int32_t slots;             /* pipeline stages (halo patch: patch slots) */
+  int32_t slots;             /* pipeline stages (two teams of the 1x1 / im2col kernel: per team; halo patch: patch slots) */
   int32_t ring;              /* k-iterations per stage (halo patch: weight-ring slabs, 0 with resident weights) */
   int32_t store_cols;        /* store-box columns */
   int32_t store_bufs;        /* staging buffers per epilogue group */
   int32_t groups;            /* consumer warpgroups per CTA: 2, 1 (1x1 / im2col kernel, 64-row tiles) or 4 (halo patch:
-                                128-column pair tasks, or two teams of single-tile tasks) */
+                                128-column pair tasks; either kernel: two teams of single-tile tasks) */
   int32_t resident_ctas;     /* CTAs resident per SM: 1 or 2 */
   int32_t chained;           /* a chained tail is fused */
   int32_t smem_bytes;        /* dynamic shared memory per CTA */
@@ -316,7 +316,12 @@ typedef struct {
  * in one N tile, single-tile classic-tiled tasks and either a chained tail after a 64-column N tile or the banded stem
  * runs on one CTA of two consumer teams of two warpgroups each (groups = 4, tiles_per_pass 1) when it has at least
  * 8 x SMs tasks and the two teams' staging buffers fit in shared memory; reserved bit YB_CONV_NO_TEAMS keeps two
- * consumer warpgroups, as does YB_CONV_PAIR_N64.  Pure host logic. */
+ * consumer warpgroups, as does YB_CONV_PAIR_N64.  A 1x1 / s1 convolution of one CTA per SM with a 128-column N tile of
+ * resident weights over whole 64-channel K chunks, chained to a 64-column tail over one or two 64-channel boxes, runs
+ * on two consumer teams too (groups = 4, layout 1x4, one k-iteration per stage and `slots` stages per team) when it
+ * has at least 8 x SMs tiles and the weights, both teams' staging buffers and two stages per team fit in shared
+ * memory; reserved bits YB_CONV_NO_TEAMS, YB_CONV_PAIR_N64 and YB_CONV_ONE_CTA keep two consumer warpgroups.  Pure
+ * host logic. */
 int yb_conv_config(const yb_op_desc* op, yb_conv_info* info);
 
 typedef struct yb_plan yb_plan;

@@ -647,8 +647,8 @@ def conv_config(op: "OpDesc") -> dict:
     # CTAs per SM x consumer warpgroups: "1x2", "2x2" (the 104-register instances) or "2x1"; "ctas_per_sm" names the
     # 104-register layout only
     cfg["layout"] = f"{info.resident_ctas}x{info.groups}"
-    # consumer warpgroups per CTA: 2, 1 (the 2x1 layout) or 4 (halo patch: 128-column pair tasks, or two consumer teams
-    # of single-tile tasks: tiles_per_pass 1)
+    # consumer warpgroups per CTA: 2, 1 (the 2x1 layout) or 4 (halo patch: 128-column pair tasks; either kernel: two
+    # consumer teams of single-tile tasks, tiles_per_pass 1)
     cfg["consumer_groups"] = int(info.groups)
     cfg["ctas_per_sm"] = 2 if cfg["layout"] == "2x2" else 1
     if patch:

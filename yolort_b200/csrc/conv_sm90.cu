@@ -18,7 +18,10 @@
 //                window of a concat buffer is just a strided tensor map; ragged M is clipped by the TMA unit).
 // Instances with ONE consumer warpgroup (256 threads, 64-row tiles, two CTAs per SM at the consumers' 232 registers) run
 // the same protocol with half the participants: the two co-resident CTAs take the place of the two consumer warpgroups,
-// and one CTA's epilogue overlaps the other's MMAs.
+// and one CTA's epilogue overlaps the other's MMAs.  The large chained 1x1 launches at N = 128, whose resident weights
+// leave room for one CTA per SM only, run on a lean 640-thread instance: two teams of two consumer warpgroups take the
+// CTA's tiles alternately, so one team's epilogue and chained tail overlap the other team's MMAs
+// (conv_wgmma_team_kernel).
 // The kernel is a template over (dtype, activation family, fused decode, chained tail).  A chained tail
 // (conv_chain.cuh) is a second, pointwise GEMM over the tile the epilogue has just staged: the consumers multiply the
 // staged boxes with the resident tail weights and a second epilogue pass stores the result.
@@ -488,7 +491,233 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   if (issuer) tma_store_wait_all<0>();
 }
 
-using ConvKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
+// ===================== two consumer teams: chained 1x1 tiles over one resident weight copy =====================
+// The large one-CTA chained 1x1 launches (C3's cv1 || cv2 -> m.0.cv1 at N = 128 with a 64-column tail): their resident
+// weights leave room for one CTA per SM only, and on that CTA's two consumer warpgroups nothing issued MMAs while a tile
+// ran its epilogue boxes, its store waits, the tail GEMM and the tail epilogue.  This lean instance has one producer
+// warpgroup and four consumer warpgroups (640 threads); warpgroups 2t + 1 and 2t + 2 form team t, which owns a whole
+// 128-row tile and runs on it exactly the chain path of conv_wgmma_kernel.  Team t takes positions t, t + 2, ... of the
+// CTA's tile list, so one team's epilogue and tail overlap the other team's MMAs.  Shared: the resident weights, the
+// resident tail weights, both bias vectors and the producer warp; per team: a named barrier (2 + t; the 512 consumer
+// threads use kConsumerBar), two 16 KB staging boxes, a TMA-store issuer whose bulk async-groups are its own, and an
+// A ring of one-k-iteration stages.  The producer fills ring k & 1 with the CTA's k-th tile, so a team's parity wait
+// on a slot always follows the fill it waited on last.  Every output element gets the k16 MMA sequence and the
+// epilogue of conv_wgmma_kernel, so the outputs are the same bits.  Only what these launches need is compiled: mode 0
+// (2-D tiled A), whole 64-channel K chunks, one N tile of resident weights, a chained tail of kN2 columns over one or
+// two 64-channel staged boxes, no fused decode and no split tail.
+constexpr int kTeamThreads = 640;
+constexpr int kTeamMaxStages = 6;        // A stages per team
+constexpr int kTeamMinTilesPerSm = 8;    // conv_team_plan
+constexpr uint32_t kTeamBar0 = 2;        // team t syncs on named barrier 2 + t
+constexpr size_t kTeamStaticSmem = (4 * kTeamMaxStages + 2) * 8 + 2 * 128 * 4;   // barriers + bias vectors
+constexpr size_t kTeamSmemBudget = 227 * 1024 - kTeamStaticSmem;
+
+template <bool kBf16, int kN, int kN2>
+__global__ void __launch_bounds__(kTeamThreads, 1)
+conv_wgmma_team_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                       const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_w2,
+                       const __grid_constant__ CUtensorMap tmap_out2, const __grid_constant__ CUtensorMap tmap_a64,
+                       const __grid_constant__ CUtensorMap tmap_out64, const ConvKernelParams p) {
+  static_assert(kN == 128 && kN2 == 64, "team instances: N = 128 with a 64-column tail");
+  constexpr int kStageBufBytes = stage_buf_bytes(2);
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t full_bar[2][kTeamMaxStages];
+  __shared__ __align__(8) uint64_t empty_bar[2][kTeamMaxStages];
+  __shared__ __align__(8) uint64_t b_full;
+  __shared__ __align__(8) uint64_t w2_full;
+  __shared__ __align__(16) float s_bias[kN];
+  __shared__ __align__(16) float s_bias2[kN2];
+
+  uint8_t* tiles = reinterpret_cast<uint8_t*>(
+      (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  const uint32_t ring_bytes = static_cast<uint32_t>(p.stages) * p.a_stage_bytes;   // [2 teams][stages][A sub-tile]
+  uint8_t* b_res = tiles + 2 * ring_bytes;                  // resident weights
+  uint8_t* staging = b_res + p.b_res_bytes;                 // [2 teams][kStageBufs][kStageBufBytes]
+  uint8_t* w2_res = staging + 2 * kStageBufs * kStageBufBytes;   // resident tail weights
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    tma_prefetch_desc(&tmap_out);
+    for (int r = 0; r < 2; ++r) {
+      for (int s = 0; s < p.stages; ++s) {
+        mbar_init(&full_bar[r][s], 1);
+        mbar_init(&empty_bar[r][s], 2);   // the two warpgroups of the team
+      }
+    }
+    mbar_init(&b_full, 1);
+    mbar_init(&w2_full, 1);
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  // the weights do not depend on the previous kernel: loaded before the grid-dependency wait, as conv_wgmma_kernel
+  if (threadIdx.x == 0) {
+    const uint32_t b_bytes = p.block_n * p.block_k * 2;
+    mbar_expect_tx(&b_full, p.num_k_iters * b_bytes);
+    for (int it = 0; it < p.num_k_iters; ++it) tma_load_2d(&tmap_b, &b_full, b_res + it * p.b_stage_bytes, it * p.block_k, 0);
+    tma_prefetch_desc(&tmap_w2);
+    tma_prefetch_desc(&tmap_out2);
+    mbar_expect_tx(&w2_full, p.ch.w2_chunks * p.ch.n2 * p.ch.w2_row_bytes);
+    for (int j = 0; j < p.ch.w2_chunks; ++j)
+      tma_load_2d(&tmap_w2, &w2_full, w2_res + j * p.ch.w2_sub_bytes, j * (p.ch.w2_row_bytes >> 1), 0);
+  }
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  // 128 x 24 + 512 x 112 <= 640 x 96: the producers lower their budget and return before the consumers raise theirs
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 24;\n" ::: "memory");
+    if (warp != 0) return;
+    // ===================== A producer: the CTA's tiles in order, tile k into ring k & 1 =====================
+    const uint32_t a_bytes = p.a_stage_bytes;
+    int kit0 = 0, kit1 = 0;   // fills of each ring so far
+    for (int t = blockIdx.x, k = 0; t < p.num_tiles; t += gridDim.x, ++k) {
+      const int r = k & 1;
+      const int m0 = t * 128;
+      int kit = r ? kit1 : kit0;
+      for (int it = 0; it < p.num_k_iters; ++it, ++kit) {
+        const int s = kit % p.stages;
+        mbar_wait(&empty_bar[r][s], ((kit / p.stages) & 1) ^ 1);
+        if (YB_ELECT()) {
+          mbar_expect_tx(&full_bar[r][s], a_bytes);
+          tma_load_2d(&tmap_a, &full_bar[r][s], tiles + r * ring_bytes + s * a_bytes, it * p.block_k, m0);
+        }
+      }
+      (r ? kit1 : kit0) = kit;
+    }
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 112;\n" ::: "memory");
+
+  // ===================== consumers: team `team`, warpgroup `half` of it multiplies rows 64 half .. +63 =====================
+  const int cw = (warp >> 2) - 1;
+  const int team = cw >> 1, half = cw & 1;
+  const int wq = warp & 3;
+  const int ctid = threadIdx.x - 128;
+  const bool issuer = (ctid & 255) == 0;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  const uint32_t team_bar = kTeamBar0 + team;
+  FragRows fr;
+  fr.loc[0] = half * 64 + wq * 16 + (lane >> 2);
+  fr.loc[1] = fr.loc[0] + 8;
+  uint8_t* team_staging = staging + static_cast<size_t>(team) * kStageBufs * kStageBufBytes;
+  uint8_t* ring = tiles + team * ring_bytes;
+  float acc[kN / 2];
+
+  for (int i = ctid; i < kN; i += 512) s_bias[i] = (i < p.bias_len) ? __ldg(p.bias + i) : 0.f;
+  for (int i = ctid; i < kN2; i += 512) s_bias2[i] = (i < p.ch.bias2_len) ? __ldg(p.ch.bias2 + i) : 0.f;
+  named_bar_sync(kConsumerBar, 512);
+  mbar_wait(&b_full, 0);
+  mbar_wait(&w2_full, 0);
+
+  int kit = 0;
+  for (int t = blockIdx.x + team * gridDim.x; t < p.num_tiles; t += 2 * gridDim.x) {
+    const int m0 = t * 128;
+    {
+      // descriptor constants, derived per tile rather than held through the epilogue (registers are short)
+      const uint32_t ab_hi = desc_hi(128, 8 * 128);                  // 64-channel rows of 128 bytes
+      const uint32_t a_wg16 = (64 * 128 * half) >> 4;                // this warpgroup's 64 rows of an A sub-tile
+      const uint32_t b_lo0 = smem_lo16(b_res);
+      const uint32_t b_step16 = p.b_stage_bytes >> 4;
+      // The first MMA overwrites the accumulators; zeroing them first tells ptxas that the previous tile's values are
+      // dead, which it cannot see through the run-time accumulate flag (they would otherwise stay live across the tail
+      // GEMM and spill).
+#pragma unroll
+      for (int i = 0; i < kN / 2; ++i) acc[i] = 0.f;
+      // ---- main loop: stage s is released once the MMAs that read it have completed (one stage in flight) ----
+      int prev_s = -1;
+      for (int it = 0; it < p.num_k_iters; ++it, ++kit) {
+        const int s = kit % p.stages;
+        mbar_wait(&full_bar[team][s], (kit / p.stages) & 1);
+        const uint32_t a_lo = smem_lo16(ring + s * p.a_stage_bytes) + a_wg16;
+        const uint32_t b_lo = b_lo0 + it * b_step16;
+        wgmma_fence();
+        // whole 64-channel chunks (conv_team_plan): four K steps, a fixed count (ptxas serialises the wgmmas of a
+        // run-time count, C7520)
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_mma<kBf16, kN>(acc, desc_lohi(a_lo + 2 * k, ab_hi), desc_lohi(b_lo + 2 * k, ab_hi), it != 0 || k != 0);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev_s >= 0 && wg_leader) mbar_arrive(&empty_bar[team][prev_s]);
+        prev_s = s;
+      }
+      wgmma_wait<0>();
+      fence_acc<kN / 2>(acc);
+      if (wg_leader) mbar_arrive(&empty_bar[team][prev_s]);
+    }
+
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      fr.row[rr] = static_cast<long long>(m0) + fr.loc[rr];
+      fr.ok[rr] = fr.row[rr] < p.M;
+    }
+    // box b of the tile stays in the team's staging buffer b until the tail GEMM has read it, so the team's previous
+    // stores must have drained both buffers before this tile writes them
+    if (issuer) tma_store_wait_read<0>();
+    named_bar_sync(team_bar, 256);
+#pragma unroll
+    for (int c0 = 0; c0 < kN; c0 += 64) {
+      uint8_t* buf = team_staging + (c0 / 64) * kStageBufBytes;
+      epilogue_box<kBf16, kN>(p.ep, acc, c0, 64, s_bias, fr, 0, buf, lane);
+      fence_proxy_async_smem();
+      named_bar_sync(team_bar, 256);
+      if (issuer) {
+        if (p.ch.store_first && c0 < p.ep.Cout) tma_store_2d(&tmap_out, buf, c0, m0);
+        tma_store_commit();
+      }
+    }
+    {
+      // every box of the tile is in shared memory and visible to the async proxy (fence + barrier above)
+      const uint32_t a2_hi = desc_hi(128, 8 * 128);
+      const uint32_t w2_hi = desc_hi(p.ch.w2_row_bytes, 8 * p.ch.w2_row_bytes);
+      const uint32_t stag_lo = smem_lo16(team_staging) + ((64 * half * 128) >> 4);
+      const uint32_t w2_lo0 = smem_lo16(w2_res);
+      const uint32_t w2_step16 = p.ch.w2_sub_bytes >> 4;
+      wgmma_fence();
+      // one or two 64-channel boxes feed the tail (conv_team_plan); each branch issues a fixed count of K steps
+      if (p.ch.own_chunks == 2) {
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            wgmma_mma<kBf16, kN2>(acc, desc_lohi(stag_lo + j * (kStageBufBytes >> 4) + 2 * k, a2_hi),
+                                  desc_lohi(w2_lo0 + j * w2_step16 + 2 * k, w2_hi), (j | k) != 0);
+      } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_mma<kBf16, kN2>(acc, desc_lohi(stag_lo + 2 * k, a2_hi), desc_lohi(w2_lo0 + 2 * k, w2_hi), k != 0);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_acc<kN2 / 2>(acc);
+    }
+    // the tail's box reuses staging buffer 0: the operand boxes are dead (both warpgroups' tail GEMMs have completed),
+    // but the stores of the first output may still be reading them
+    if (issuer) tma_store_wait_read<0>();
+    named_bar_sync(team_bar, 256);
+    EpilogueParams ep2 = p.ch.ep2;
+    ep2.residual = nullptr;   // never set for a tail (chain_setup); known here, the epilogue drops its row addresses
+#pragma unroll
+    for (int c0 = 0; c0 < kN2; c0 += 64) {
+      uint8_t* buf = team_staging + ((c0 / 64) & 1) * kStageBufBytes;
+      epilogue_box<kBf16, kN2>(ep2, acc, c0, 64, s_bias2, fr, 0, buf, lane);
+      fence_proxy_async_smem();
+      if (issuer) tma_store_wait_read<0>();   // box k + 1 overwrites the buffer of box k - 1
+      named_bar_sync(team_bar, 256);
+      if (issuer) {
+        if (c0 < p.ch.ep2.Cout) tma_store_2d(&tmap_out2, buf, c0, m0);
+        tma_store_commit();
+      }
+    }
+  }
+  if (issuer) tma_store_wait_all<0>();
+}
+
+using ConvKernelFn =void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
                               const CUtensorMap, const CUtensorMap, const ConvKernelParams);
 
 // One kernel per (dtype, N tile, fused decode, chained tail N, CTAs per SM, consumer warpgroups): the MMA width and the
@@ -496,6 +725,8 @@ using ConvKernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtens
 // instructions are in flight.  conv_configure admits exactly these shapes.
 template <bool kBf16>
 ConvKernelFn select_conv_kernel_t(const ConvKernelParams& kp) {
+  if (kp.groups == 4)   // two consumer teams (conv_team_plan): N = 128 with a 64-column tail
+    return kp.block_n == 128 && kp.ch.n2 == 64 ? conv_wgmma_team_kernel<kBf16, 128, 64> : nullptr;
   if (kp.groups == 1) {
     // one consumer warpgroup, two CTAs per SM, at the one-CTA instances' 232 consumer registers: the 256-column layers,
     // as two 128-column N tiles (conv_plan).  No N = 256 instance: ptxas allocates against the 128 registers of
@@ -542,6 +773,7 @@ ConvKernelFn select_conv_kernel(const ConvKernelParams& kp) {
 }  // namespace
 
 static int conv_plan(const yb_op_desc& d, int ctas, int groups, ConvKernelParams& kp, dim3& grid, size_t& smem_bytes);
+static void conv_team_plan(ConvKernelParams& kp, size_t& smem_bytes);
 
 // Validation of an fp16 / bf16 convolution descriptor, shared with the halo-patch kernel (pure host logic).
 int conv_validate(const yb_op_desc& d) {
@@ -576,16 +808,45 @@ static int conv_configure(const yb_op_desc& d, ConvKernelParams& kp, dim3& grid,
   YB_REQUIRE(!(d.reserved & YB_CONV_BAND_STEM),
              "conv: banded stem weights (reserved bit 1) need the halo-patch kernel, which this %dx%d map does not qualify for",
              d.H, d.W);
-  // Three layouts, tried in this order:
+  // Four layouts, tried in this order:
   //   two CTAs of two consumer warpgroups (104 registers) when the shape has such an instance;
   //   otherwise two CTAs of ONE consumer warpgroup (64-row tiles, 232 registers) when the shape has that instance;
+  //   otherwise one CTA of two consumer teams of two warpgroups when the one-CTA plan qualifies (conv_team_plan);
   //   one CTA of two consumer warpgroups.
   // Each two-CTA plan must fit half of the SM's shared memory and have a tile for each of the 2 x SMs CTAs.
-  // YB_CONV_ONE_CTA keeps the last layout (tests compare the launches bit for bit).
+  // YB_CONV_ONE_CTA and YB_CONV_NO_TEAMS keep the last layout (tests compare the launches bit for bit), and so does
+  // YB_CONV_PAIR_N64, which names the two-warpgroup launch of every four-warpgroup one.
   if (!(d.reserved & YB_CONV_ONE_CTA) &&
       (conv_plan(d, 2, 2, kp, grid, smem_bytes) == YB_OK || conv_plan(d, 2, 1, kp, grid, smem_bytes) == YB_OK))
     return YB_OK;
-  return conv_plan(d, 1, 2, kp, grid, smem_bytes);
+  const int rc1 = conv_plan(d, 1, 2, kp, grid, smem_bytes);
+  if (rc1 == YB_OK && !(d.reserved & (YB_CONV_ONE_CTA | YB_CONV_NO_TEAMS | YB_CONV_PAIR_N64)))
+    conv_team_plan(kp, smem_bytes);
+  return rc1;
+}
+
+// Two consumer teams (conv_wgmma_team_kernel) for a one-CTA plan of a chained 1x1 / s1 launch (mode 0) with resident
+// weights in one N tile of 128 columns, whole 64-channel K chunks, a 64-column tail over one or two 64-channel boxes and
+// no fused decode -- the shapes the team instances compile -- when it has at least kTeamMinTilesPerSm tiles per SM and
+// the weights, the tail weights, each team's two staging boxes and a ring of at least two 16 KB A stages per team fit
+// in 227 KB less the kernel's static shared memory.  The tiling, the grid and the MMA sequence of every output element
+// stay those of the one-CTA plan; only the A ring changes (one k-iteration per stage, one ring per team).  The
+// threshold keeps every smaller launch on two warpgroups (DESIGN.md section 3).
+static void conv_team_plan(ConvKernelParams& kp, size_t& smem_bytes) {
+  if (!(kp.ctas == 1 && kp.groups == 2 && kp.mode == 0 && kp.ch.on && !kp.decode_on && kp.b_resident &&
+        kp.n_tiles == 1 && kp.block_n == 128 && kp.ch.n2 == 64 && kp.block_k == 64 && kp.kk_last == 4 &&
+        kp.ch.ksteps == 4 && kp.num_tiles >= kTeamMinTilesPerSm * num_sms()))
+    return;
+  const size_t fixed = kp.b_res_bytes + 2 * kStageBufs * static_cast<size_t>(stage_buf_bytes(2)) +
+                       static_cast<size_t>(kp.ch.w2_chunks) * kp.ch.w2_sub_bytes + 1024;
+  if (fixed >= kTeamSmemBudget) return;
+  int stages = static_cast<int>((kTeamSmemBudget - fixed) / (2 * static_cast<size_t>(kp.a_stage_bytes)));
+  if (stages < 2) return;
+  if (stages > kTeamMaxStages) stages = kTeamMaxStages;
+  kp.groups = 4;
+  kp.kpg = 1;
+  kp.stages = stages;
+  smem_bytes = fixed + 2 * static_cast<size_t>(stages) * kp.a_stage_bytes;
 }
 
 // Tiling, pipeline depth, shared-memory layout and launch shape for `ctas` CTAs per SM of `groups` consumer warpgroups
@@ -734,7 +995,7 @@ int im2col_conv_config(const yb_op_desc& d, yb_conv_info* info) {
     info->slots = kp.stages;
     info->ring = kp.kpg;
     info->store_cols = kp.store_cols;
-    info->store_bufs = kStageBufs;   // shared by the consumer warpgroups
+    info->store_bufs = kStageBufs;   // shared by the consumer warpgroups (of a team, with two teams)
     info->groups = kp.groups;
     info->resident_ctas = kp.ctas;
     info->chained = kp.ch.on;
@@ -767,7 +1028,8 @@ int im2col_conv_create(const yb_op_desc& d, ConvOp** out) {
   Im2colConvOp* op = new Im2colConvOp();
   ConvKernelParams& kp = op->kp;
   int rc = conv_configure(d, kp, op->grid, op->smem_bytes);
-  const uint32_t block_m = tile_rows(kp.groups);   // rows of the A, output and tail-output boxes
+  const bool teams = kp.groups == 4;
+  const uint32_t block_m = tile_rows(teams ? 2 : kp.groups);   // rows of the A, output and tail-output boxes
   const CUtensorMapDataType dt = kp.ep.is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   if (rc == YB_OK)
     rc = kp.mode == 0 ? tmap_matrix(&op->tmap_a, "conv input", dt, d.in, d.Cin, kp.M, d.in_cstride, kp.block_k, block_m,
@@ -803,8 +1065,21 @@ int im2col_conv_create(const yb_op_desc& d, ConvOp** out) {
   }
   if (rc == YB_OK) {
     op->fn = select_conv_kernel(kp);
-    rc = set_smem_attributes(reinterpret_cast<const void*>(op->fn), kSmemBudget, kp.ctas, op->smem_bytes,
-                             cta_threads(kp.groups), "conv");
+    rc = set_smem_attributes(reinterpret_cast<const void*>(op->fn), teams ? kTeamSmemBudget : kSmemBudget, kp.ctas,
+                             op->smem_bytes, cta_threads(kp.groups), "conv");
+    if (rc == YB_OK && teams) {   // the 640-thread CTA with up to 227 KB of shared memory must fit on an SM
+      int per_sm = 0;
+      const cudaError_t e =
+          cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, op->fn, cta_threads(kp.groups), op->smem_bytes);
+      if (e != cudaSuccess) {
+        set_error("conv: cudaOccupancyMaxActiveBlocksPerMultiprocessor failed: %s", cudaGetErrorString(e));
+        rc = YB_ERR_CUDA;
+      } else if (per_sm < 1) {
+        set_error("conv: the two-team CTA (%d threads, %zu bytes of shared memory) does not fit on an SM",
+                  cta_threads(kp.groups), op->smem_bytes);
+        rc = YB_ERR_INVALID;
+      }
+    }
   }
   if (rc != YB_OK) {
     delete op;
