@@ -249,11 +249,13 @@ typedef struct {
 #define YB_CONV_ONE_CTA 16       /* keep one CTA per SM where the shape would take two (tests compare the two launches
                                     bit for bit) */
 #define YB_CONV_NO_TAIL_SPLIT 64 /* 1x1 / im2col kernel: run the last round's tiles whole instead of splitting them over
-                                    the idle CTAs (tests compare the two launches bit for bit, A/B timing) */
+                                    the idle CTAs, and single tiles instead of two-tile tasks (tests compare the
+                                    launches bit for bit, A/B timing) */
 #define YB_CONV_PAIR_N64 128     /* halo-patch kernel: keep streamed-weight pair tasks at 64 columns on two consumer
                                     warpgroups instead of 128 columns on four; either kernel: keep two-team launches on
-                                    two consumer warpgroups: every launch on four runs on two (tests compare the two
-                                    launches bit for bit, A/B timing) */
+                                    two consumer warpgroups; 1x1 / im2col kernel: keep streamed-weight launches on single
+                                    tiles of two consumer warpgroups instead of two-tile tasks on four: every launch on
+                                    four runs on two (tests compare the two launches bit for bit, A/B timing) */
 #define YB_CONV_NO_TEAMS 256     /* halo-patch and 1x1 / im2col kernels: keep chained and banded-stem launches on two
                                     consumer warpgroups instead of two teams of two (tests compare the two launches bit
                                     for bit, A/B timing) */
@@ -278,7 +280,7 @@ typedef struct {
   int32_t block_n;           /* N-tile width (the wgmma N) */
   int32_t n_tiles;           /* N tiles */
   int32_t weights_resident;  /* the weights of the CTA's N tile stay in shared memory */
-  int32_t tiles_per_pass;    /* M tiles per weight pass (halo patch: 2 when pairs of tiles share each weight slab) */
+  int32_t tiles_per_pass;    /* M tiles per weight pass (2 when pairs of tiles share each weight slab) */
   int32_t slots;             /* pipeline stages (two teams of the 1x1 / im2col kernel: per team; halo patch: patch slots) */
   int32_t ring;              /* k-iterations per stage (halo patch: weight-ring slabs, 0 with resident weights) */
   int32_t store_cols;        /* store-box columns */
@@ -320,8 +322,13 @@ typedef struct {
  * resident weights over whole 64-channel K chunks, chained to a 64-column tail over one or two 64-channel boxes, runs
  * on two consumer teams too (groups = 4, layout 1x4, one k-iteration per stage and `slots` stages per team) when it
  * has at least 8 x SMs tiles and the weights, both teams' staging buffers and two stages per team fit in shared
- * memory; reserved bits YB_CONV_NO_TEAMS, YB_CONV_PAIR_N64 and YB_CONV_ONE_CTA keep two consumer warpgroups.  Pure
- * host logic. */
+ * memory; reserved bits YB_CONV_NO_TEAMS, YB_CONV_PAIR_N64 and YB_CONV_ONE_CTA keep two consumer warpgroups.  A
+ * one-CTA 1x1 / im2col convolution that streams its weights in 128-column N tiles over whole 64-channel K chunks,
+ * without a residual, chained tail or fused decode, runs as tasks of two 128-row M tiles sharing each weight slab on
+ * four consumer warpgroups (groups = 4, tiles_per_pass 2, layout 1x4x2 in _C.conv_config) when it has at least 100 M
+ * tiles and either at most one per SM, three or more N tiles or at least 400 M tiles, and the grid min(tasks, SMs) is
+ * a multiple of the N tiles; reserved bits YB_CONV_PAIR_N64, YB_CONV_ONE_CTA and YB_CONV_NO_TAIL_SPLIT keep the
+ * one-CTA plan.  Pure host logic. */
 int yb_conv_config(const yb_op_desc* op, yb_conv_info* info);
 
 typedef struct yb_plan yb_plan;

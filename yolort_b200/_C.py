@@ -645,10 +645,12 @@ def conv_config(op: "OpDesc") -> dict:
     # the halo-patch kernel reports its staging buffers, the others their consumer warpgroups (which share two buffers)
     cfg["store_bufs" if patch else "epilogue_groups"] = int(info.store_bufs if patch else info.groups)
     # CTAs per SM x consumer warpgroups: "1x2", "2x2" (the 104-register instances) or "2x1"; "ctas_per_sm" names the
-    # 104-register layout only
-    cfg["layout"] = f"{info.resident_ctas}x{info.groups}"
-    # consumer warpgroups per CTA: 2, 1 (the 2x1 layout) or 4 (halo patch: 128-column pair tasks; either kernel: two
-    # consumer teams of single-tile tasks, tiles_per_pass 1)
+    # 104-register layout only.  The 1x1 / im2col kernel's two-tile tasks on four warpgroups are "1x4x2" (x M tiles per
+    # task), apart from its two consumer teams of single-tile tasks ("1x4").
+    pairs = not patch and info.groups == 4 and info.tiles_per_pass == 2
+    cfg["layout"] = f"{info.resident_ctas}x{info.groups}" + ("x2" if pairs else "")
+    # consumer warpgroups per CTA: 2, 1 (the 2x1 layout) or 4 (halo patch: 128-column pair tasks; 1x1 / im2col kernel:
+    # two-tile tasks, tiles_per_pass 2; either kernel: two consumer teams of single-tile tasks, tiles_per_pass 1)
     cfg["consumer_groups"] = int(info.groups)
     cfg["ctas_per_sm"] = 2 if cfg["layout"] == "2x2" else 1
     if patch:

@@ -21,7 +21,8 @@
 // and one CTA's epilogue overlaps the other's MMAs.  The large chained 1x1 launches at N = 128, whose resident weights
 // leave room for one CTA per SM only, run on a lean 640-thread instance: two teams of two consumer warpgroups take the
 // CTA's tiles alternately, so one team's epilogue and chained tail overlap the other team's MMAs
-// (conv_wgmma_team_kernel).
+// (conv_wgmma_team_kernel).  The deep launches that stream their weights run on a 640-thread instance too: a task is two
+// 128-row tiles that share every weight slab, so each slab crosses from L2 once per two tiles (conv_wgmma_quad_kernel).
 // The kernel is a template over (dtype, activation family, fused decode, chained tail).  A chained tail
 // (conv_chain.cuh) is a second, pointwise GEMM over the tile the epilogue has just staged: the consumers multiply the
 // staged boxes with the resident tail weights and a second epilogue pass stores the result.
@@ -63,7 +64,8 @@ struct ConvKernelParams {
   // halves (kernel: 64-row or 64-column; split = 1: num_tasks = num_tiles, every task a whole tile)
   int full_tiles, split, num_tasks;
   int ctas;        // CTAs per SM the launch is planned for (1 or 2): selects the kernel instance
-  int groups;      // consumer warpgroups per CTA (2, or 1 with two CTAs per SM): selects the kernel instance
+  int groups;      // consumer warpgroups per CTA (2, 1 with two CTAs per SM, or 4): selects the kernel instance
+  int pair;        // M tiles per task: 1, or 2 when two tiles share each streamed weight slab (conv_quad_plan)
   int store_cols;  // columns per TMA store box: 64 / 32 / 16
   int bias_len;    // length of the (padded) bias vector
   int kk_last;     // K=16 steps of the LAST channel chunk (Cin need not fill it: TMA zero-fills, the MMA skips)
@@ -717,6 +719,188 @@ conv_wgmma_team_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   if (issuer) tma_store_wait_all<0>();
 }
 
+// ===================== four consumer warpgroups: two tiles per streamed weight slab =====================
+// The deep 1x1 and stride-2 im2col launches whose weights do not fit in shared memory stream a 16 KB weight slab from L2
+// for every k-iteration of every 128-row tile: as many bytes as their activations.  Here a task is two consecutive
+// 128-row M tiles (2q, 2q + 1) x one 128-column N tile, and a pipeline stage holds both tiles' A sub-tiles and ONE
+// weight slab, so the weight stream from L2 is halved.  Warpgroups 2t + 1 and 2t + 2 form team t, which owns tile t of
+// the task as the two consumer warpgroups of conv_wgmma_kernel own a tile: 64 rows each, m64n128k16, 64 accumulators
+// per thread.  All four read the slab; a stage is released (four arrivals) once the commit group after it completes.
+// Per team: a named barrier (2 + t), two 16 KB staging boxes and a TMA-store issuer, so both teams' epilogues run while
+// the producer fills the next task's stages.  Every output element gets the k16 MMA sequence and the epilogue of
+// conv_wgmma_kernel, so the outputs are the same bits.  Only what these launches need is compiled: modes 0 and 1, whole
+// 64-channel K chunks, streamed weights, 128 columns, one N tile per CTA (the grid is a multiple of the N tiles), no
+// residual, chained tail, fused decode or split tail (conv_quad_plan).
+constexpr size_t kQuadStaticSmem = 2 * kMaxStages * 8 + 128 * 4;   // barriers + bias vector (ptxas -v)
+constexpr size_t kQuadSmemBudget = 227 * 1024 - kQuadStaticSmem;
+constexpr int kQuadMinMTiles = 100;    // conv_quad_plan
+constexpr int kQuadWideMTiles = 400;
+
+template <bool kBf16>
+__global__ void __launch_bounds__(kTeamThreads, 1)
+conv_wgmma_quad_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                       const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap,
+                       const __grid_constant__ CUtensorMap, const __grid_constant__ CUtensorMap,
+                       const __grid_constant__ CUtensorMap, const ConvKernelParams p) {
+  constexpr int kN = 128;
+  constexpr int kStageBufBytes = stage_buf_bytes(2);
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t full_bar[kMaxStages];
+  __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
+  __shared__ __align__(16) float s_bias[kN];
+
+  uint8_t* tiles = reinterpret_cast<uint8_t*>(
+      (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  // stage = [A of tile 0][A of tile 1][B slab]
+  const uint32_t stage_bytes = 2 * p.a_stage_bytes + p.b_stage_bytes;
+  uint8_t* staging = tiles + static_cast<size_t>(p.stages) * stage_bytes;   // [2 teams][kStageBufs][kStageBufBytes]
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    tma_prefetch_desc(&tmap_out);
+    for (int s = 0; s < p.stages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 4);   // every consumer warpgroup reads every stage
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  // 128 x 24 + 512 x 112 <= 640 x 96: the producers lower their budget and return before the consumers raise theirs
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 24;\n" ::: "memory");
+    if (warp != 0) return;
+    // ===================== TMA producer: both tiles' A and one weight slab per k-iteration =====================
+    const uint32_t a_bytes = p.a_stage_bytes, b_bytes = p.block_n * p.block_k * 2;
+    const int m_tiles = p.num_tiles / p.n_tiles;
+    int kit = 0;
+    for (int t = blockIdx.x; t < p.num_tasks; t += gridDim.x) {
+      const int q = t / p.n_tiles;
+      const int n0 = (t - q * p.n_tiles) * p.block_n;
+      const int cnt = min(2, m_tiles - 2 * q);   // the odd last pair has one tile
+      for (int it = 0; it < p.num_k_iters; ++it, ++kit) {
+        const int s = kit % p.stages;
+        mbar_wait(&empty_bar[s], ((kit / p.stages) & 1) ^ 1);
+        uint8_t* a_dst = tiles + s * stage_bytes;
+        if (YB_ELECT()) {
+          mbar_expect_tx(&full_bar[s], cnt * a_bytes + b_bytes);
+          const int tap = it / p.chunks;
+          const int chunk = it - tap * p.chunks;
+          for (int j = 0; j < cnt; ++j) {
+            const int m0 = (2 * q + j) * 128;
+            if (p.mode == 0) {
+              tma_load_2d(&tmap_a, &full_bar[s], a_dst + j * a_bytes, chunk * p.block_k, m0);
+            } else {   // the tile's first output pixel, as conv_wgmma_kernel's producer derives it
+              const int cn = m0 / p.HoWo;
+              const int rem = m0 - cn * p.HoWo;
+              const int ho = rem / p.Wo;
+              const int wo = rem - ho * p.Wo;
+              const int r = tap / p.ksize;
+              const int sx = tap - r * p.ksize;
+              tma_load_im2col_4d(&tmap_a, &full_bar[s], a_dst + j * a_bytes, chunk * p.block_k, wo * p.stride - p.pad,
+                                 ho * p.stride - p.pad, cn, static_cast<uint16_t>(sx), static_cast<uint16_t>(r));
+            }
+          }
+          tma_load_2d(&tmap_b, &full_bar[s], a_dst + 2 * a_bytes, it * p.block_k, n0);
+        }
+      }
+    }
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 112;\n" ::: "memory");
+
+  // ===================== consumers: team `team`, warpgroup `half` of it multiplies rows 64 half .. +63 =====================
+  const int cw = (warp >> 2) - 1;
+  const int team = cw >> 1, half = cw & 1;
+  const int wq = warp & 3;
+  const int ctid = threadIdx.x - 128;
+  const bool issuer = (ctid & 255) == 0;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  const uint32_t team_bar = kTeamBar0 + team;
+  FragRows fr;
+  fr.loc[0] = half * 64 + wq * 16 + (lane >> 2);
+  fr.loc[1] = fr.loc[0] + 8;
+  uint8_t* team_staging = staging + static_cast<size_t>(team) * kStageBufs * kStageBufBytes;
+  EpilogueParams ep = p.ep;
+  ep.residual = nullptr;   // never set for these launches (conv_quad_plan); known here, the epilogue drops its row addresses
+  float acc[kN / 2];
+
+  // grid % n_tiles == 0 (conv_quad_plan): task % n_tiles, the N tile, is the same for every task of this CTA
+  const int n0 = (blockIdx.x % p.n_tiles) * kN;
+  for (int i = ctid; i < kN; i += 512) s_bias[i] = (n0 + i < p.bias_len) ? __ldg(p.bias + n0 + i) : 0.f;
+  named_bar_sync(kConsumerBar, 512);
+
+  const int m_tiles = p.num_tiles / p.n_tiles;
+  int kit = 0, store_idx = 0;
+  for (int t = blockIdx.x; t < p.num_tasks; t += gridDim.x) {
+    const int mt = 2 * (t / p.n_tiles) + team;
+    // Team 1 has no tile in the odd last pair.  It still issues its MMAs, on whatever its A slots hold, and discards the
+    // result: a branch around the MMAs would make ptxas serialise every wgmma of the kernel (C7520).  It waits for and
+    // releases every stage like the other warpgroups.
+    const bool active = mt < m_tiles;
+    const int m0 = mt * 128;
+    {
+      // descriptor constants, derived per task rather than held through the epilogue (registers are short)
+      const uint32_t ab_hi = desc_hi(128, 8 * 128);                              // 64-channel rows of 128 bytes
+      const uint32_t a_off16 = (p.a_stage_bytes * team + 64 * 128 * half) >> 4;   // this warpgroup's 64 rows
+      const uint32_t b_off16 = (2 * p.a_stage_bytes) >> 4;
+      const uint32_t tiles_lo = smem_lo16(tiles);
+      const uint32_t stage16 = stage_bytes >> 4;
+      // The first MMA overwrites the accumulators; zeroing them first tells ptxas that the previous task's values are
+      // dead, which it cannot see through the run-time accumulate flag.
+#pragma unroll
+      for (int i = 0; i < kN / 2; ++i) acc[i] = 0.f;
+      // ---- main loop: stage s is released once the MMAs that read it have completed (one stage in flight) ----
+      int prev_s = -1;
+      for (int it = 0; it < p.num_k_iters; ++it, ++kit) {
+        const int s = kit % p.stages;
+        mbar_wait(&full_bar[s], (kit / p.stages) & 1);
+        const uint32_t st_lo = tiles_lo + s * stage16;
+        wgmma_fence();
+        // whole 64-channel chunks (conv_quad_plan): four K steps, a fixed count (ptxas serialises the wgmmas of a
+        // run-time count, C7520)
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_mma<kBf16, kN>(acc, desc_lohi(st_lo + a_off16 + 2 * k, ab_hi), desc_lohi(st_lo + b_off16 + 2 * k, ab_hi),
+                               it != 0 || k != 0);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev_s >= 0 && wg_leader) mbar_arrive(&empty_bar[prev_s]);
+        prev_s = s;
+      }
+      wgmma_wait<0>();
+      fence_acc<kN / 2>(acc);
+      if (wg_leader) mbar_arrive(&empty_bar[prev_s]);
+    }
+
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      fr.row[rr] = static_cast<long long>(m0) + fr.loc[rr];
+      fr.ok[rr] = active && fr.row[rr] < p.M;
+    }
+    // the team's tile in two 64-column boxes through its two staging buffers: before the barrier the issuer waits until
+    // the previous store has read its buffer, which the next box overwrites
+#pragma unroll
+    for (int c0 = 0; c0 < kN; c0 += 64, ++store_idx) {
+      uint8_t* buf = team_staging + (store_idx & 1) * kStageBufBytes;
+      epilogue_box<kBf16, kN>(ep, acc, c0, 64, s_bias, fr, n0, buf, lane);
+      fence_proxy_async_smem();
+      if (issuer) tma_store_wait_read<0>();
+      named_bar_sync(team_bar, 256);
+      if (issuer) {
+        if (active && n0 + c0 < p.ep.Cout) tma_store_2d(&tmap_out, buf, n0 + c0, m0);
+        tma_store_commit();
+      }
+    }
+  }
+  if (issuer) tma_store_wait_all<0>();
+}
+
 using ConvKernelFn =void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
                               const CUtensorMap, const CUtensorMap, const ConvKernelParams);
 
@@ -725,6 +909,8 @@ using ConvKernelFn =void (*)(const CUtensorMap, const CUtensorMap, const CUtenso
 // instructions are in flight.  conv_configure admits exactly these shapes.
 template <bool kBf16>
 ConvKernelFn select_conv_kernel_t(const ConvKernelParams& kp) {
+  if (kp.groups == 4 && kp.pair == 2)   // two-tile tasks over one streamed weight slab (conv_quad_plan)
+    return kp.block_n == 128 && !kp.ch.on ? conv_wgmma_quad_kernel<kBf16> : nullptr;
   if (kp.groups == 4)   // two consumer teams (conv_team_plan): N = 128 with a 64-column tail
     return kp.block_n == 128 && kp.ch.n2 == 64 ? conv_wgmma_team_kernel<kBf16, 128, 64> : nullptr;
   if (kp.groups == 1) {
@@ -774,6 +960,7 @@ ConvKernelFn select_conv_kernel(const ConvKernelParams& kp) {
 
 static int conv_plan(const yb_op_desc& d, int ctas, int groups, ConvKernelParams& kp, dim3& grid, size_t& smem_bytes);
 static void conv_team_plan(ConvKernelParams& kp, size_t& smem_bytes);
+static void conv_quad_plan(ConvKernelParams& kp, dim3& grid, size_t& smem_bytes);
 
 // Validation of an fp16 / bf16 convolution descriptor, shared with the halo-patch kernel (pure host logic).
 int conv_validate(const yb_op_desc& d) {
@@ -808,20 +995,24 @@ static int conv_configure(const yb_op_desc& d, ConvKernelParams& kp, dim3& grid,
   YB_REQUIRE(!(d.reserved & YB_CONV_BAND_STEM),
              "conv: banded stem weights (reserved bit 1) need the halo-patch kernel, which this %dx%d map does not qualify for",
              d.H, d.W);
-  // Four layouts, tried in this order:
+  // Five layouts, tried in this order:
   //   two CTAs of two consumer warpgroups (104 registers) when the shape has such an instance;
   //   otherwise two CTAs of ONE consumer warpgroup (64-row tiles, 232 registers) when the shape has that instance;
   //   otherwise one CTA of two consumer teams of two warpgroups when the one-CTA plan qualifies (conv_team_plan);
+  //   otherwise one CTA of four consumer warpgroups on two-tile tasks when the one-CTA plan qualifies (conv_quad_plan);
   //   one CTA of two consumer warpgroups.
   // Each two-CTA plan must fit half of the SM's shared memory and have a tile for each of the 2 x SMs CTAs.
-  // YB_CONV_ONE_CTA and YB_CONV_NO_TEAMS keep the last layout (tests compare the launches bit for bit), and so does
-  // YB_CONV_PAIR_N64, which names the two-warpgroup launch of every four-warpgroup one.
+  // YB_CONV_ONE_CTA keeps the last layout (tests compare the launches bit for bit), and so does YB_CONV_PAIR_N64, which
+  // names the two-warpgroup launch of every four-warpgroup one.  YB_CONV_NO_TEAMS keeps it instead of two teams, and
+  // YB_CONV_NO_TAIL_SPLIT instead of two-tile tasks (its plan is the one-CTA plan of whole single tiles).
   if (!(d.reserved & YB_CONV_ONE_CTA) &&
       (conv_plan(d, 2, 2, kp, grid, smem_bytes) == YB_OK || conv_plan(d, 2, 1, kp, grid, smem_bytes) == YB_OK))
     return YB_OK;
   const int rc1 = conv_plan(d, 1, 2, kp, grid, smem_bytes);
   if (rc1 == YB_OK && !(d.reserved & (YB_CONV_ONE_CTA | YB_CONV_NO_TEAMS | YB_CONV_PAIR_N64)))
     conv_team_plan(kp, smem_bytes);
+  if (rc1 == YB_OK && !(d.reserved & (YB_CONV_ONE_CTA | YB_CONV_PAIR_N64 | YB_CONV_NO_TAIL_SPLIT)))
+    conv_quad_plan(kp, grid, smem_bytes);
   return rc1;
 }
 
@@ -849,6 +1040,43 @@ static void conv_team_plan(ConvKernelParams& kp, size_t& smem_bytes) {
   smem_bytes = fixed + 2 * static_cast<size_t>(stages) * kp.a_stage_bytes;
 }
 
+// Two-tile tasks on four consumer warpgroups (conv_wgmma_quad_kernel) for a one-CTA plan that streams its weights in
+// 128-column N tiles over whole 64-channel K chunks, without a residual, chained tail or fused decode -- the shapes the
+// quad instances compile.  The T = ceil(m_tiles / 2) x n_tiles pair tasks run on G = min(T, SMs) CTAs, G a multiple of
+// the N tiles (every CTA keeps one N tile).  These launches are bound by the L2 -> SM stream, which the shared weight
+// slab cuts by a quarter, so they win even where the wider tasks add a round of the grid (c2's ops 8 and 27, 3.03
+// rounds of pairs: DESIGN.md section 3).  The rule takes the sizes measured: at least kQuadMinMTiles M tiles, and
+// either at most one per SM, three or more N tiles, or at least kQuadWideMTiles M tiles; other sizes keep two
+// warpgroups (not measured).  The plan also needs two stages of two A sub-tiles and one weight slab next to both teams' staging boxes
+// in 227 KB less the kernel's static shared memory.  The tiling and the MMA sequence of every output element stay
+// those of the one-CTA plan; the task list, the grid and the pipeline change, and the split tail goes.
+static void conv_quad_plan(ConvKernelParams& kp, dim3& grid, size_t& smem_bytes) {
+  if (!(kp.ctas == 1 && kp.groups == 2 && !kp.b_resident && kp.block_n == 128 && !kp.ch.on && !kp.decode_on &&
+        kp.ep.residual == nullptr && kp.block_k == 64 && kp.kk_last == 4))
+    return;
+  const int sms = num_sms();
+  const int m_tiles = kp.num_tiles / kp.n_tiles;
+  const int T = (m_tiles + 1) / 2 * kp.n_tiles;
+  const int G = T < sms ? T : sms;
+  if (G % kp.n_tiles != 0 || m_tiles < kQuadMinMTiles ||
+      !(m_tiles <= sms || kp.n_tiles >= 3 || m_tiles >= kQuadWideMTiles))
+    return;
+  const uint32_t stage_bytes = 2 * kp.a_stage_bytes + kp.b_stage_bytes;
+  const size_t fixed = 2 * kStageBufs * static_cast<size_t>(stage_buf_bytes(2)) + 1024;
+  int stages = static_cast<int>((kQuadSmemBudget - fixed) / stage_bytes);
+  if (stages < 2) return;
+  if (stages > kMaxStages) stages = kMaxStages;
+  kp.groups = 4;
+  kp.pair = 2;
+  kp.kpg = 1;
+  kp.stages = stages;
+  kp.split = 1;
+  kp.full_tiles = kp.num_tiles;
+  kp.num_tasks = T;
+  grid = dim3(G, 1, 1);
+  smem_bytes = fixed + static_cast<size_t>(stages) * stage_bytes;
+}
+
 // Tiling, pipeline depth, shared-memory layout and launch shape for `ctas` CTAs per SM of `groups` consumer warpgroups
 // (conv_configure has validated the descriptor).  With ctas = 2 the plan gets half of the SM's shared memory, less the
 // per-CTA reservation and the kernel's static shared memory, and fails when it does not fit there, when the layout has
@@ -861,6 +1089,7 @@ static int conv_plan(const yb_op_desc& d, int ctas, int groups, ConvKernelParams
   kp = ConvKernelParams();
   kp.ctas = ctas;
   kp.groups = groups;
+  kp.pair = 1;
   kp.M = static_cast<int>(static_cast<long long>(d.N) * Ho * Wo);
   kp.ep.Cout = d.Cout;
   const int m_tiles = (kp.M + block_m - 1) / block_m;
@@ -991,7 +1220,7 @@ int im2col_conv_config(const yb_op_desc& d, yb_conv_info* info) {
     info->block_n = kp.block_n;
     info->n_tiles = kp.n_tiles;
     info->weights_resident = kp.b_resident;
-    info->tiles_per_pass = 1;
+    info->tiles_per_pass = kp.pair;
     info->slots = kp.stages;
     info->ring = kp.kpg;
     info->store_cols = kp.store_cols;
@@ -1028,7 +1257,7 @@ int im2col_conv_create(const yb_op_desc& d, ConvOp** out) {
   Im2colConvOp* op = new Im2colConvOp();
   ConvKernelParams& kp = op->kp;
   int rc = conv_configure(d, kp, op->grid, op->smem_bytes);
-  const bool teams = kp.groups == 4;
+  const bool teams = kp.groups == 4;   // two consumer teams, or two-tile tasks on four consumer warpgroups
   const uint32_t block_m = tile_rows(teams ? 2 : kp.groups);   // rows of the A, output and tail-output boxes
   const CUtensorMapDataType dt = kp.ep.is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   if (rc == YB_OK)
@@ -1065,8 +1294,9 @@ int im2col_conv_create(const yb_op_desc& d, ConvOp** out) {
   }
   if (rc == YB_OK) {
     op->fn = select_conv_kernel(kp);
-    rc = set_smem_attributes(reinterpret_cast<const void*>(op->fn), teams ? kTeamSmemBudget : kSmemBudget, kp.ctas,
-                             op->smem_bytes, cta_threads(kp.groups), "conv");
+    const size_t budget = kp.pair == 2 ? kQuadSmemBudget : (teams ? kTeamSmemBudget : kSmemBudget);
+    rc = set_smem_attributes(reinterpret_cast<const void*>(op->fn), budget, kp.ctas, op->smem_bytes,
+                             cta_threads(kp.groups), "conv");
     if (rc == YB_OK && teams) {   // the 640-thread CTA with up to 227 KB of shared memory must fit on an SM
       int per_sm = 0;
       const cudaError_t e =
@@ -1075,7 +1305,7 @@ int im2col_conv_create(const yb_op_desc& d, ConvOp** out) {
         set_error("conv: cudaOccupancyMaxActiveBlocksPerMultiprocessor failed: %s", cudaGetErrorString(e));
         rc = YB_ERR_CUDA;
       } else if (per_sm < 1) {
-        set_error("conv: the two-team CTA (%d threads, %zu bytes of shared memory) does not fit on an SM",
+        set_error("conv: the four-warpgroup CTA (%d threads, %zu bytes of shared memory) does not fit on an SM",
                   cta_threads(kp.groups), op->smem_bytes);
         rc = YB_ERR_INVALID;
       }
