@@ -7,11 +7,15 @@ on the GPU (`check_case`, used by tests/test_gpu_conv_cases.py and by run_conv /
 
 `check_case` compares a launch with an fp64 convolution of the same fp16/bf16-rounded operands, under a bound that
 scales with the operands' magnitude (see `tau`), and checks that nothing outside the destination view is written, that
-a second launch gives the same bits and that a two-CTA launch gives the bits of the one-CTA launch.
+a second launch gives the same bits and that a launch of any of the `VARIANTS` (two CTAs per SM, one consumer
+warpgroup, the split tail, four consumer warpgroups) gives the bits of each of its pinned launches.  The variants' own
+case tables (tests/conv_cases_*.py) use the same machinery.
 """
 import ctypes
 import dataclasses
-from typing import Callable, Optional
+import os
+import re
+from typing import Callable, NamedTuple, Optional
 
 import torch
 import torch.nn.functional as F
@@ -143,11 +147,102 @@ def fake_ptr(name: str) -> int:
 
 
 # ---- what the planner does with a case (yb_conv_config) ----------------------------------------------------------------
+def config(case: Case, extra: int = 0) -> dict:
+    """yb_conv_config of `case`, with reserved bits `extra` added (host logic, fake pointers)."""
+    d, _ch = build_desc(case, fake_ptr)
+    d.reserved |= extra
+    return _C.conv_config(d)
+
+
+def _kernel(cfg: dict) -> str:
+    """The kernel template a launch runs: the four-warpgroup layouts are kernels of their own."""
+    if cfg["patch_kernel"]:
+        if cfg["layout"] == "1x4":
+            return "conv3x3_patch_quad_kernel" if cfg["tiles_per_pass"] == 2 else "conv3x3_patch_team_kernel"
+        return "conv3x3_patch_kernel"
+    return {"1x4": "conv_wgmma_team_kernel", "1x4x2": "conv_wgmma_quad_kernel"}.get(cfg["layout"], "conv_wgmma_kernel")
+
+
 def instance_key(case: Case, d, cfg: dict) -> tuple:
-    """(kernel, dtype, N tile, fused decode, tail N, CTAs per SM): the template instance the launch runs."""
-    kernel = "patch" if cfg["patch_kernel"] else "conv"
-    return (kernel, "bf16" if case.dtype == BF16 else "f16", cfg["block_n"], bool(d.decode), cfg["tail_n"],
-            cfg["ctas_per_sm"])
+    """(kernel, dtype, N tile, fused decode, tail N, layout): the template instance the launch runs."""
+    return (_kernel(cfg), "bf16" if case.dtype == BF16 else "f16", cfg["block_n"], bool(d.decode), cfg["tail_n"],
+            cfg["layout"])
+
+
+def selector_instances() -> set:
+    """Every instance_key that select_conv_kernel_t (csrc/conv_sm90.cu) and select_patch_kernel_t
+    (csrc/conv3x3_patch_sm90.cu) can return, read from their source: a new instance fails tests/test_conv_coverage.py
+    until a case reaches it."""
+    csrc = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "yolort_b200", "csrc")
+    with open(os.path.join(csrc, "conv_sm90.cu")) as f:
+        conv = f.read()
+    with open(os.path.join(csrc, "conv3x3_patch_sm90.cu")) as f:
+        patch = f.read()
+    found = []     # (kernel, N, decode, tail N, layout)
+    for m in re.finditer(r"conv_wgmma_kernel<kBf16, (\d+), (true|false), (\d+), (\d)(?:, (\d))?>", conv):
+        found.append(("conv_wgmma_kernel", int(m[1]), m[2] == "true", int(m[3]), f"{m[4]}x{m[5] or 2}"))
+    for m in re.finditer(r"conv_wgmma_team_kernel<kBf16, (\d+), (\d+)>", conv):
+        found.append(("conv_wgmma_team_kernel", int(m[1]), False, int(m[2]), "1x4"))
+    for _ in re.finditer(r"conv_wgmma_quad_kernel<kBf16>", conv):
+        found.append(("conv_wgmma_quad_kernel", 128, False, 0, "1x4x2"))
+    for m in re.finditer(r"conv3x3_patch_kernel<kBf16, (\d+), (\d+), (\d)>", patch):
+        found.append(("conv3x3_patch_kernel", int(m[1]), False, int(m[2]), f"{m[3]}x2"))
+    for m in re.finditer(r"conv3x3_patch_team_kernel<kBf16, (\d+), (\d+)>", patch):
+        found.append(("conv3x3_patch_team_kernel", int(m[1]), False, int(m[2]), "1x4"))
+    for _ in re.finditer(r"conv3x3_patch_quad_kernel<kBf16>", patch):
+        found.append(("conv3x3_patch_quad_kernel", 128, False, 0, "1x4"))
+    return {(k, dt, *rest) for dt in ("f16", "bf16") for k, *rest in found}
+
+
+class Variant(NamedTuple):
+    takes: Callable[[dict], bool]   # on the launch's yb_conv_config
+    bits: tuple                     # reserved bits, each of which pins the plain one-CTA, two-warpgroup launch
+    pinned: dict                    # what yb_conv_config reports for each pinned launch
+    may_keep_arena: bool = False    # a model launch may rewrite the bytes already in the arena (the deep layers of an
+                                    # untrained model: yolov5l at 1280², pan.layer_blocks.4.m.1.cv2)
+
+
+# Every launch variant besides the plain one-CTA, two-warpgroup launch.  Each writes the bits of its pinned launches:
+# every output element gets the same k16 MMA sequence and epilogue either way.  YB_CONV_PAIR_N64 names the two-warpgroup
+# launch of every four-warpgroup one.
+VARIANTS = {
+    "2x2": Variant(lambda cfg: cfg["layout"] == "2x2", (_C.YB_CONV_ONE_CTA,), {"ctas_per_sm": 1, "grid": SMS}),
+    "2x1": Variant(lambda cfg: cfg["layout"] == "2x1", (_C.YB_CONV_ONE_CTA,), {"layout": "1x2"}),
+    "split tail": Variant(lambda cfg: cfg["tail_split"] > 1, (_C.YB_CONV_NO_TAIL_SPLIT,),
+                          {"tail_split": 1, "tail_tiles": 0}),
+    "patch quad": Variant(lambda cfg: _kernel(cfg) == "conv3x3_patch_quad_kernel", (_C.YB_CONV_PAIR_N64,),
+                          {"consumer_groups": 2, "block_n": 64, "tiles_per_pass": 2}, may_keep_arena=True),
+    "patch team": Variant(lambda cfg: _kernel(cfg) == "conv3x3_patch_team_kernel",
+                          (_C.YB_CONV_NO_TEAMS, _C.YB_CONV_PAIR_N64), {"consumer_groups": 2, "layout": "1x2"}),
+    "1x1 team": Variant(lambda cfg: _kernel(cfg) == "conv_wgmma_team_kernel",
+                        (_C.YB_CONV_NO_TEAMS, _C.YB_CONV_PAIR_N64), {"consumer_groups": 2, "layout": "1x2"}),
+    "1x1 quad": Variant(lambda cfg: _kernel(cfg) == "conv_wgmma_quad_kernel", (_C.YB_CONV_PAIR_N64,),
+                        {"consumer_groups": 2, "layout": "1x2", "tiles_per_pass": 1}, may_keep_arena=True),
+}
+
+
+# The tiling fields each pinning bit keeps: the pinned launch runs the same tiles on two consumer warpgroups.
+KEEPS = {
+    "2x2": ("chained",),
+    "patch team": ("block_n", "n_tiles", "weights_resident", "tiles_per_pass", "store_cols", "chained", "tail_n", "grid",
+                   "m_tiles", "work_items"),
+    "1x1 team": ("block_n", "n_tiles", "weights_resident", "tiles_per_pass", "store_cols", "chained", "tail_n", "grid",
+                 "m_tiles", "work_items", "tail_tiles", "tail_split"),
+    "1x1 quad": ("block_n", "n_tiles", "weights_resident", "store_cols", "m_tiles", "work_items"),
+}
+
+
+def variants(cfg: dict) -> list:
+    """Names of the VARIANTS a launch takes."""
+    return [v for v, var in VARIANTS.items() if var.takes(cfg)]
+
+
+def check_pinned(pinned: dict, cfg: dict, variant: str, bit: int, what) -> None:
+    """The launch of `cfg` pinned by `bit` reports what VARIANTS[variant] states, with the tiling KEEPS names."""
+    want = VARIANTS[variant].pinned
+    assert {k: pinned[k] for k in want} == want, (what, variant, bit, pinned)
+    for k in KEEPS.get(variant, ()):
+        assert pinned[k] == cfg[k], (what, variant, bit, k, pinned, cfg)
 
 
 def plan_paths(case: Case, cfg: dict) -> set:
@@ -273,12 +368,13 @@ def _cases():
 
 CASES = _cases()
 
-# Instances no case of this table reaches, with the reason and the test that covers them.
+# Instances no case of any table reaches, with the reason and the test that covers them.
 EXCLUDED = {
-    ("conv", "f16", 256, True, 0, 1): "fused decode needs a detection head and a candidate arena: "
-                                      "tests/test_gpu_network.py::test_fused_head_decode_equals_unfused",
-    ("conv", "bf16", 256, True, 0, 1): "fused decode needs a detection head and a candidate arena: "
-                                       "tests/test_gpu_network.py::test_fused_head_decode_equals_unfused",
+    **{("conv_wgmma_kernel", dt, 256, True, 0, "1x2"): "fused decode needs a detection head and a candidate arena: "
+       "tests/test_gpu_network.py::test_fused_head_decode_equals_unfused" for dt in ("f16", "bf16")},
+    **{("conv3x3_patch_team_kernel", dt, 128, False, 0, "1x4"): "the banded stem needs band weights "
+       "(engine.stem_band): tests/test_gpu_conv_variants.py::test_model_launches_match_pinned_launches[yolov5s]"
+       for dt in ("f16", "bf16")},
 }
 
 
@@ -391,7 +487,7 @@ def check_case(case: Case, device=torch.device("cuda:0"), legacy_tol=None) -> di
     d, _ch = build_desc(stored, fake_ptr)
     cfg = _C.conv_config(d)
     key = instance_key(c, d, cfg)
-    print(f"{c.name}: instance {key} grid {cfg['grid']} paths {sorted(plan_paths(c, cfg))}")
+    print(f"{c.name}: instance {key} grid {cfg['grid']} paths {sorted(plan_paths(c, cfg))} variants {variants(cfg)}")
     out, out2 = _launch(stored, t, device)
 
     # ---- nothing outside the destination view(s) changed ----
@@ -431,15 +527,19 @@ def check_case(case: Case, device=torch.device("cuda:0"), legacy_tol=None) -> di
     if c.chain is not None:
         assert torch.equal(again2, out2), "second launch of the tail differs"
 
-    # ---- two CTAs per SM: the bits of the one-CTA launch ----
-    if cfg["ctas_per_sm"] == 2:
-        one = dataclasses.replace(stored, reserved=stored.reserved | _C.YB_CONV_ONE_CTA)
-        d1, _c1 = build_desc(one, fake_ptr)
-        assert _C.conv_config(d1)["ctas_per_sm"] == 1
-        o1, o21 = _launch(one, t, device)
-        assert torch.equal(o1, out), "two-CTA launch differs from the one-CTA launch"
-        if c.chain is not None:
-            assert torch.equal(o21, out2), "two-CTA tail differs from the one-CTA launch"
+    # ---- every variant the launch takes: the bits of each of its pinned launches, first output and tail ----
+    for v in variants(cfg):
+        for bit in VARIANTS[v].bits:
+            pinned = dataclasses.replace(stored, reserved=stored.reserved | bit)
+            check_pinned(config(pinned), cfg, v, bit, c.name)
+            o1, o21 = _launch(pinned, t, device)
+            assert torch.equal(o1, out), f"{v} launch differs from its pinned launch (reserved bit {bit:#x})"
+            if c.chain is not None:
+                assert torch.equal(o21, out2), f"{v} tail differs from its pinned launch (reserved bit {bit:#x})"
+            if sf:       # the pinned launch of the case as given: the same tail, nothing of the first output written
+                o1, o21 = _launch(dataclasses.replace(c, reserved=c.reserved | bit), t, device)
+                assert torch.equal(o21, out2), f"{v}: store_first=0 pinned launch changes the tail ({bit:#x})"
+                assert torch.equal(o1, t["out0"]), f"{v}: store_first=0 pinned launch wrote the first output ({bit:#x})"
 
     # ---- store_first = 0: the same tail bits, and nothing of the first output written ----
     if sf:

@@ -12,11 +12,6 @@ from yolort_b200 import _C
 ROWS = 128                                                # rows of the one-CTA tile the threshold counts
 
 
-def one_group_key(case: Case, d, cfg: dict) -> tuple:
-    """(kernel, dtype, N tile, fused decode, tail N, layout): the template instance the launch runs."""
-    return ("conv", "bf16" if case.dtype == BF16 else "f16", cfg["block_n"], bool(d.decode), 0, cfg["layout"])
-
-
 def one_group_paths(case: Case, cfg: dict) -> set:
     """Named plan paths of the one-group layout (and of the rule that keeps a launch off it)."""
     p = set()

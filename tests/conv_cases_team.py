@@ -2,7 +2,7 @@
 stride-1 3x3 convolutions with resident weights in one N tile and classic single-tile tasks, chained after a 64-column
 N tile over whole 64-channel chunks, run on one CTA of two consumer teams of two warpgroups when the launch has at
 least 8 tasks per SM (yb_conv_config: `groups` 4, `tiles_per_pass` 1, `chained` 1).  The banded stem's team instance
-needs the stem's band weights; tests/test_gpu_conv_team.py covers it through the yolov5s plan.
+needs the stem's band weights; tests/test_gpu_conv_variants.py covers it through the yolov5s plan.
 
 The cases use the Case / build_desc / check_case machinery of tests/conv_cases.py and are sized from the device's SM
 count so that each lands on the side of the rule its name states ("team": two teams, "pair": two warpgroups).

@@ -1,15 +1,35 @@
-"""The case table of tests/conv_cases.py reaches every fp16/bf16 convolution kernel instance and every plan path (host
-logic, no GPU needed; SM-dependent sizes follow the device's SM count, 132 without a GPU).
+"""The case tables of the fp16/bf16 convolution kernels (tests/conv_cases.py and tests/conv_cases_*.py) reach every kernel
+instance and every plan path, and every launch variant keeps to its own table (host logic, no GPU needed; SM-dependent
+sizes follow the device's SM count, 132 without a GPU).
 
 The instance list comes from the kernel selectors' source, so a new instance fails this test until a case reaches it.
 """
-import os
-import re
-
-from conv_cases import CASES, EXCLUDED, SMS, build_desc, fake_ptr, instance_key, plan_paths
+import conv_cases
+import conv_cases_one_group
+import conv_cases_quad
+import conv_cases_quad_1x1
+import conv_cases_tail_split
+import conv_cases_team
+import conv_cases_team_1x1
+from conv_cases import EXCLUDED, SMS, VARIANTS, build_desc, check_pinned, config, fake_ptr, instance_key, plan_paths, \
+    selector_instances, variants
 from yolort_b200 import _C
 
-CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "yolort_b200", "csrc")
+TABLES = (conv_cases, conv_cases_one_group, conv_cases_quad, conv_cases_quad_1x1, conv_cases_tail_split, conv_cases_team,
+          conv_cases_team_1x1)
+
+# The tables whose cases may take each variant: a case of any other table that takes it has moved off the launch its
+# table is about.
+REACHED_BY = {
+    "2x2": {conv_cases},
+    "2x1": {conv_cases_one_group, conv_cases_tail_split},
+    "split tail": {conv_cases_one_group, conv_cases_quad_1x1, conv_cases_tail_split},
+    "patch quad": {conv_cases_quad},
+    "patch team": {conv_cases_team},
+    "1x1 team": {conv_cases_team_1x1},
+    "1x1 quad": {conv_cases_quad_1x1},
+}
+assert set(REACHED_BY) == set(VARIANTS)
 
 REQUIRED_PATHS = {
     # 1x1 / im2col kernel
@@ -28,38 +48,24 @@ REQUIRED_PATHS = {
 }
 
 
-def selector_instances() -> set:
-    """Every (kernel, dtype, N, decode, tail N, CTAs) that select_conv_kernel_t / select_patch_kernel_t can return."""
-    with open(os.path.join(CSRC, "conv_sm90.cu")) as f:
-        conv = f.read()
-    with open(os.path.join(CSRC, "conv3x3_patch_sm90.cu")) as f:
-        patch = f.read()
-    out = set()
-    for dt in ("f16", "bf16"):
-        for m in re.finditer(r"conv_wgmma_kernel<kBf16, (\d+), (true|false), (\d+), (\d+)>", conv):
-            out.add(("conv", dt, int(m[1]), m[2] == "true", int(m[3]), int(m[4])))
-        for m in re.finditer(r"conv3x3_patch_kernel<kBf16, (\d+), (\d+), (\d+)>", patch):
-            out.add(("patch", dt, int(m[1]), False, int(m[2]), int(m[3])))
-    return out
-
-
-def _plans():
-    for c in CASES:
-        d, _ch = build_desc(c, fake_ptr)
-        cfg = _C.conv_config(d)
-        yield c, instance_key(c, d, cfg), plan_paths(c, cfg)
+def _plans(tables=TABLES):
+    for table in tables:
+        for c in table.CASES:
+            d, _ch = build_desc(c, fake_ptr)
+            cfg = _C.conv_config(d)
+            yield table, c, instance_key(c, d, cfg), cfg
 
 
 def test_case_names_are_unique():
-    names = [c.name for c in CASES]
-    assert len(names) == len(set(names))
+    names = [c.name for _, c, _, _ in _plans()]
+    assert len(names) == len(set(names)), sorted(n for n in set(names) if names.count(n) > 1)
 
 
 def test_every_instance_is_reached():
     inst = selector_instances()
-    assert len(inst) >= 54, sorted(inst)      # the patterns still match the selectors (27 instances per dtype today)
+    assert len(inst) == 68, sorted(inst)      # the patterns still match the selectors (34 instances per dtype today)
     reached = {}
-    for c, key, _ in _plans():
+    for _, c, key, _ in _plans():
         reached.setdefault(key, []).append(c.name)
     unknown = set(reached) - inst
     assert not unknown, f"cases planned onto instances the selectors do not list: {sorted(unknown)}"
@@ -74,17 +80,35 @@ def test_every_instance_is_reached():
 
 def test_every_plan_path_is_reached():
     seen = {}
-    for c, _, paths in _plans():
-        for p in paths:
+    for _, c, _, cfg in _plans([conv_cases]):
+        for p in plan_paths(c, cfg):
             seen.setdefault(p, c.name)
     for p in sorted(REQUIRED_PATHS):
         print(f"  {p}: {seen.get(p, 'MISSING')}")
     assert REQUIRED_PATHS <= set(seen), sorted(REQUIRED_PATHS - set(seen))
 
 
+def test_variants_stay_in_their_tables():
+    """Every variant is taken by a case of each table listed for it, and by no case of another table."""
+    takers = {}
+    for table, c, _, cfg in _plans():
+        for v in variants(cfg):
+            assert table in REACHED_BY[v], (v, table.__name__, c.name)
+            takers.setdefault(v, set()).add(table)
+    assert takers == REACHED_BY, {v: sorted(t.__name__ for t in ts) for v, ts in takers.items()}
+
+
+def test_pinning_bits_give_the_reference_launch():
+    """Each bit of a variant plans every case that takes it on the launch the variant names, with the same tiling."""
+    for _, c, _, cfg in _plans():
+        for v in variants(cfg):
+            for bit in VARIANTS[v].bits:
+                check_pinned(config(c, bit), cfg, v, bit, c.name)
+
+
 def test_two_cta_threshold_at_2x_sms_tiles():
     """The same 1x1 layer plans two CTAs per SM at exactly 2 x SMs tiles and one CTA at one tile fewer."""
-    by_name = {c.name: c for c in CASES}
+    by_name = {c.name: c for c in conv_cases.CASES}
     for dt in ("f16", "bf16"):
         for name, ctas, grid in ((f"{dt} 2cta 1x1 Cout32 at 2xSMs", 2, 2 * SMS), (f"{dt} 1cta 1x1 Cout32 at 2xSMs-1", 1, SMS)):
             c = by_name[name]

@@ -1,43 +1,17 @@
-"""The four-consumer-warpgroup instance of the halo-patch kernel: every instance is reached, the cases take the path
-their names state, the rule holds on both sides of its edges, the reserved bit keeps the 64-column pairs, and the
-c2-c5 layers that take it are the ones the rule names (host logic, no GPU needed; SM-dependent sizes follow the device's
-SM count, 132 without a GPU)."""
-import os
-import re
-
+"""The four-consumer-warpgroup instance of the halo-patch kernel: the cases take the path their names state and reach
+an odd last pair, the rule holds on both sides of its edges, and the c2-c5 layers that take it are the ones the rule
+names (host logic, no GPU needed; SM-dependent sizes follow the device's SM count, 132 without a GPU).  Instance
+coverage, the pinning bit and the other tables are checked in tests/test_conv_coverage.py."""
 import conv_cases
 import conv_cases_quad as q
-from conv_cases import BF16, F16, Case, build_desc, fake_ptr
-from yolort_b200 import _C
+from conv_cases import BF16, F16, VARIANTS, Case, config
 
-CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "yolort_b200", "csrc")
-
-
-def _plan(c, extra=0):
-    d, _ch = build_desc(c, fake_ptr)
-    d.reserved |= extra
-    return _C.conv_config(d)
-
-
-def quad_instances() -> set:
-    with open(os.path.join(CSRC, "conv3x3_patch_sm90.cu")) as f:
-        src = f.read()
-    return {dt for dt in ("f16", "bf16") for _ in re.finditer(r"return conv3x3_patch_quad_kernel<kBf16>;", src)}
-
-
-def _is_quad(cfg) -> bool:
-    return cfg["patch_kernel"] == 1 and cfg["consumer_groups"] == 4
-
-
-def test_case_names_are_unique():
-    names = [c.name for c in q.CASES]
-    assert len(names) == len(set(names))
-    assert not set(names) & {c.name for c in conv_cases.CASES}
+_is_quad = VARIANTS["patch quad"].takes
 
 
 def test_cases_take_the_path_their_name_states():
     for c in q.CASES:
-        cfg = _plan(c)
+        cfg = config(c)
         quad = c.name.split()[1] == "quad"
         assert cfg["patch_kernel"] and cfg["tiles_per_pass"] == 2 and not cfg["weights_resident"], (c.name, cfg)
         assert _is_quad(cfg) == quad, (c.name, cfg)
@@ -51,15 +25,8 @@ def test_cases_take_the_path_their_name_states():
 
 
 def test_every_instance_is_reached_and_the_odd_last_pair():
-    assert quad_instances() == {"f16", "bf16"}
-    reached = {("bf16" if c.dtype == BF16 else "f16", _plan(c)["m_tiles"] % 2) for c in q.CASES if _is_quad(_plan(c))}
+    reached = {("bf16" if c.dtype == BF16 else "f16", config(c)["m_tiles"] % 2) for c in q.CASES if _is_quad(config(c))}
     assert reached == {(dt, odd) for dt in ("f16", "bf16") for odd in (0, 1)}, sorted(reached)
-
-
-def test_reserved_bit_keeps_the_64_column_pairs():
-    for c in q.CASES:
-        cfg = _plan(c, _C.YB_CONV_PAIR_N64)
-        assert cfg["consumer_groups"] == 2 and cfg["block_n"] <= 64 and cfg["tiles_per_pass"] == 2, (c.name, cfg)
 
 
 def _tasks(cfg) -> int:
@@ -73,19 +40,12 @@ def test_rule_edges():
     for T in (G // 2 + 1, G - 1, G, G + 1, G + G // 2, G + G // 2 + 1, 2 * G, 2 * G + G // 2 + 1):
         for dt in (F16, BF16):
             c = Case("edge", 2 * T, 16, 8, 128, 128, k=3, dtype=dt)
-            cfg = _plan(c)
+            cfg = config(c)
             r = T % G
             want = T >= G and (r == 0 or r > G // 2)
             assert cfg["tiles_per_pass"] == 2
             assert _is_quad(cfg) == want, (T, cfg)
             assert _tasks(cfg) == (T if want else 2 * T), (T, cfg)
-
-
-def test_other_paths_stay():
-    """Chains, resident weights, stride 2 and the stem never take four warpgroups."""
-    for c in conv_cases.CASES:
-        cfg = _plan(c)
-        assert not _is_quad(cfg), (c.name, cfg)
 
 
 # The stride-1 3x3 convolutions with streamed weights of the bench configs (the Bottleneck cv2 of the C3 blocks at
@@ -107,6 +67,6 @@ def test_bench_layers():
         return   # the expectations are those of a 132-SM H100
     for cfgname, side, c, n, want in BENCH_LAYERS:
         for dt in (F16, BF16):
-            cfg = _plan(Case(cfgname, n, side, side, c, c, k=3, dtype=dt, residual=True))
+            cfg = config(Case(cfgname, n, side, side, c, c, k=3, dtype=dt, residual=True))
             assert cfg["patch_kernel"] and cfg["tiles_per_pass"] == 2, (cfgname, side, c, cfg)
             assert _is_quad(cfg) == want, (cfgname, side, c, cfg)
