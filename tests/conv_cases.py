@@ -371,7 +371,8 @@ CASES = _cases()
 # Instances no case of any table reaches, with the reason and the test that covers them.
 EXCLUDED = {
     **{("conv_wgmma_kernel", dt, 256, True, 0, "1x2"): "fused decode needs a detection head and a candidate arena: "
-       "tests/test_gpu_network.py::test_fused_head_decode_equals_unfused" for dt in ("f16", "bf16")},
+       "tests/test_gpu_postprocess_paths.py::test_fused_decode_case (tests/postprocess_cases.py FUSED_CASES)"
+       for dt in ("f16", "bf16")},
     **{("conv3x3_patch_team_kernel", dt, 128, False, 0, "1x4"): "the banded stem needs band weights "
        "(engine.stem_band): tests/test_gpu_conv_variants.py::test_model_launches_match_pinned_launches[yolov5s]"
        for dt in ("f16", "bf16")},

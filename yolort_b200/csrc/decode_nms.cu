@@ -198,6 +198,7 @@ constexpr int kRowMaxBytes = 512;    // longest row handled (A*K 16-bit logits p
 constexpr int kRowPitch = kRowMaxBytes + 16;   // shared-memory row pitch: 132 words -> lanes spread over 8 banks
 constexpr int kRowList = 512;        // block-local candidate list (entries beyond it fall back to global atomics)
 constexpr int kRowPairs = kRowPixels * YB_MAX_ANCHORS;   // per-warp list of (pixel, anchor) pairs that passed objectness
+constexpr int kRowMaxExtent = 1023;  // widest / tallest level: px and py take 10 bits each in the pair word (PairBits)
 
 // bit positions in the row kernel's (pixel, anchor) pair word: px | py << 10 | level << kLv | anchor << kAnchor | lane << kLane
 template <typename Params>
@@ -327,7 +328,7 @@ decode_rows_kernel(const __grid_constant__ Params p, Workspace ws, int blocks_pe
     if (a >= p.n_anchors) break;
     const bool pass = (pass_bits >> a) & 1u;
     const uint32_t bal = __ballot_sync(0xffffffffu, pass);
-    if (pass)   // px, py: 10 bits each (maps up to 1023 wide), level, anchor 2, source lane 5
+    if (pass)   // px, py: 10 bits each (levels up to kRowMaxExtent), level, anchor 2, source lane 5
       s_pairs[n_pairs + __popc(bal & lt_lanes)] =
           make_uint2(static_cast<uint32_t>(px) | static_cast<uint32_t>(py) << 10 | static_cast<uint32_t>(lv) << PairBits<Params>::kLv |
                          static_cast<uint32_t>(a) << PairBits<Params>::kAnchor | static_cast<uint32_t>(lane) << PairBits<Params>::kLane,
@@ -1214,8 +1215,8 @@ extern "C" int yb_decode_candidates(const yb_nms_params* p, const yb_head_level*
   dp.score_thresh = p->score_thresh;
   dp.cap_per_image = cap;
   // NHWC rows (the plan's head buffers): every level is [.., A*K logits of one pixel, pad] with 16-bit elements,
-  // a 16-byte aligned pitch of at most 512 bytes -> the coalesced row kernel; anything else (the reference's
-  // [N,A,H,W,K] layout, fp32 logits) -> one thread per anchor.
+  // a 16-byte aligned pitch of at most 512 bytes, levels at most kRowMaxExtent wide and tall -> the coalesced row
+  // kernel; anything else (the reference's [N,A,H,W,K] layout, fp32 logits) -> one thread per anchor.
   bool rows = (dtype == YB_F16 || dtype == YB_BF16) && p->n_anchors <= YB_MAX_ANCHORS;
   dp.pix_start[0] = 0;
   for (int l = 0; l < YB_MAX_LEVELS; ++l) {
@@ -1223,7 +1224,8 @@ extern "C" int yb_decode_candidates(const yb_nms_params* p, const yb_head_level*
     dp.pix_start[l + 1] = dp.pix_start[l] + (on ? levels[l].H * levels[l].W : 0);
     if (on) {
       const yb_head_level& L = levels[l];
-      rows = rows && L.stride_a == p->n_classes + 5 && L.stride_x % 8 == 0 && L.stride_x * 2 <= kRowMaxBytes &&
+      rows = rows && L.H <= kRowMaxExtent && L.W <= kRowMaxExtent && L.stride_a == p->n_classes + 5 &&
+             L.stride_x % 8 == 0 && L.stride_x * 2 <= kRowMaxBytes &&
              L.stride_x >= static_cast<long long>(p->n_anchors) * (p->n_classes + 5) && L.stride_y % 8 == 0 && L.stride_n % 8 == 0 &&
              (reinterpret_cast<uintptr_t>(L.logits) & 15) == 0;
     }
@@ -1357,8 +1359,8 @@ int fill_tta_params(const yb_nms_params* p, int n_passes, const yb_tta_pass* pas
       if (dtype < 0) dtype = L.dtype;
       YB_REQUIRE(L.dtype == dtype && (dtype == YB_F16 || dtype == YB_BF16),
                  "decode_nms_tta: every level must hold fp16 (or every level bf16) logits");
-      YB_REQUIRE(L.logits != nullptr && L.H > 0 && L.W > 0 && L.H <= 1023 && L.W <= 1023,
-                 "decode_nms_tta: pass %d level %d empty or wider than 1023", q, l);
+      YB_REQUIRE(L.logits != nullptr && L.H > 0 && L.W > 0 && L.H <= kRowMaxExtent && L.W <= kRowMaxExtent,
+                 "decode_nms_tta: pass %d level %d empty or wider than %d", q, l, kRowMaxExtent);
       // the row kernel's layout: NHWC rows of A*(nc+5) 16-bit logits, 16-byte aligned, at most 512 bytes
       YB_REQUIRE(L.stride_a == p->n_classes + 5 && L.stride_x % 8 == 0 && L.stride_x * 2 <= kRowMaxBytes &&
                      L.stride_x >= static_cast<long long>(p->n_anchors) * (p->n_classes + 5) && L.stride_y % 8 == 0 &&
