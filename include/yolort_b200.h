@@ -787,6 +787,14 @@ int yb_v5_resize_prepare(int n_jobs, yb_v5_resize_job* jobs, int64_t* total_bloc
 /* Resizes every job in one launch.  jobs_dev: the prepared jobs on the device.  No job may read another's dst. */
 int yb_v5_resize(int n_jobs, const yb_v5_resize_job* jobs_dev, int64_t total_blocks, void* stream);
 
+/* yb_v5_resize_area: load_image's cv2.resize(INTER_AREA) (augment=False, the validation loader) of uint8 [H, W, 3]
+ * images whose output is no larger than the source on either axis, OpenCV 4.x's 8-bit arithmetic.  Integer factors
+ * (both scales within DBL_EPSILON of an integer): 2 x 2 is (sum + 2) >> 2, any other ix x iy
+ * cvRound(float(sum) * (1.f / (ix * iy))).  Otherwise computeResizeAreaTab's taps (in double, each weight rounded once
+ * to float) and ResizeArea_Invoker's float accumulation order.  Same jobs as yb_v5_resize; a launch of its own. */
+int yb_v5_resize_area_prepare(int n_jobs, yb_v5_resize_job* jobs, int64_t* total_blocks);
+int yb_v5_resize_area(int n_jobs, const yb_v5_resize_job* jobs_dev, int64_t total_blocks, void* stream);
+
 /* yb_v5_compose: one training sample per descriptor.  The warp reads a virtual canvas: up to YB_V5_MAX_PLACES
  * rectangles, each a view of a (resized) image placed at an offset, and the value 114 everywhere else; the canvas
  * itself is never written.  An output pixel maps back through the flips, then through each canvas's warp (or reads
@@ -826,6 +834,26 @@ int yb_v5_compose_prepare(int n_samples, const yb_v5_sample* samples, int64_t* b
 /* Computes every sample in one launch.  samples_dev: the descriptors on the device.  No host synchronisation; a
  * repeated call writes the same bits. */
 int yb_v5_compose(int n_samples, const yb_v5_sample* samples_dev, int64_t blocks_per_sample, void* stream);
+
+/* YOLOv5's validation rescale (val.py v6.0): predictions and labels of one rect batch back to each image's native
+ * pixels, in torch's CPU float32 arithmetic (on CUDA tensors torch multiplies by the float reciprocal of gain
+ * instead, which can differ by one unit in the last place).  A box goes through scale_coords(..., ratio_pad) and clip_coords: x - pad_w, y - pad_h, each
+ * divided by gain with correct rounding, then x clamped to [0, w0] and y to [0, h0] (NaN kept, as torch.clamp keeps it).  A target row (image, cls, x, y, w, h)
+ * normalised is first multiplied by (canvas_w, canvas_h) and turned into xyxy (xywh2xyxy, w / 2 as w * 0.5); it is
+ * written to targets_out, and one whose image index is not an integer in [0, n) is only converted.  One launch, no
+ * host synchronisation. */
+typedef struct {
+  float* boxes;                /* [n, D, 4] xyxy, in place; slots d >= counts[i] are not touched              */
+  const int32_t* counts;       /* [n]                                                                         */
+  const float* targets;        /* [T, 6] (image, cls, x, y, w, h) normalised to the canvas                    */
+  float* targets_out;          /* [T, 6] (image, cls, x1, y1, x2, y2) native pixels; may be targets            */
+  const float* params;         /* [n, 5] per image: gain, pad_w, pad_h, h0, w0                                */
+  int32_t n, D;
+  int64_t T;
+  float canvas_w, canvas_h;
+} yb_v5_rescale;
+
+int yb_v5_rescale_coords(const yb_v5_rescale* r, void* stream);
 
 /* YOLOv5's AutoAnchor (yolort/v5/utils/autoanchor.py; yolort_b200/v5/utils/autoanchor.py draws every random number on
  * the host): csrc/autoanchor.cu, restated in oracle/restate_autoanchor.py.  Labels are float32 (w, h) pairs. */

@@ -78,8 +78,11 @@ EXPORTED_SYMBOLS = (
     "yb_v5_mixup",
     "yb_v5_resize_prepare",
     "yb_v5_resize",
+    "yb_v5_resize_area_prepare",
+    "yb_v5_resize_area",
     "yb_v5_compose_prepare",
     "yb_v5_compose",
+    "yb_v5_rescale_coords",
     "yb_conv_wgrad_workspace_bytes",
     "yb_conv_wgrad_config",
     "yb_conv_wgrad",
@@ -316,7 +319,7 @@ YB_V5_MAX_PLACES = 4
 
 
 class V5ResizeJob(ctypes.Structure):
-    """yb_v5_resize_job: one cv2.resize(INTER_LINEAR) of load_image (include/yolort_b200.h)."""
+    """yb_v5_resize_job: one cv2.resize(INTER_LINEAR or INTER_AREA) of load_image (include/yolort_b200.h)."""
     _fields_ = [
         ("src", ctypes.c_void_p), ("dst", ctypes.c_void_p),
         ("src_stride_y", ctypes.c_int64), ("src_stride_x", ctypes.c_int64), ("src_stride_c", ctypes.c_int64),
@@ -351,6 +354,15 @@ class V5Sample(ctypes.Structure):
         ("out_h", ctypes.c_int32), ("out_w", ctypes.c_int32), ("ops", ctypes.c_int32), ("n_canvases", ctypes.c_int32),
         ("mix_r", ctypes.c_double), ("mix_omr", ctypes.c_double), ("canvas", V5Canvas * 2),
         ("lut", (ctypes.c_uint8 * 256) * 3),
+    ]
+
+
+class V5Rescale(ctypes.Structure):
+    """yb_v5_rescale: val.py's scale_coords / clip_coords of one batch (include/yolort_b200.h)."""
+    _fields_ = [
+        ("boxes", ctypes.c_void_p), ("counts", ctypes.c_void_p), ("targets", ctypes.c_void_p),
+        ("targets_out", ctypes.c_void_p), ("params", ctypes.c_void_p), ("n", ctypes.c_int32), ("D", ctypes.c_int32),
+        ("T", ctypes.c_int64), ("canvas_w", ctypes.c_float), ("canvas_h", ctypes.c_float),
     ]
 
 
@@ -464,6 +476,9 @@ def lib() -> ctypes.CDLL:
                               ctypes.c_void_p]
     L.yb_v5_resize_prepare.argtypes = [ctypes.c_int, ctypes.POINTER(V5ResizeJob), ctypes.POINTER(ctypes.c_int64)]
     L.yb_v5_resize.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
+    L.yb_v5_resize_area_prepare.argtypes = [ctypes.c_int, ctypes.POINTER(V5ResizeJob), ctypes.POINTER(ctypes.c_int64)]
+    L.yb_v5_resize_area.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
+    L.yb_v5_rescale_coords.argtypes = [ctypes.POINTER(V5Rescale), ctypes.c_void_p]
     L.yb_v5_compose_prepare.argtypes = [ctypes.c_int, ctypes.POINTER(V5Sample), ctypes.POINTER(ctypes.c_int64)]
     L.yb_v5_compose.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
     L.yb_conv_wgrad_workspace_bytes.restype = ctypes.c_size_t
@@ -815,6 +830,19 @@ def decode_nms(head_outputs: List[torch.Tensor], layout: str, strides, anchors_p
         num_classes = int(t0.shape[4]) - 5 if layout == "nahwk" else None
         if num_classes is None:
             raise NativeLibraryError("decode_nms: num_classes is required for the nhwc layout")
+    boxes, scores, labels, counts, host = decode_nms_complete(head_outputs, layout, strides, anchors_px, num_classes,
+                                                              score_thresh, nms_thresh, detections_per_img, semantics,
+                                                              rescale)
+    n = counts.numel()
+    return [{"scores": scores[i, :host[i]], "labels": labels[i, :host[i]], "boxes": boxes[i, :host[i]]} for i in range(n)]
+
+
+def decode_nms_complete(head_outputs: List[torch.Tensor], layout: str, strides, anchors_px, num_classes: int,
+                        score_thresh: float, nms_thresh: float, detections_per_img: int, semantics: int = NMS_TV_AUTO,
+                        rescale: Optional[torch.Tensor] = None):
+    """decode_nms_padded that drops nothing: one device->host read of counts + status, and a rerun with a larger
+    arena while an image overflowed its candidate share.  Returns (boxes, scores, labels, counts, host), host the
+    counts followed by the status as a python list."""
     dev = head_outputs[0].device
     while True:
         boxes, scores, labels, counts, status = decode_nms_padded(
@@ -823,11 +851,10 @@ def decode_nms(head_outputs: List[torch.Tensor], layout: str, strides, anchors_p
         host = torch.cat([counts.to(torch.int64), status]).tolist()     # one D2H + one conversion for the whole batch
         n = counts.numel()
         if host[n + 1] == 0:
-            break
+            return boxes, scores, labels, counts, host
         arena = _arenas[dev]
         arena.cap_per_image = max(2 * arena.cap_per_image, int(host[n + 2]))
         arena.ws = None
-    return [{"scores": scores[i, :host[i]], "labels": labels[i, :host[i]], "boxes": boxes[i, :host[i]]} for i in range(n)]
 
 
 class FusedPost:
@@ -1348,16 +1375,38 @@ def _keep_alive(tensors: Sequence[torch.Tensor], device: torch.device) -> None:
             t.record_stream(stream)
 
 
-def v5_resize(jobs, tensors: Sequence[torch.Tensor], device: torch.device) -> None:
-    """Runs the load_image resize jobs `jobs` (V5ResizeJob array, pointers set) in one launch; `tensors` are the
-    sources and destinations they point into.  Nothing synchronises."""
+def v5_resize(jobs, tensors: Sequence[torch.Tensor], device: torch.device, area: bool = False) -> None:
+    """Runs the load_image resize jobs `jobs` (V5ResizeJob array, pointers set) in one launch, INTER_LINEAR or, with
+    `area`, INTER_AREA (every job shrinking); `tensors` are the sources and destinations they point into.  Nothing
+    synchronises."""
     n = len(jobs)
     total = ctypes.c_int64(0)
-    check(lib().yb_v5_resize_prepare(n, jobs, ctypes.byref(total)), "yb_v5_resize_prepare")
+    L = lib()
+    prepare, run, what = ((L.yb_v5_resize_area_prepare, L.yb_v5_resize_area, "yb_v5_resize_area") if area else
+                          (L.yb_v5_resize_prepare, L.yb_v5_resize, "yb_v5_resize"))
+    check(prepare(n, jobs, ctypes.byref(total)), what + "_prepare")
     with device_guard(device):
         d_jobs = _descs_to_device(jobs, device)
-        check(lib().yb_v5_resize(n, d_jobs.data_ptr(), total.value, current_stream_ptr(device)), "yb_v5_resize")
+        check(run(n, d_jobs.data_ptr(), total.value, current_stream_ptr(device)), what)
         _keep_alive(tensors, device)
+
+
+def v5_rescale_coords(boxes: Optional[torch.Tensor], counts: Optional[torch.Tensor], targets: Optional[torch.Tensor],
+                      targets_out: Optional[torch.Tensor], params: torch.Tensor, canvas_hw=(0, 0)) -> None:
+    """yb_v5_rescale_coords: `boxes` [n, D, 4] float32 (slots below `counts` [n] int32) rescaled in place by the
+    per-image `params` [n, 5] (gain, pad_w, pad_h, h0, w0); `targets` [T, 6] normalised to the canvas_hw canvas into
+    `targets_out` as native xyxy.  Contiguous CUDA tensors of one device; one launch, nothing synchronises."""
+    r = V5Rescale()
+    dev = params.device
+    r.params = params.data_ptr()
+    r.n = int(params.shape[0])
+    if boxes is not None:
+        r.boxes, r.counts, r.D = boxes.data_ptr(), counts.data_ptr(), int(boxes.shape[1])
+    if targets is not None:
+        r.targets, r.targets_out, r.T = targets.data_ptr(), targets_out.data_ptr(), int(targets.shape[0])
+    r.canvas_h, r.canvas_w = float(canvas_hw[0]), float(canvas_hw[1])
+    with device_guard(dev):
+        check(lib().yb_v5_rescale_coords(ctypes.byref(r), current_stream_ptr(dev)), "yb_v5_rescale_coords")
 
 
 def v5_compose(samples, tensors: Sequence[torch.Tensor], device: torch.device) -> None:

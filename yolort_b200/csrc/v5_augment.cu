@@ -9,12 +9,17 @@
 //                       rectangles; four consecutive pixels per thread, 12-byte stores along contiguous rows
 //   v5_mixup_kernel     im * r + im2 * (1 - r) in IEEE double, truncated to uint8
 //   v5_resize_kernel    load_image's cv2.resize(INTER_LINEAR) of the mosaic loader, OpenCV's 8-bit fixed point
+//   v5_resize_area_kernel  load_image's cv2.resize(INTER_AREA) of the validation loader (augment=False)
 //   v5_compose_kernel   one launch for a batch of training samples: the warp of each sample reads a virtual canvas
 //                       (placed image views, 114 elsewhere), mixup, the colour steps and the flips, CHW stores
 //                       (the two mosaic-loader kernels are restated in oracle/restate_v5mosaic.py)
+//   v5_rescale_kernel   val.py's scale_coords / clip_coords of a batch's padded detections and its targets
+//                       (INTER_AREA and the rescale are restated in oracle/restate_v5val.py)
 //
 // Built with -fmad=false (Makefile) and written with _rn intrinsics: every product and sum is rounded on its own, as
 // OpenCV's x86 build rounds them; the two fused products of HSV2RGB are fmaf, as OpenCV's AVX2 build fuses them.
+#include <cfloat>
+
 #include "v5_augment.cuh"
 
 namespace yb {
@@ -156,6 +161,91 @@ __device__ __forceinline__ int find_job(const yb_v5_resize_job* jobs, int n, int
   return lo - 1;
 }
 
+// INTER_AREA's taps of output index d along an axis of ssz -> dsz (computeResizeAreaTab, in IEEE double as the host
+// computes them): a leading partial tap at s1 - 1, full taps s1 .. s2 - 1, a trailing partial tap at s2; each weight is
+// rounded once to float.
+struct AreaTaps {
+  int s1, s2;
+  bool lead, trail;
+  float a_lead, a_full, a_trail;
+};
+
+__device__ __forceinline__ AreaTaps area_taps(int d, int ssz, double scale) {
+  AreaTaps t;
+  const double f1 = __dmul_rn(double(d), scale);
+  const double f2 = __dadd_rn(f1, scale);
+  const double cell = fmin(scale, __dsub_rn(double(ssz), f1));
+  t.s2 = min(int(floor(f2)), ssz - 1);
+  t.s1 = min(int(ceil(f1)), t.s2);
+  const double lead = __dsub_rn(double(t.s1), f1), trail = __dsub_rn(f2, double(t.s2));
+  t.lead = lead > 1e-3;
+  t.trail = trail > 1e-3;
+  t.a_lead = __double2float_rn(__ddiv_rn(lead, cell));
+  t.a_full = __double2float_rn(__ddiv_rn(1.0, cell));
+  t.a_trail = __double2float_rn(__ddiv_rn(fmin(fmin(trail, 1.0), cell), cell));
+  return t;
+}
+
+__device__ __forceinline__ int area_tap(const AreaTaps& t, int k, float& a) {
+  // tap k of 0 .. count-1 in table order
+  if (t.lead) {
+    if (k == 0) {
+      a = t.a_lead;
+      return t.s1 - 1;
+    }
+    --k;
+  }
+  if (k < t.s2 - t.s1) {
+    a = t.a_full;
+    return t.s1 + k;
+  }
+  a = t.a_trail;
+  return t.s2;
+}
+
+__device__ __forceinline__ int area_count(const AreaTaps& t) { return int(t.lead) + (t.s2 - t.s1) + int(t.trail); }
+
+// cv::resize(INTER_AREA) of one 8-bit output pixel, both axes shrinking.  Integer factors (both scales within
+// DBL_EPSILON of an integer): 2 x 2 is (sum + 2) >> 2, any other ix x iy cvRound(float(sum) * (1.f / (ix * iy))).
+// Otherwise ResizeArea_Invoker's order: per source row tap, buf = sum over the column taps of float(S) * alpha, in tap
+// order; the output row's first row tap sets sum = beta * buf, each further one adds sum += beta * buf; cvRound(sum).
+__device__ __forceinline__ void area_pixel(const yb_v5_resize_job& j, int dy, int dx, uint8_t* o) {
+  const double scale_x = __drcp_rn(__ddiv_rn(double(j.dst_w), double(j.src_w)));
+  const double scale_y = __drcp_rn(__ddiv_rn(double(j.dst_h), double(j.src_h)));
+  const int ix = __double2int_rn(scale_x), iy = __double2int_rn(scale_y);
+  const int64_t sy_ = j.src_stride_y, sx_ = j.src_stride_x, sc_ = j.src_stride_c;
+  if (fabs(__dsub_rn(scale_x, double(ix))) < DBL_EPSILON && fabs(__dsub_rn(scale_y, double(iy))) < DBL_EPSILON) {
+    const uint8_t* s = j.src + int64_t(dy) * iy * sy_ + int64_t(dx) * ix * sx_;
+    const float inv = __fdiv_rn(1.0f, float(ix * iy));
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      int sum = 0;
+      for (int y = 0; y < iy; ++y)
+        for (int x = 0; x < ix; ++x) sum += int(__ldg(s + y * sy_ + x * sx_ + k * sc_));
+      o[k] = uint8_t(ix == 2 && iy == 2 ? (sum + 2) >> 2 : min(max(__float2int_rn(__fmul_rn(float(sum), inv)), 0), 255));
+    }
+    return;
+  }
+  const AreaTaps tx = area_taps(dx, j.src_w, scale_x), ty = area_taps(dy, j.src_h, scale_y);
+  const int nx = area_count(tx), ny = area_count(ty);
+  float sum[3] = {0.0f, 0.0f, 0.0f};
+  for (int r = 0; r < ny; ++r) {
+    float beta;
+    const uint8_t* row = j.src + int64_t(area_tap(ty, r, beta)) * sy_;
+    float buf[3] = {0.0f, 0.0f, 0.0f};
+    for (int c = 0; c < nx; ++c) {
+      float alpha;
+      const uint8_t* s = row + int64_t(area_tap(tx, c, alpha)) * sx_;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) buf[k] = __fadd_rn(buf[k], __fmul_rn(float(__ldg(s + k * sc_)), alpha));
+    }
+#pragma unroll
+    for (int k = 0; k < 3; ++k) sum[k] = r == 0 ? __fmul_rn(beta, buf[k]) : __fadd_rn(sum[k], __fmul_rn(beta, buf[k]));
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k) o[k] = uint8_t(min(max(__float2int_rn(sum[k]), 0), 255));
+}
+
 // One output pixel per thread.  INTER_LINEAR: the horizontal pass S = src[sx] * a0 + src[sx + 1] * a1 of rows sy and
 // sy + 1, then ((S0 >> 4) * b0 >> 16) + ((S1 >> 4) * b1 >> 16) + 2 >> 2 (VResizeLinear's 8-bit form, vector and
 // scalar alike).  An exact 2x downscale is INTER_AREA in OpenCV: (the 2 x 2 sum + 2) >> 2.
@@ -192,6 +282,16 @@ __global__ void __launch_bounds__(kThreads) v5_resize_kernel(const yb_v5_resize_
     const int v = ((((s0 >> 4) * b0) >> 16) + (((s1 >> 4) * b1) >> 16) + 2) >> 2;
     o[k] = uint8_t(min(max(v, 0), 255));
   }
+}
+
+// cv2.resize(INTER_AREA), one output pixel per thread.  A kernel of its own: its double tap arithmetic would raise
+// v5_resize_kernel's registers.
+__global__ void __launch_bounds__(kThreads) v5_resize_area_kernel(const yb_v5_resize_job* __restrict__ jobs, int n) {
+  const int b = int(blockIdx.x);
+  const yb_v5_resize_job& j = jobs[find_job(jobs, n, b)];
+  const int64_t p = int64_t(b - j.block_start) * kThreads + threadIdx.x;
+  if (p >= int64_t(j.dst_h) * j.dst_w) return;
+  area_pixel(j, int(p / j.dst_w), int(p % j.dst_w), j.dst + 3 * p);
 }
 
 // A tap of a virtual canvas: the placement holding it, or the border value 114.
@@ -291,6 +391,53 @@ __global__ void __launch_bounds__(kThreads) v5_compose_kernel(const yb_v5_sample
   }
 }
 
+// scale_coords(img1_shape, coords, img0_shape, ratio_pad) then clip_coords in torch's CPU float32 arithmetic: x - pad,
+// divided by gain with correct rounding (the python scalars rounded to float32), clamp to [0, w0] and [0, h0] with NaN
+// passed through as torch.clamp passes it.  On CUDA tensors torch multiplies by the float reciprocal of gain instead,
+// which can differ from this quotient by one unit in the last place.
+__device__ __forceinline__ float clamp_torch(float v, float hi) {
+  v = v < 0.0f ? 0.0f : v;
+  return v > hi ? hi : v;
+}
+
+__device__ __forceinline__ void rescale_box(const float* prm, float (&b)[4]) {
+  b[0] = clamp_torch(__fdiv_rn(__fsub_rn(b[0], prm[1]), prm[0]), prm[4]);
+  b[1] = clamp_torch(__fdiv_rn(__fsub_rn(b[1], prm[2]), prm[0]), prm[3]);
+  b[2] = clamp_torch(__fdiv_rn(__fsub_rn(b[2], prm[1]), prm[0]), prm[4]);
+  b[3] = clamp_torch(__fdiv_rn(__fsub_rn(b[3], prm[2]), prm[0]), prm[3]);
+}
+
+// Threads [0, n * D) take the detections (slot d < counts[i] only); threads [n * D, n * D + T) the targets, which go
+// first through val.py's targets[:, 2:] *= [W, H, W, H] and xywh2xyxy (w / 2 is w * 0.5 on the device).
+__global__ void __launch_bounds__(kThreads) v5_rescale_kernel(yb_v5_rescale r) {
+  const int64_t i = int64_t(blockIdx.x) * kThreads + threadIdx.x;
+  const int64_t nd = int64_t(r.n) * r.D;
+  if (i < nd) {
+    const int img = int(i / r.D);
+    if (int(i % r.D) >= r.counts[img]) return;
+    float4* p = reinterpret_cast<float4*>(r.boxes) + i;
+    const float4 v = *p;
+    float b[4] = {v.x, v.y, v.z, v.w};
+    rescale_box(r.params + 5 * img, b);
+    *p = make_float4(b[0], b[1], b[2], b[3]);
+    return;
+  }
+  const int64_t t = i - nd;
+  if (t >= r.T) return;
+  const float* s = r.targets + 6 * t;
+  float* o = r.targets_out + 6 * t;
+  const float fi = s[0];
+  o[0] = fi;
+  o[1] = s[1];
+  const float x = __fmul_rn(s[2], r.canvas_w), y = __fmul_rn(s[3], r.canvas_h);
+  const float hw = __fmul_rn(__fmul_rn(s[4], r.canvas_w), 0.5f), hh = __fmul_rn(__fmul_rn(s[5], r.canvas_h), 0.5f);
+  float b[4] = {__fsub_rn(x, hw), __fsub_rn(y, hh), __fadd_rn(x, hw), __fadd_rn(y, hh)};
+  const int img = int(fi);
+  if (fi == float(img) && img >= 0 && img < r.n) rescale_box(r.params + 5 * img, b);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) o[2 + k] = b[k];
+}
+
 int64_t blocks_for(int64_t pixels) { return (pixels + kBlockPix - 1) / kBlockPix; }
 
 }  // namespace
@@ -343,26 +490,48 @@ extern "C" int yb_v5_mixup(const uint8_t* a_dev, const uint8_t* b_dev, uint8_t* 
   return YB_OK;
 }
 
-extern "C" int yb_v5_resize_prepare(int n_jobs, yb_v5_resize_job* jobs, int64_t* total_blocks) {
-  YB_REQUIRE(n_jobs > 0 && jobs && total_blocks, "v5_resize_prepare: null argument or no jobs");
+namespace yb {
+namespace {
+int resize_prepare(const char* what, bool area, int n_jobs, yb_v5_resize_job* jobs, int64_t* total_blocks) {
+  YB_REQUIRE(n_jobs > 0 && jobs && total_blocks, "%s: null argument or no jobs", what);
   int64_t blocks = 0;
   for (int i = 0; i < n_jobs; ++i) {
     yb_v5_resize_job& j = jobs[i];
-    YB_REQUIRE(j.src && j.dst && j.src_h > 0 && j.src_w > 0 && j.dst_h > 0 && j.dst_w > 0,
-               "v5_resize_prepare: job %d has no pixels", i);
+    YB_REQUIRE(j.src && j.dst && j.src_h > 0 && j.src_w > 0 && j.dst_h > 0 && j.dst_w > 0, "%s: job %d has no pixels",
+               what, i);
     YB_REQUIRE(j.src_h < (1 << 24) && j.src_w < (1 << 24) && j.dst_h < (1 << 24) && j.dst_w < (1 << 24),
-               "v5_resize_prepare: job %d: beyond 2^24 a side", i);
+               "%s: job %d: beyond 2^24 a side", what, i);
+    YB_REQUIRE(!area || (j.dst_h <= j.src_h && j.dst_w <= j.src_w), "%s: job %d: %d x %d -> %d x %d does not shrink",
+               what, i, j.src_h, j.src_w, j.dst_h, j.dst_w);
     j.block_start = int32_t(blocks);
     blocks += (int64_t(j.dst_h) * j.dst_w + kThreads - 1) / kThreads;
-    YB_REQUIRE(blocks < (int64_t(1) << 31), "v5_resize_prepare: batch too large");
+    YB_REQUIRE(blocks < (int64_t(1) << 31), "%s: batch too large", what);
   }
   *total_blocks = blocks;
   return YB_OK;
+}
+}  // namespace
+}  // namespace yb
+
+extern "C" int yb_v5_resize_prepare(int n_jobs, yb_v5_resize_job* jobs, int64_t* total_blocks) {
+  return resize_prepare("v5_resize_prepare", false, n_jobs, jobs, total_blocks);
 }
 
 extern "C" int yb_v5_resize(int n_jobs, const yb_v5_resize_job* jobs_dev, int64_t total_blocks, void* stream_) {
   YB_REQUIRE(n_jobs > 0 && jobs_dev && total_blocks > 0, "v5_resize: null argument or no jobs");
   v5_resize_kernel<<<unsigned(total_blocks), kThreads, 0, static_cast<cudaStream_t>(stream_)>>>(jobs_dev, n_jobs);
+  YB_CHECK_CUDA(cudaGetLastError());
+  return YB_OK;
+}
+
+extern "C" int yb_v5_resize_area_prepare(int n_jobs, yb_v5_resize_job* jobs, int64_t* total_blocks) {
+  return resize_prepare("v5_resize_area_prepare", true, n_jobs, jobs, total_blocks);
+}
+
+extern "C" int yb_v5_resize_area(int n_jobs, const yb_v5_resize_job* jobs_dev, int64_t total_blocks, void* stream_) {
+  YB_REQUIRE(n_jobs > 0 && jobs_dev && total_blocks > 0, "v5_resize_area: null argument or no jobs");
+  v5_resize_area_kernel<<<unsigned(total_blocks), kThreads, 0, static_cast<cudaStream_t>(stream_)>>>(jobs_dev,
+                                                                                                    n_jobs);
   YB_CHECK_CUDA(cudaGetLastError());
   return YB_OK;
 }
@@ -400,6 +569,21 @@ extern "C" int yb_v5_compose(int n_samples, const yb_v5_sample* samples_dev, int
              "v5_compose: null argument or no samples");
   const dim3 grid{unsigned(blocks_per_sample), unsigned(n_samples), 1u};
   v5_compose_kernel<<<grid, kThreads, 0, static_cast<cudaStream_t>(stream_)>>>(samples_dev);
+  YB_CHECK_CUDA(cudaGetLastError());
+  return YB_OK;
+}
+
+extern "C" int yb_v5_rescale_coords(const yb_v5_rescale* r, void* stream_) {
+  YB_REQUIRE(r && r->n >= 0 && r->D >= 0 && r->T >= 0, "v5_rescale_coords: null argument or negative size");
+  const int64_t nd = int64_t(r->n) * r->D;
+  YB_REQUIRE(nd == 0 || (r->boxes && r->counts && (reinterpret_cast<uintptr_t>(r->boxes) & 15) == 0),
+             "v5_rescale_coords: boxes and counts are required (boxes 16-byte aligned)");
+  YB_REQUIRE(r->T == 0 || (r->targets && r->targets_out), "v5_rescale_coords: targets need an output");
+  YB_REQUIRE(r->params || (nd == 0 && r->T == 0), "v5_rescale_coords: no params");
+  const int64_t blocks = (nd + r->T + kThreads - 1) / kThreads;
+  if (blocks == 0) return YB_OK;
+  YB_REQUIRE(blocks < (int64_t(1) << 31), "v5_rescale_coords: too many boxes");
+  v5_rescale_kernel<<<unsigned(blocks), kThreads, 0, static_cast<cudaStream_t>(stream_)>>>(*r);
   YB_CHECK_CUDA(cudaGetLastError());
   return YB_OK;
 }

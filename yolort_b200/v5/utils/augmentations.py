@@ -26,7 +26,7 @@ from torch import Tensor
 from ... import _C
 
 __all__ = ["augment_hsv", "random_perspective", "box_candidates", "bbox_ioa", "mixup", "cutout", "apply_batch",
-           "HYP_SCRATCH"]
+           "letterbox", "HYP_SCRATCH"]
 
 # yolort/v5/data/hyps/hyp.scratch.yaml: the augmentation keys
 HYP_SCRATCH = {"hsv_h": 0.015, "hsv_s": 0.7, "hsv_v": 0.4, "degrees": 0.0, "translate": 0.1, "scale": 0.5,
@@ -369,3 +369,13 @@ def apply_batch(images: Sequence[Tensor], targets: Optional[Sequence[Optional[Di
         t["labels"] = torch.from_numpy(lab[:, 0].copy()).to(wh[2]).to(wh[1])
         out_targets.append(t)
     return outs, out_targets
+
+
+def letterbox(im, new_shape=(640, 640), color=(114, 114, 114), auto=True, scale_fill=False, scaleup=True, stride=32):
+    """letterbox (yolort/v5/utils/augmentations.py:99-137) of a CUDA uint8 [H, W, 3] image: resize with
+    cv2.resize(INTER_LINEAR) when the size changes, then a constant border of `color` with the reference's
+    int(round(d -/+ 0.1)) pads.  Returns (im [h, w, 3] uint8 in the image's channel order, ratio, (dw, dh)), with
+    ratio and (dw, dh) the reference's values."""
+    from .datasets import letterbox_image
+
+    return letterbox_image(im, new_shape, color, auto, scale_fill, scaleup, stride)

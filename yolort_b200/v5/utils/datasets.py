@@ -29,7 +29,8 @@ from torch import Tensor
 from ... import _C
 from . import augmentations as _aug
 
-__all__ = ["load_image", "load_mosaic", "train_batch", "xywhn2xyxy", "xyxy2xywhn", "HYP_SCRATCH"]
+__all__ = ["load_image", "load_mosaic", "train_batch", "rect_batches", "val_batch", "xywhn2xyxy", "xyxy2xywhn",
+           "HYP_SCRATCH"]
 
 # yolort/v5/data/hyps/hyp.scratch.yaml: the augmentation keys of augmentations.HYP_SCRATCH and the loader's own
 HYP_SCRATCH = dict(_aug.HYP_SCRATCH, mosaic=1.0, mixup=0.0, copy_paste=0.0)
@@ -105,6 +106,54 @@ def letterbox_geometry(h: int, w: int, s: int):
     return (new_unpad[1], new_unpad[0]), ratio, (dw, dh), (top, left), out
 
 
+def letterbox_arith(shape, new_shape=(640, 640), auto=True, scale_fill=False, scaleup=True, stride=32):
+    """letterbox's arithmetic (yolort/v5/utils/augmentations.py:99-137) for an image of shape (h, w), the reference's
+    expressions in its order: ((nh, nw), ratio, (dw, dh), (top, bottom, left, right))."""
+    if isinstance(new_shape, int):
+        new_shape = (new_shape, new_shape)
+    r = min(new_shape[0] / shape[0], new_shape[1] / shape[1])
+    if not scaleup:  # only scale down, do not scale up (for better val mAP)
+        r = min(r, 1.0)
+    ratio = r, r  # width, height ratios
+    new_unpad = int(round(shape[1] * r)), int(round(shape[0] * r))
+    dw, dh = new_shape[1] - new_unpad[0], new_shape[0] - new_unpad[1]  # wh padding
+    if auto:  # minimum rectangle
+        dw, dh = np.mod(dw, stride), np.mod(dh, stride)  # wh padding
+    elif scale_fill:  # stretch
+        dw, dh = 0.0, 0.0
+        new_unpad = (new_shape[1], new_shape[0])
+        ratio = new_shape[1] / shape[1], new_shape[0] / shape[0]  # width, height ratios
+    dw /= 2  # divide padding into 2 sides
+    dh /= 2
+    pads = int(round(dh - 0.1)), int(round(dh + 0.1)), int(round(dw - 0.1)), int(round(dw + 0.1))
+    return (new_unpad[1], new_unpad[0]), ratio, (dw, dh), pads
+
+
+def rect_batches(shapes, img_size: int = 640, batch_size: int = 32, stride: int = 32, pad: float = 0.5):
+    """The rect block of upstream v6.0's LoadImagesAndLabels.__init__ for images of `shapes` [(h, w)]: (irect, bi,
+    batch_shapes).  The images sorted by aspect ratio h / w (numpy's default argsort) are irect; sorted image j goes
+    to batch bi[j] = j // batch_size, whose canvas is batch_shapes[bi[j]] = (H, W), multiples of `stride` (the
+    model's largest: 64 for the P6 models)."""
+    s = np.array([(w, h) for h, w in shapes], dtype=np.float64)  # wh
+    n = len(s)
+    if n == 0:
+        raise ValueError("rect_batches: no images")
+    bi = np.floor(np.arange(n) / batch_size).astype(int)  # batch index
+    nb = bi[-1] + 1  # number of batches
+    ar = s[:, 1] / s[:, 0]  # aspect ratio
+    irect = ar.argsort()
+    ar = ar[irect]
+    batch_shapes = [[1, 1]] * nb
+    for i in range(nb):
+        ari = ar[bi == i]
+        mini, maxi = ari.min(), ari.max()
+        if maxi < 1:
+            batch_shapes[i] = [maxi, 1]
+        elif mini > 1:
+            batch_shapes[i] = [1, 1 / mini]
+    return irect, bi, np.ceil(np.array(batch_shapes) * img_size / stride + pad).astype(int) * stride
+
+
 class Canvas:
     """A virtual canvas: placements (key, y0, x0, y1, x1, oy, ox) -- canvas [y0, y1) x [x0, x1) reads the loaded
     image `key` at (y - oy, x - ox), 114 elsewhere -- and the inverse warp that reads it (inv None: no warp)."""
@@ -138,13 +187,37 @@ class Planner:
         self.shapes, self.labels, self.s, self.hyp = list(shapes), list(labels), int(img_size), hyp
         self.n = len(self.shapes)
         self.loads: Dict[object, tuple] = {}
+        self.area = set()           # loads resized with INTER_AREA (load_image with augment=False, r < 1)
 
-    def load(self, index: int) -> Tuple[int, int]:
+    def load(self, index: int, augment: bool = True) -> Tuple[int, int]:
         h0, w0 = self.shapes[index]
         hw = load_shape(h0, w0, self.s)
         if hw != (h0, w0):
             self.loads[index] = (None, hw)
+            if not augment and self.s < max(h0, w0):
+                self.area.add(index)
         return hw
+
+    def val_sample(self, index: int, shape: Tuple[int, int]):
+        """__getitem__'s augment=False branch into the batch canvas `shape` (H, W): load_image(augment=False), then
+        letterbox(auto=False, scaleup=False).  Returns (Sample, shapes)."""
+        h0, w0 = self.shapes[index]
+        h, w = self.load(index, augment=False)
+        (nh, nw), ratio, pad, (top, bottom, left, right) = letterbox_arith((h, w), shape, auto=False, scaleup=False)
+        key = index
+        if (nh, nw) != (h, w):
+            key = ("letterbox", index)
+            self.loads[key] = (index, (nh, nw))
+        cv = Canvas(nh + top + bottom, nw + left + right)
+        cv.places.append((key, top, left, top + nh, left + nw, top, left))
+        labels = self.labels[index].copy()
+        if labels.size:  # normalized xywh to pixel xyxy format
+            labels[:, 1:] = xywhn2xyxy(labels[:, 1:], ratio[0] * w, ratio[1] * h, padw=pad[0], padh=pad[1])
+        if len(labels):
+            labels[:, 1:5] = xyxy2xywhn(labels[:, 1:5], w=cv.w, h=cv.h, clip=True, eps=1E-3)
+        smp = Sample(cv.h, cv.w)
+        smp.canvases, smp.labels = [cv], labels
+        return smp, ((h0, w0), ((h / h0, w / w0), pad))
 
     def mosaic(self, index: int):
         """load_mosaic's draws: (canvas, labels4 xyxy)."""
@@ -270,7 +343,9 @@ def _run_loads(planner: Planner, images: Sequence[Tensor], dev) -> Dict[object, 
     total = sum(-(-n // 16) * 16 for n in sizes.values())
     buf = torch.empty((max(total, 1),), dtype=torch.uint8, device=dev) if planner.loads else None
     off = 0
-    for keys in levels:
+    # INTER_AREA loads take a launch of their own
+    levels = [[k for k in levels[0] if k not in planner.area], [k for k in levels[0] if k in planner.area], levels[1]]
+    for level, keys in enumerate(levels):
         if not keys:
             continue
         jobs = (_C.V5ResizeJob * len(keys))()
@@ -285,7 +360,7 @@ def _run_loads(planner: Planner, images: Sequence[Tensor], dev) -> Dict[object, 
             j.src_h, j.src_w, j.dst_h, j.dst_w = int(src.shape[0]), int(src.shape[1]), h, w
             loaded[k] = dst
             srcs += [src, dst]
-        _C.v5_resize(jobs, srcs, dev)
+        _C.v5_resize(jobs, srcs, dev, area=level == 1)
     return loaded
 
 
@@ -326,13 +401,14 @@ def _compose(samples: List[Sample], images, loaded, outs: Sequence[Tensor], stri
 
 
 # -- upstream's functions ------------------------------------------------------------------------------------------
-def load_image(im, img_size: int):
-    """load_image (v6.0, augment=True): `im` resized by r = img_size / max(h0, w0) with cv2.resize(INTER_LINEAR) to
-    (int(h0 * r), int(w0 * r)) when r != 1, else `im` itself; returns (im, (h0, w0), (h, w))."""
+def load_image(im, img_size: int, augment: bool = True):
+    """load_image (v6.0): `im` resized by r = img_size / max(h0, w0) to (int(h0 * r), int(w0 * r)) when r != 1, else
+    `im` itself; returns (im, (h0, w0), (h, w)).  The resize is cv2.resize(INTER_AREA) when r < 1 and not `augment`
+    (the validation loader's), else cv2.resize(INTER_LINEAR).  A side that resizes to 0 raises ValueError."""
     _aug._check_image(im, "load_image")
     h0, w0 = int(im.shape[0]), int(im.shape[1])
     planner = Planner([(h0, w0)], [None], img_size, HYP_SCRATCH)
-    h, w = planner.load(0)
+    h, w = planner.load(0, augment=bool(augment))
     if (h, w) == (h0, w0):
         return im, (h0, w0), (h, w)
     return _run_loads(planner, [im], im.device)[0], (h0, w0), (h, w)
@@ -395,3 +471,108 @@ def train_batch(images: Sequence[Tensor], labels, indices: Sequence[int], img_si
         rows.append(lab)
     targets = torch.from_numpy(np.concatenate(rows, 0)).to(dev)
     return imgs, targets
+
+
+class ValPlan:
+    """val_batch's host plan of one rect batch, and its two launches: `resize()` (the INTER_AREA shrinks, then the
+    INTER_LINEAR resizes) and `compose(imgs)` (every canvas, CHW RGB, into a contiguous uint8 [N, 3, H, W]).
+    `shapes` and `targets()` are collate_fn's; `targets()` copies from pinned memory without waiting for the device."""
+
+    def __init__(self, images: Sequence[Tensor], labels, indices: Sequence[int], batch_shape, img_size: int = 640,
+                 channel_order: str = "bgr"):
+        if channel_order not in ("bgr", "rgb"):
+            raise ValueError(f"channel_order must be 'bgr' or 'rgb', got {channel_order!r}")
+        self.images = list(images)
+        self.dev, labels = _check_inputs(self.images, list(labels), None, HYP_SCRATCH, "val_batch")
+        indices = [int(i) for i in indices]
+        if not indices:
+            raise ValueError("val_batch: no indices")
+        if any(i < 0 or i >= len(self.images) for i in indices):
+            raise IndexError(f"val_batch: an index outside 0..{len(self.images) - 1}")
+        H, W = (int(v) for v in batch_shape)
+        self.H, self.W = H, W
+        if H < 1 or W < 1:
+            raise ValueError(f"val_batch: batch_shape {tuple(batch_shape)}")
+        self.rgb = channel_order == "rgb"
+        self.planner = Planner([(int(im.shape[0]), int(im.shape[1])) for im in self.images], labels, img_size,
+                               HYP_SCRATCH)
+        self.samples, self.shapes = [], []
+        for i in indices:
+            smp, shp = self.planner.val_sample(i, (H, W))
+            if (smp.out_h, smp.out_w) != (H, W):
+                raise ValueError(f"val_batch: image {i} letterboxes to {smp.out_h}x{smp.out_w}, not the canvas {H}x{W}")
+            self.samples.append(smp)
+            self.shapes.append(shp)
+        self.loaded = None
+
+    def resize(self) -> None:
+        self.loaded = _run_loads(self.planner, self.images, self.dev)
+
+    def compose(self, imgs: Tensor) -> None:
+        n, H, W = len(self.samples), self.H, self.W
+        if tuple(imgs.shape) != (n, 3, H, W) or imgs.dtype != torch.uint8 or not imgs.is_contiguous():
+            raise ValueError(f"val_batch: the output must be a contiguous uint8 [{n}, 3, {H}, {W}] tensor")
+        plane = H * W
+        # channel k of the sample lands in plane k (RGB) or 2 - k (BGR)
+        outs = [imgs[k] if self.rgb else imgs[k, 2] for k in range(n)]
+        strides = [(W, 1, plane if self.rgb else -plane)] * n
+        _compose(self.samples, self.images, self.loaded, outs, strides, self.rgb, False, self.dev)
+
+    def targets(self) -> Tensor:
+        rows = []
+        for k, smp in enumerate(self.samples):
+            lab = np.zeros((len(smp.labels), 6), np.float32)
+            lab[:, 1:] = smp.labels
+            lab[:, 0] = k
+            rows.append(lab)
+        return torch.from_numpy(np.concatenate(rows, 0)).pin_memory().to(self.dev, non_blocking=True)
+
+
+def val_batch(images: Sequence[Tensor], labels, indices: Sequence[int], batch_shape, img_size: int = 640,
+              channel_order: str = "bgr"):
+    """`collate_fn([dataset[i] for i in indices])` [0], [1] and [3] of upstream v6.0's LoadImagesAndLabels(augment=False,
+    rect=True): per index load_image(augment=False) (cv2.resize INTER_AREA when it shrinks) and letterbox(auto=False,
+    scaleup=False) centred in the batch canvas `batch_shape` (H, W) (rect_batches' batch_shapes).  Returns
+    (imgs uint8 [N, 3, H, W] RGB, targets float32 [T, 6] (image, cls, x, y, w, h normalised to the canvas), shapes
+    [((h0, w0), ((h / h0, w / w0), (dw, dh)))]), the images and targets on the images' device; nothing waits for the
+    device.  `labels` are train_batch's; channel_order "rgb" takes RGB images (decode_jpeg's) as they are."""
+    plan = ValPlan(images, labels, indices, batch_shape, img_size, channel_order)
+    plan.resize()
+    imgs = torch.empty((len(plan.samples), 3, plan.H, plan.W), dtype=torch.uint8, device=plan.dev)
+    plan.compose(imgs)
+    return imgs, plan.targets(), plan.shapes
+
+
+def letterbox_image(im, new_shape=(640, 640), color=(114, 114, 114), auto=True, scale_fill=False, scaleup=True,
+                    stride=32):
+    """augmentations.letterbox: the resize (cv2 INTER_LINEAR, when the size changes) and the constant border, one
+    compose launch; HWC in the image's channel order."""
+    _aug._check_image(im, "letterbox")
+    color = tuple(int(c) for c in color)
+    if len(color) != 3 or any(c < 0 or c > 255 for c in color):
+        raise ValueError(f"letterbox: color must be three values in 0..255, got {color}")
+    h, w = int(im.shape[0]), int(im.shape[1])
+    (nh, nw), ratio, pad, (top, bottom, left, right) = letterbox_arith((h, w), new_shape, auto, scale_fill, scaleup,
+                                                                       stride)
+    if nh < 1 or nw < 1:
+        raise ValueError(f"letterbox: a {h}x{w} image resizes to {nh}x{nw}")
+    planner = Planner([(h, w)], [None], max(h, w), HYP_SCRATCH)
+    key = 0
+    if (nh, nw) != (h, w):
+        key = ("letterbox", 0)
+        planner.loads[key] = (0, (nh, nw))
+    oh, ow = nh + top + bottom, nw + left + right
+    out = torch.empty((oh, ow, 3), dtype=torch.uint8, device=im.device)
+    if color == (114, 114, 114):    # the compose kernel's border value: one launch writes the whole canvas
+        dst, smp = out, Sample(oh, ow)
+        cv = Canvas(oh, ow)
+        cv.places.append((key, top, left, top + nh, left + nw, top, left))
+    else:
+        out[...] = torch.tensor(color, dtype=torch.uint8).to(im.device)
+        dst, smp = out[top:top + nh, left:left + nw], Sample(nh, nw)
+        cv = Canvas(nh, nw)
+        cv.places.append((key, 0, 0, nh, nw, 0, 0))
+    smp.canvases = [cv]
+    loaded = _run_loads(planner, [im], im.device)
+    _compose([smp], [im], loaded, [dst], [tuple(int(v) for v in dst.stride())], False, False, im.device)
+    return out, ratio, pad
